@@ -1,8 +1,8 @@
 /*
- * b200ms.h -- C-ABI of libb200ms.so: the B200 (sm_100a) implementation of Morphik's ColPali
+ * b200ms.h -- C-ABI of libb200ms.so: the H100 (sm_90a) implementation of Morphik's ColPali
  * late-interaction (MaxSim) scoring path.  Plain pointers and sizes only; no C++/torch types.
  *
- * Drop-in boundary (reference paths relative to /root/reference):
+ * Drop-in boundary (reference paths relative to the morphik-core repository root):
  *   The reference has no FFI on this path; its scorers are reached through the Python plugin
  *   interface core/vector_store/base_vector_store.py:7-65 (BaseVectorStore).  The host mirror of that
  *   interface lives in morphik-core_b200/store.py and calls this library through ctypes
@@ -115,7 +115,7 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
 
 /* ---- the hot path ---------------------------------------------------------------------------- */
 /* group_scores[g, p] = sum over the (<=32) tokens of group g of max over the rows of page p of <q_t, d_r>
- *   BF16 / F8 corpus: float32 (fp32 accumulate on tcgen05);  I8: int32 exact;  B1: int32 sum_t max_r (128 - hamming).
+ *   BF16 / F8 corpus: float32 (fp32 accumulate on wgmma);  I8: int32 exact;  B1: int32 sum_t max_r (128 - hamming).
  * q_packed: device [roundup(n_groups,4)*32, 128] of the corpus dtype; q_lens/group_offsets (HOST) as produced by
  * b200ms_pack_queries (B1 needs the true token counts; may be NULL for BF16/I8).
  * group_scores: device [n_groups_padded, ld] with ld >= n_pages, n_groups_padded = roundup(n_groups,4).
@@ -271,12 +271,8 @@ int b200ms_score_times_ms(b200ms_t* h, float* out_ms, int n);
 /* Tuning knobs (0 keeps the default): rows per work unit, CTAs to launch. */
 int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas);
 /* Named options:
- *   "pair_cta"        CTA pairs with tcgen05 cta_group::2, M = N = 256: 0 = off, 1 = passes of >= 3 query tiles, 2 = also
- *                     exactly 2 tiles (default)
- *   "b1_tensor"       1 = score 1-bit corpora on tcgen05 with in-kernel bit expansion, 0 = POPC kernel, 2 = auto by group count
- *   "rowm"            1 (default) = full scans of <= 2 query groups (<= 64 query tokens; sign-bit corpora: 1 group) run on
- *                     maxsim_rowm_kernel: patch rows are the tcgen05 M operand, the query tokens N = 32 or 64, four lane-quadrant
- *                     epilogue warps in parallel; 0 = the query-as-M kernels (same results bit for bit)
+ *   "b1_tensor"       full scans of 1-bit corpora: 1 = wgmma kernel with in-kernel bit expansion, 0 = POPC kernel, 2 (default)
+ *                     = POPC for one or two 32-token query groups, wgmma for three or more (same results bit for bit)
  *   "zero_pad_compat" N > 0: reproduce colpali_engine score_multi_vector's zero-padding quirk with batch size N (128 upstream,
  *                     processing_colpali.py:350-362): a page shorter than the longest page of its batch scores
  *                     sum_t max(max_r <q_t,d_r>, 0).  Rerank calls batch the candidates in first-stage order (exactly the
@@ -285,7 +281,7 @@ int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas);
  *   "zero_copy"       1 (default): host entry points move small calls (<= 256 query rows) through mapped pinned memory
  *   "host_graph"      1 (default): small unmasked host searches (pack -> score -> top-k) are captured into a CUDA graph on their
  *                     second use and replayed as one launch; 0 = three plain launches (same results)
- *   "fde_gemm"        1 (default): FDE scan on tcgen05 when fde_dim % 64 == 0, 0 = SIMT scan
+ *   "fde_gemm"        1 (default): FDE scan on wgmma when fde_dim % 64 == 0, 0 = SIMT scan
  *   "unit_rows", "max_ctas"   work-unit size (needs a new b200ms_set_corpus) and launch width. */
 int b200ms_set_option(b200ms_t* h, const char* name, int64_t value);
 

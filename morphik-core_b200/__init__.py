@@ -1,6 +1,6 @@
-"""morphik-core_b200 -- B200-native ColPali late-interaction (MaxSim) path for Morphik.
+"""morphik-core_b200 -- H100-native ColPali late-interaction (MaxSim) path for Morphik.
 
-Host side is Python (like the reference) calling hand-written sm_100a CUDA through the C-ABI in
+Host side is Python (like the reference) calling hand-written sm_90a CUDA through the C-ABI in
 include/b200ms.h (ctypes).  Modules:
   _native   ctypes binding of libb200ms.so (fails loudly when the library is missing; there is no CPU fallback)
   index     MaxSimIndex: device-resident packed corpus + search (torch only holds the tensors)

@@ -2,7 +2,7 @@
 
 The declarations mirror include/b200ms.h one to one (tests/test_cabi_symbols.py checks that every symbol the
 header declares is exported).  Importing this module never touches CUDA; creating a handle does and raises
-``NativeError`` when no B200 is present.  There is deliberately no fallback implementation.
+``NativeError`` when no H100 is present.  There is deliberately no fallback implementation.
 """
 from __future__ import annotations
 
@@ -27,13 +27,13 @@ class NativeError(RuntimeError):
 
 
 def _load() -> ctypes.CDLL:
-    override = os.environ.get("B200MS_LIB")  # developer A/B aid (tools/build_variants.py): an explicit variant of the library
+    override = os.environ.get("B200MS_LIB")  # developer A/B aid: an explicit variant of the library
     if override:
         return _declare(ctypes.CDLL(override))
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python __graft_entry__.py build` "
-            "(nvcc, sm_100a). morphik-core_b200 has no CPU fallback."
+            "(nvcc, sm_90a). morphik-core_b200 has no CPU fallback."
         )
     from . import build_native
 

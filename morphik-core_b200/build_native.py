@@ -1,7 +1,7 @@
-"""Build libb200ms.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libb200ms.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python morphik-core_b200/build_native.py [--force]
-The output morphik-core_b200/lib/libb200ms.so is git-ignored but travels to the GPU box with the snapshot.
+The output morphik-core_b200/lib/libb200ms.so (and the objects, build.log and source stamp beside it) is git-ignored.
 """
 import os
 import subprocess
@@ -11,10 +11,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libb200ms.so")
-SOURCES = ["api.cu", "maxsim_umma.cu", "maxsim_umma_pair.cu", "maxsim_rowm.cu", "maxsim_b1.cu", "maxsim_b1_umma.cu", "pack.cu", "topk.cu", "fde.cu", "comm.cu"]
-HEADERS = ["common.cuh", "ptx.cuh", "umma_tile.cuh", os.path.join("..", "..", "include", "b200ms.h")]
+SOURCES = ["api.cu", "maxsim_wgmma.cu", "maxsim_b1.cu", "pack.cu", "topk.cu", "fde.cu", "comm.cu"]
+HEADERS = ["common.cuh", "ptx.cuh", "mma_tile.cuh", os.path.join("..", "..", "include", "b200ms.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-Xptxas", "-v", "--expt-relaxed-constexpr",
 ]
 
@@ -81,7 +81,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         print("\n".join(log))
     if failed:
         raise RuntimeError("nvcc failed; see output above")
-    link = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-ldl"]
+    link = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-ldl"]
     subprocess.run(link, check=True)
     with open(STAMP, "w") as f:
         f.write(source_hash() + "\n")

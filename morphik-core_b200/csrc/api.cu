@@ -124,7 +124,7 @@ static EncodeTiledFn encode_fn(b200ms_t* h) {
   return fn;
 }
 
-// [n_rows, row_bytes] row-major view; box = one 128-byte K panel x box_rows rows, 128-byte swizzle (what the UMMA
+// [n_rows, row_bytes] row-major view; box = one 128-byte K panel x box_rows rows, 128-byte swizzle (what the wgmma
 // K-major SWIZZLE_128B descriptor expects).  Out-of-range rows read as zero.  row_bytes is 256 for bf16 rows and 128 for
 // the one-byte dtypes by default; the FDE matrix passes its own (fde_dim * 2).
 int make_tmap_rows(b200ms_t* h, CUtensorMap* out, const void* base, int dtype, int64_t n_rows, int box_rows, int64_t row_bytes) {
@@ -231,17 +231,14 @@ B200MS_API int b200ms_create(int device, b200ms_t** out) {
   DeviceGuard g(device);
   cudaDeviceProp prop;
   if (int e = check_cuda(nullptr, cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) return e;
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     return set_error(nullptr, B200MS_ECUDA, std::string("create: device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-                                                ", this library is built for sm_100a (B200) only");
+                                                ", this library is built for sm_90a (H100) only");
   }
   b200ms_t* h = new b200ms_t();
   h->device = device;
   h->num_sms = prop.multiProcessorCount;
   if (const char* e = getenv("B200MS_B1_TENSOR")) h->b1_tensor = atoi(e);
-  if (const char* e = getenv("B200MS_PAIR_CTA")) h->pair_cta = atoi(e);
-  if (const char* e = getenv("B200MS_ROWM")) h->rowm = atoi(e) != 0;
-  if (const char* e = getenv("B200MS_ROWM_FAST")) h->rowm_fast_path = atoi(e);
   if (const char* e = getenv("B200MS_ZERO_COPY")) h->zero_copy = atoi(e);
   if (const char* e = getenv("B200MS_UNIT_ROWS")) { if (atoll(e) > 0) h->unit_rows = atoll(e); }
   if (int e = check_cuda(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking), "cudaStreamCreate")) {
@@ -268,7 +265,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
     if (g2.exec) cudaGraphExecDestroy(g2.exec);
   DeviceBuf* bufs[] = {&h->chunk_page, &h->unit_start, &h->page_start, &h->page_len, &h->clamp_pages, &h->clamp_slots,
                        &h->meta, &h->meta_b, &h->q_raw, &h->q_packed, &h->scores, &h->mask, &h->mask_index, &h->out_all,
-                       &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->b1_q_i8, &h->b1_tok_const,
+                       &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->b1_q_i8, &h->b1_tok_const, &h->f8_q_f16,
                        &h->fde_simhash, &h->fde_ams_index, &h->fde_ams_sign, &h->fde_tmp, &h->fde_q_bf16, &h->fde_final_index,
                        &h->fde_final_sign};
   for (DeviceBuf* b : bufs)
@@ -320,16 +317,12 @@ B200MS_API int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas) {
 B200MS_API int b200ms_set_option(b200ms_t* h, const char* name, int64_t value) {
   if (!h || !name) return B200MS_EINVAL;
   const std::string n(name);
-  if (n == "pair_cta" && value >= 0 && value <= 2) {
-    h->pair_cta = int(value);
-  } else if (n == "b1_tensor" && value >= 0 && value <= 2) {
+  if (n == "b1_tensor" && value >= 0 && value <= 2) {
     h->b1_tensor = int(value);
   } else if (n == "zero_pad_compat" && value >= 0 && value <= (int64_t(1) << 30)) {
     h->zero_pad_batch = int(value);
   } else if (n == "zero_copy" && value >= 0 && value <= 1) {
     h->zero_copy = int(value);
-  } else if (n == "rowm" && value >= 0 && value <= 1) {
-    h->rowm = int(value);
   } else if (n == "fde_gemm" && value >= 0 && value <= 1) {
     h->fde_gemm = int(value);
   } else if (n == "host_graph" && value >= 0 && value <= 1) {
@@ -538,20 +531,18 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   const int n_groups_padded = (n_groups + 3) & ~3;
   if (c.dtype == B200MS_B1) {
     if (!goff || !ntok_dev || n_q <= 0) return set_error(h, B200MS_EINVAL, "score: B1 needs the per-group token counts");
-    // b1_tensor: 0 = POPC kernel, 1 = tcgen05 kernel, 2 (default) = measured crossover: one 32-token group is faster on the
-    // POPC pipe (1.59 vs 2.49 ms / 65536 pages), two or more groups on the tensor cores (a 128-token tile costs the same
-    // as one token there).  Rerank of a candidate list stays on the POPC kernel.
-    // A full scan of ONE group runs with the patch rows as the M operand and the expanded bits in TMEM (maxsim_rowm.cu).
-    const bool rowm_path = !cs.ids && h->rowm && h->b1_tensor != 0 && n_groups == 1;
-    const bool tensor_path = rowm_path || (!cs.ids && (h->b1_tensor == 1 || (h->b1_tensor == 2 && n_groups >= 2)));
+    // b1_tensor: 0 = POPC kernel, 1 = wgmma kernel (bits expanded to int8, maxsim_wgmma.cu), 2 (default) = by group count:
+    // the POPC pipe costs one pass per 32-token group, the wgmma kernel about the same for up to 4 groups.  Full scans of
+    // 65 536 pages x 1024 rows (tools/time_scan.py --b1-groups) on an NVIDIA H100 80GB HBM3 at a 700 W power limit: 1 group
+    // 1.65 ms POPC vs 3.80 ms wgmma, 2 groups 3.16 vs 3.81, 3 groups 4.85 vs 3.81, 8 groups 12.76 vs 4.75.  Rerank of a
+    // candidate list stays on the POPC kernel.
+    const bool tensor_path = !cs.ids && (h->b1_tensor == 1 || (h->b1_tensor == 2 && n_groups >= 3));
     if ((tensor_path && c.has_empty) || cs.per_query)
       if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(n_groups_padded) * size_t(ld) * 4, s), "score: memset")) return e;
     if (!h->capturing)
       if (int e = check_cuda(h, cudaEventRecord(h->ev0[slot], s), "score: event record")) return e;
-    if (rowm_path) {
-      if (int e = launch_score_rowm(h, q_packed, n_groups, ntok_dev, nullptr, group_scores, ld, s)) return e;
-    } else if (tensor_path) {
-      if (int e = launch_score_b1_umma(h, q_packed, ntok_dev, n_groups, group_scores, ld, s)) return e;
+    if (tensor_path) {
+      if (int e = launch_score_b1_wgmma(h, q_packed, ntok_dev, n_groups, group_scores, ld, s)) return e;
     } else if (cs.per_query) {
       for (int q = 0; q < n_q; ++q) {
         if (goff[q + 1] <= goff[q]) continue;
@@ -619,13 +610,10 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
       sub.n_units = int(int64_t(q_hi - q_lo) * cs.stride);
       if (sub.clamp_bits) sub.clamp_bits += s0 / 32;
       void* sc = static_cast<uint8_t*>(group_scores) + size_t(s0) * 4;
-      if (int e = launch_score_umma(h, &sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
+      if (int e = launch_score_wgmma(h, &sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
     }
-  } else if (!cs.ids && h->rowm && n_groups <= kRowmMaxGroups) {
-    // the lone query: patch rows as the M operand, four epilogue warps in parallel (maxsim_rowm.cu)
-    if (int e = launch_score_rowm(h, q_packed, n_groups, nullptr, plan.clamp_bits, group_scores, ld, s)) return e;
   } else {
-    if (int e = launch_score_umma(h, &plan, q_packed, n_groups, group_scores, ld, s)) return e;
+    if (int e = launch_score_wgmma(h, &plan, q_packed, n_groups, group_scores, ld, s)) return e;
   }
   if (!h->capturing) {
     if (int e = check_cuda(h, cudaEventRecord(h->ev1[slot], s), "score: event record")) return e;

@@ -16,7 +16,6 @@ constexpr int kDim = B200MS_DIM;
 constexpr int kGroup = B200MS_ROW_GROUP;  // 32 rows: padding granule of pages and queries ("chunk")
 constexpr int kTileN = 128;               // patch rows per MMA tile (4 chunks)
 constexpr int kTileM = 128;               // query rows per MMA tile (4 groups)
-constexpr int kRowmMaxGroups = 2;         // maxsim_rowm.cu (patch rows as the M operand): scans of <= 2 query groups
 
 struct DeviceBuf {  // grow-only device scratch
   void* p = nullptr;
@@ -86,15 +85,16 @@ struct b200ms {
   bms::PinnedBuf stage;         // host entry points: [metadata | query rows | results], mapped into the device address space
   bms::DeviceBuf topk_keys, topk_ids;  // first-level (per-slice) top-k candidates
   bms::DeviceBuf b1_q_i8, b1_tok_const;  // tensor-core 1-bit scorer: +-1 int8 query tiles and per-token constants
+  bms::DeviceBuf f8_q_f16;  // e4m3 corpora: the query rows widened to f16 (A operand of the f16 MMA)
   bms::DeviceBuf cand_pad;  // batched rerank: per-query candidate lists re-laid out with a 32-slot-aligned stride
   bms::DeviceBuf cand_start, cand_end, cand_mask;  // candidate (rerank) mode: per-slot chunk ranges, valid-slot bitmask
   bms::DeviceBuf fde_simhash, fde_ams_index, fde_ams_sign, fde_tmp;  // FDE configuration (device copies) + scratch
-  bms::DeviceBuf fde_q_bf16;                      // scan: query FDEs split into bf16 hi/lo rows (tcgen05 B operand)
+  bms::DeviceBuf fde_q_bf16;                      // scan: query FDEs split into bf16 hi/lo rows (wgmma B operand)
   bms::DeviceBuf fde_final_index, fde_final_sign; // optional final count-sketch projection (final_projection_dimension)
   int fde_dim = 0, fde_reps = 0, fde_ksim = 0, fde_proj = 0;
   int fde_inner_dim = 0;   // reps * 2^ksim * proj (before the optional final projection)
   int fde_fill_empty = 0;  // fill_empty_partitions (documents): empty partition <- projection of the nearest point
-  int fde_gemm = 1;        // 1: scan on tcgen05 (fde_scan_umma_kernel) when the shape allows, 0: SIMT scan
+  int fde_gemm = 1;        // 1: scan on wgmma (fde_scan_wgmma_kernel) when the shape allows, 0: SIMT scan
   float fde_scale = 1.f;
   int zero_copy = 1;       // host entry points: small calls read queries / write results through mapped pinned memory
   bms::Comm* comm = nullptr;
@@ -106,21 +106,12 @@ struct b200ms {
   int64_t launches = 0;
   int64_t unit_rows = 4096;
   int max_ctas = 0;
-  int b1_tensor = 2;  // 1-bit corpora: 0 = POPC kernel, 1 = tcgen05 kernel (bits expanded to {0,1} int8 in smem), 2 = auto
-  int pair_cta = 2;   // CTA-pair kernels (cta_group::2, maxsim_umma_pair.cu): 0 off, 1 for passes of >= 3 query tiles, 2 (default) also for 2 tiles
-  int pair_clusters = -1;  // co-resident CTA pairs the device reports for the pair kernel (-1: not queried yet)
+  int b1_tensor = 2;  // 1-bit full scans: 0 = POPC kernel, 1 = wgmma kernel (bits expanded to {0,1} int8 in smem), 2 = by group count
   int zero_pad_batch = 0;  // > 0: reproduce score_multi_vector's zero-padding quirk with this batch size (128 upstream)
-  CUtensorMap tmap_q;  // query tiles; re-encoded only when (pointer, dtype, rows) change
+  CUtensorMap tmap_q;  // query rows in 16-row boxes; re-encoded only when (pointer, dtype, rows) change
   const void* tmap_q_base = nullptr;
   int tmap_q_dtype = -1;
   int64_t tmap_q_rows = -1;
-  CUtensorMap tmap_qn;  // the same query rows as a 32*NG-row box (maxsim_rowm.cu: the query is the N operand)
-  const void* tmap_qn_base = nullptr;
-  int tmap_qn_dtype = -1;
-  int64_t tmap_qn_rows = -1;
-  int tmap_qn_box = 0;
-  int rowm_fast_path = 1;   // A/B knob (env B200MS_ROWM_FAST): epilogue fast path for 8-tile blocks inside one page (A/B: faster for every dtype)
-  int rowm = 1;  // option "rowm": full scans of <= kRowmMaxGroups query groups run on maxsim_rowm_kernel (0: query-as-M kernels)
   // CUDA graphs of the small zero-copy host search (pack -> score -> top-k): key -> executable graph
   struct HostGraph {
     uint64_t key = 0;
@@ -158,20 +149,15 @@ int search_core(b200ms_t* h, const void* q_src, int src_dtype, const int32_t* q_
                 const void* meta_in_place, const void* meta_host_block);
 
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
-int launch_score_umma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, int n_groups_real, void* group_scores,
-                      int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
-constexpr int B200MS_EUNSUPPORTED_PAIR = -100;  // internal: pair kernel cannot be scheduled on this device
-int launch_score_umma_pair(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, int nm, int m_tile_base,
-                           int n_groups_real, void* scores, int64_t ld, cudaStream_t s);
+int launch_score_wgmma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, int n_groups_real, void* group_scores,
+                       int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
 int launch_score_b1(b200ms_t* h, const int64_t* cand_ids, int64_t n_cand, const void* q_packed, int n_groups,
                     const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo, int g_hi);
 int launch_pad_cands(b200ms_t* h, const int64_t* src, int n_cand, int n_lists, int64_t stride, int64_t* dst, cudaStream_t s);
 int launch_clamp_slots(b200ms_t* h, const int64_t* cand_ids, int n_cand, int n_lists, int64_t list_stride, int batch,
                        uint32_t* clamp_bits, cudaStream_t s);
-int launch_score_b1_umma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
-                         void* group_scores, int64_t ld, cudaStream_t s);
-int launch_score_rowm(b200ms_t* h, const void* q_packed, int n_groups_real, const int32_t* ntok_dev, const uint32_t* clamp_bits,
-                      void* group_scores, int64_t ld, cudaStream_t s);
+int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
+                          void* group_scores, int64_t ld, cudaStream_t s);
 int launch_cand_units(b200ms_t* h, const int64_t* cand_ids, int n_cand, int32_t* unit_start, int32_t* unit_end,
                       uint32_t* slot_mask, cudaStream_t s);
 int launch_hamming_batch(b200ms_t* h, const void* q, const void* cand, int64_t n, uint32_t* out, cudaStream_t s);

@@ -18,8 +18,8 @@
 // oracle's loops (oracle/fde_oracle.c) in fp32.
 //
 // Scan: scores[q, p] = <q_fde[q], F[p]> * inv_norm[p].  HBM-bound (2 * fde_dim bytes per page, 20 KB in the reference
-// configuration) -- fde_scan_umma_kernel streams the matrix ONCE per batch of up to 128 queries through tcgen05
-// (pages = M, queries = N), fde_scan_kernel is the SIMT fallback for shapes the tensor path does not take.
+// configuration) -- fde_scan_wgmma_kernel streams the matrix ONCE per batch of up to 128 queries through wgmma
+// (pages = M, queries = N), fde_scan_kernel is the SIMT scan for shapes the tensor path does not take.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -238,61 +238,51 @@ fde_scan_kernel(const uint4* __restrict__ F, const float* __restrict__ inv_norm,
   }
 }
 
-// ------------------------------------------------------------------------------------------------ tcgen05 scan
-// D[128 pages x NQP] = F_tile[128 x fde_dim] * Qb[NQP x fde_dim]^T on the tensor cores, fp32 accumulation in TMEM.
-//   A (M side) = 128 consecutive FDE rows, streamed from HBM by TMA in K-blocks of 64 bf16 (16 KB, SWIZZLE_128B);
+// ------------------------------------------------------------------------------------------------ wgmma scan
+// D[128 pages x NQP] = F_tile[128 x fde_dim] * Qb[NQP x fde_dim]^T on the tensor cores, fp32 accumulation in registers.
+//   A (M side) = 128 consecutive FDE rows, streamed from HBM by TMA in K-blocks of 64 bf16 (16 KB, SWIZZLE_128B); consumer
+//                warpgroup e multiplies rows 64e .. 64e+63;
 //   B (N side) = the query FDEs as bf16 rows: row q = hi(q_fde[q]) and row H+q = lo = bf16(q_fde[q] - hi), so that
 //                D[:, q] + D[:, H+q] reproduces the fp32 query to ~2^-17 relative (the FDE corpus itself is bf16);
 //                re-read per K-block from L2 (NQP * 128 B beside the 16 KB of A; evict_last keeps it resident).
 // The matrix is read ONCE for up to 128 queries; one query costs the same HBM pass (it is the bandwidth that is paid for).
-// Persistent, one CTA per SM, 256 threads: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7
-// epilogue (thread = one page of the tile: adds the hi/lo halves, scales by 1/||F_p||, writes scores[q, p] -- for a fixed
-// q the 32 lanes of a warp write 32 consecutive pages, one coalesced 128-byte store).
+// Persistent, one CTA per SM, 384 threads: warp 0 TMA producer, warpgroups 1-2 wgmma m64n64k16 (NQP / 64 accumulators of
+// 32 registers) and epilogue (adds the hi/lo halves, scales by 1/||F_p||, writes scores[q, p]).
 // Algorithmic bytes per page: 2 * fde_dim (+ 4 * n_q of scores written).
-constexpr int kScanThreads = 256;
+constexpr int kScanThreads = 384;
 constexpr uint32_t kScanATile = 128 * 128;  // 128 rows x 64 bf16
 
+template <int NCH>  // NQP = 64 * NCH query columns, H = NQP / 2
 __global__ void __launch_bounds__(kScanThreads, 1)
-fde_scan_umma_kernel(const __grid_constant__ CUtensorMap tmap_f, const __grid_constant__ CUtensorMap tmap_q,
-                     const float* __restrict__ inv_norm, int64_t n_pages, int n_kblocks, int n_q, int q_base, int half_cols,
-                     float* __restrict__ scores, int64_t ld, int num_stages) {
-  const int nqp = 2 * half_cols;                        // MMA N: hi rows [0, H), lo rows [H, 2H)
-  const uint32_t b_bytes = uint32_t(nqp) * 128u;
-  const uint32_t stage_bytes = kScanATile + b_bytes;    // multiples of 1024 (nqp % 32 == 0)
+fde_scan_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_f, const __grid_constant__ CUtensorMap tmap_q,
+                      const float* __restrict__ inv_norm, int64_t n_pages, int n_kblocks, int n_q, int q_base,
+                      float* __restrict__ scores, int64_t ld, int num_stages) {
+  constexpr int kNqp = 64 * NCH;
+  constexpr int kHalf = kNqp / 2;
+  constexpr uint32_t kStageBytes = kScanATile + uint32_t(kNqp) * 128u;  // multiple of 1024
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(num_stages) * stage_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + size_t(num_stages) * kStageBytes);
   uint64_t* full = bars;         // [num_stages] TMA -> MMA
-  uint64_t* empty = bars + 16;   // [num_stages] MMA -> TMA
-  uint64_t* tfull = bars + 32;   // [2] MMA -> epilogue
-  uint64_t* tempty = bars + 34;  // [2] epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 40);
+  uint64_t* empty = bars + 16;   // [num_stages] MMA -> TMA (one arrival per consumer warp)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int64_t n_tiles = (n_pages + 127) / 128;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_f);
     prefetch_tmap(&tmap_q);
     for (int i = 0; i < num_stages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);
+      mbar_init(&empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc_512(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       const uint64_t pol_f = policy_evict_first();
       const uint64_t pol_q = policy_evict_last();
       int stage = 0;
@@ -300,8 +290,8 @@ fde_scan_umma_kernel(const __grid_constant__ CUtensorMap tmap_f, const __grid_co
       for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         for (int kb = 0; kb < n_kblocks; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], stage_bytes);
-          uint8_t* a = smem + size_t(stage) * stage_bytes;
+          mbar_expect_tx(&full[stage], kStageBytes);
+          uint8_t* a = smem + size_t(stage) * kStageBytes;
           tma_load_2d(&tmap_f, &full[stage], a, kb * 64, int32_t(tile * 128), pol_f);
           tma_load_2d(&tmap_q, &full[stage], a + kScanATile, kb * 64, 0, pol_q);
           if (++stage == num_stages) {
@@ -311,84 +301,55 @@ fde_scan_umma_kernel(const __grid_constant__ CUtensorMap tmap_f, const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = umma_idesc(0, 128, nqp);
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t t = 0;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t buf = t & 1;
-      mbar_wait(&tempty[buf], ((t >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * 256;
-      for (int kb = 0; kb < n_kblocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_addr = smem_u32(smem + size_t(stage) * stage_bytes);
-          const uint64_t ad = umma_desc_kmajor_sw128(a_addr);
-          const uint64_t bd = umma_desc_kmajor_sw128(a_addr + kScanATile);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) umma_ss<0>(d_tmem, ad + ks * 2, bd + ks * 2, idesc, (kb | ks) != 0);
-          umma_commit(&empty[stage]);
-          if (kb == n_kblocks - 1) umma_commit(&tfull[buf]);
-        }
-        __syncwarp();
-        if (++stage == num_stages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    const int quad = warp & 3;
-    const uint32_t lane_base = tmem_base + (uint32_t(quad * 32) << 16);
-    uint32_t t = 0;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t buf = t & 1;
-      const int64_t p = tile * 128 + quad * 32 + lane;
-      const float inv = p < n_pages ? __ldg(inv_norm + p) : 0.f;
-      mbar_wait(&tfull[buf], (t >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = lane_base + buf * 256;
-      if (half_cols == 16) {  // <= 16 queries: hi and lo halves sit in one 32-column load
-        uint32_t v[32];
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[buf]);
-        if (p < n_pages) {
-#pragma unroll
-          for (int q = 0; q < 16; ++q)
-            if (q < n_q) scores[int64_t(q_base + q) * ld + p] = (__uint_as_float(v[q]) + __uint_as_float(v[16 + q])) * inv;
-        }
-      } else {
-        for (int c = 0; c < half_cols; c += 32) {
-          uint32_t hi[32], lo[32];
-          tmem_ld_32x32(taddr + c, hi);
-          tmem_ld_32x32(taddr + half_cols + c, lo);
-          tmem_ld_wait();
-          if (c + 32 >= half_cols) {  // last chunk read: the accumulator may be overwritten
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[buf]);
-          }
-          if (p < n_pages) {
-#pragma unroll
-            for (int q = 0; q < 32; ++q)
-              if (c + q < n_q) scores[int64_t(q_base + c + q) * ld + p] = (__uint_as_float(hi[q]) + __uint_as_float(lo[q])) * inv;
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_512(tmem_base);
+  const int wg = (warp >> 2) - 1;
+  const int w = warp & 3;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    float acc[NCH][32];
+    for (int kb = 0; kb < n_kblocks; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t a_addr = smem_u32(smem + size_t(stage) * kStageBytes);
+      const uint64_t ad = wgmma_desc_kmajor_sw128(a_addr + uint32_t(wg) * 64u * 128u);
+      const uint64_t bd = wgmma_desc_kmajor_sw128(a_addr + kScanATile);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch)
+          wgmma_m64n64k16_bf16(acc[ch], ad + ks * 2, bd + uint64_t(ch * 64 * 128 / 16) + ks * 2, (kb | ks) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int ch = 0; ch < NCH; ++ch) reg_fence_all(acc[ch]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);
+      if (++stage == num_stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    // thread rows r0 = 16w + l/4 and r0 + 8 of this warpgroup's 64 pages; columns 8j + 2(l%4) + {0,1} of every chunk
+    const int64_t p0 = tile * 128 + wg * 64 + 16 * w + (lane >> 2);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t p = p0 + 8 * i;
+      if (p >= n_pages) continue;
+      const float inv = __ldg(inv_norm + p);
+#pragma unroll
+      for (int col = 0; col < kHalf; col += 8)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int q = col + 2 * (lane & 3) + c;  // hi column q, lo column kHalf + q
+          const int hi_ch = col / 64, hi_j = (col % 64) / 8;
+          const int lo_ch = (col + kHalf) / 64, lo_j = ((col + kHalf) % 64) / 8;
+          if (q < n_q)
+            scores[int64_t(q_base + q) * ld + p] = (acc[hi_ch][4 * hi_j + 2 * i + c] + acc[lo_ch][4 * lo_j + 2 * i + c]) * inv;
+        }
+    }
   }
 }
 
@@ -464,7 +425,7 @@ int launch_fde_scan(b200ms_t* h, const void* F, const float* inv_norm, int64_t n
   if (int e = make_tmap_rows(h, &tf, F, B200MS_BF16, n_pages, 128, int64_t(fd) * 2)) return e;
   for (int qb = 0; qb < n_q; qb += 128) {
     const int n_here = n_q - qb < 128 ? n_q - qb : 128;
-    const int half = n_here <= 16 ? 16 : ((n_here + 31) & ~31);
+    const int half = n_here <= 32 ? 32 : n_here <= 64 ? 64 : 128;
     const int nqp = 2 * half;
     if (int e = reserve(h, h->fde_q_bf16, size_t(nqp) * fd * 2 + 1024)) return e;
     __nv_bfloat16* qb16 = reinterpret_cast<__nv_bfloat16*>((reinterpret_cast<uintptr_t>(h->fde_q_bf16.p) + 1023) & ~uintptr_t(1023));
@@ -477,13 +438,21 @@ int launch_fde_scan(b200ms_t* h, const void* F, const float* inv_norm, int64_t n
     int stages = int((232448u - 1024u - 1024u) / stage_bytes);
     if (stages > 12) stages = 12;
     const uint32_t smem = 1024 + uint32_t(stages) * stage_bytes + 1024;
-    if (int e = ensure_smem(h, reinterpret_cast<const void*>(fde_scan_umma_kernel), int(smem), "cudaFuncSetAttribute(fde_scan_umma)"))
-      return e;
+    const void* kern = nqp == 64    ? reinterpret_cast<const void*>(fde_scan_wgmma_kernel<1>)
+                       : nqp == 128 ? reinterpret_cast<const void*>(fde_scan_wgmma_kernel<2>)
+                                    : reinterpret_cast<const void*>(fde_scan_wgmma_kernel<4>);
+    if (int e = ensure_smem(h, kern, int(smem), "cudaFuncSetAttribute(fde_scan_wgmma)")) return e;
     const int64_t n_tiles = (n_pages + 127) / 128;
     const int grid = int(n_tiles < h->num_sms ? n_tiles : h->num_sms);
-    fde_scan_umma_kernel<<<grid, kScanThreads, smem, s>>>(tf, tq, inv_norm, n_pages, fd / 64, n_here, qb, half, scores, ld, stages);
+    const int nkb = fd / 64;
+    if (nqp == 64)
+      fde_scan_wgmma_kernel<1><<<grid, kScanThreads, smem, s>>>(tf, tq, inv_norm, n_pages, nkb, n_here, qb, scores, ld, stages);
+    else if (nqp == 128)
+      fde_scan_wgmma_kernel<2><<<grid, kScanThreads, smem, s>>>(tf, tq, inv_norm, n_pages, nkb, n_here, qb, scores, ld, stages);
+    else
+      fde_scan_wgmma_kernel<4><<<grid, kScanThreads, smem, s>>>(tf, tq, inv_norm, n_pages, nkb, n_here, qb, scores, ld, stages);
     h->launches++;
-    if (int e = check_cuda(h, cudaGetLastError(), "launch fde_scan_umma")) return e;
+    if (int e = check_cuda(h, cudaGetLastError(), "launch fde_scan_wgmma")) return e;
   }
   return B200MS_OK;
 }

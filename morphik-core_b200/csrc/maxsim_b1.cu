@@ -12,7 +12,7 @@
 // coalesced 512-byte request (lane i loads row i as a uint4), parked in a per-warp shared-memory slab, and
 // replayed row by row as 128-bit broadcast reads; per (row, token) the work is 6 LOP3 + 3 POPC (carry-save trick, see
 // the kernel) + 2 ADD + 1 MIN.
-// Bound: the integer POPC pipe, not HBM (16 B per patch vector; SURVEY 8d) -- see DESIGN.md.
+// Bound: the integer POPC pipe, not HBM (16 B per patch vector; SURVEY 8d).
 #include "common.cuh"
 #include "ptx.cuh"
 

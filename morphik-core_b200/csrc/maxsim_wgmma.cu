@@ -1,0 +1,581 @@
+// maxsim_wgmma.cu -- the bf16, int8, fp8 and 1-bit MaxSim scorers on Hopper (sm_90a) warpgroup MMA.
+//
+// Replaces the reference's float scorer  einsum("bnd,csd->bcns").max(3).sum(2)  (colpali_engine score_multi_vector,
+// called at core/vector_store/fast_multivector_store.py:553-555) and the SQL public.max_sim of the 1-bit path
+// (core/vector_store/multi_vector_store.py:287-311).  The [B_q, C, T, P] similarity tensor is never materialised: each
+// 64 x 128 (query tokens x patch rows) product lives only in the registers of one warpgroup.
+//
+// Data layout in HBM
+//   corpus rows   [n_rows, 128] bf16|s8|e4m3 (or [n_rows, 16 B] sign bits), row-major, every page padded to a multiple of
+//                 32 rows ("chunks") by repeating its last row; chunk_page[c] = page index of chunk c
+//   work units    unit_start[u] .. unit_end[u] = chunk range of unit u, always whole pages (so no page is ever split across
+//                 CTAs and the per-token running max never crosses a CTA boundary)
+//   queries       [n_groups*32, 128] same dtype, each query padded with zero rows to 32-row groups; a query tile is 4 groups
+//                 = 128 query tokens
+//   scores        group_scores[g, p] (f32 | s32), g = 32-token group, p = page (slot_mode: candidate slot)
+//
+// Kernel (persistent, one CTA per SM, 384 threads, warp-specialised):
+//   warpgroup 0     producer.  Dense dtypes: one thread streams 128-row patch tiles (SWIZZLE_128B TMA boxes) through an
+//                   S-stage mbarrier ring.  1-bit corpora: all 128 threads fetch 16 B of sign bits per row and expand them
+//                   to {0,1} bytes in the same swizzled K-major layout (thread r owns row r of the tile); e4m3 corpora: the
+//                   same, 128 B of e4m3 per row widened to f16 (mma_tile.cuh says why).
+//   warpgroups 1-2  MMA + epilogue.  Warpgroup e owns the resident query tiles m with m % 2 == e.  A query tile is loaded as
+//                   two 64-row wgmma A blocks: block h holds tokens 16h .. 16h+15 of each of the four groups, so warp w of the
+//                   warpgroup ends up holding all 32 tokens of group w (rows l/4 and l/4+8 of both blocks) and sums its
+//                   group with warp shuffles only.  Per patch tile and query tile: two m64n128 wgmma chains (8 x k16 for
+//                   bf16 / f16, 4 x k32 for int8), per-thread max over the 8 columns of every chunk it holds, a quad
+//                   shuffle for the other 24, a running max per (token, page), and at a page end the group's sum.
+// 1-bit:  128 - ham(q, d) = (128 - popc(q)) + <q', d'>  with q' = +1 / -1 per query bit and d' = 1 / 0 per document bit, so
+//         max_r (128 - ham) = c_t + max_r <q'_t, d'_r> runs as the int8 kernel plus a per-token constant c_t (0 for padding).
+#include "common.cuh"
+#include "mma_tile.cuh"
+#include "ptx.cuh"
+
+namespace bms {
+
+constexpr int kThreads = 384;
+constexpr uint32_t kQBlockBytes = 64 * 128;  // one 64-row A block of one 128-byte panel
+
+// ------------------------------------------------------------------ 1-bit query side: bits -> +-1 int8 rows + token constants
+__global__ void __launch_bounds__(256)
+b1_query_expand_kernel(const uint8_t* __restrict__ q_bits /*[rows,16]*/, const int32_t* __restrict__ group_ntok, int n_rows,
+                       int8_t* __restrict__ out /*[rows,128]*/, int32_t* __restrict__ tok_const /*[rows]*/) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // one thread per (row, byte of bits)
+  const int row = idx >> 4, b = idx & 15;
+  if (row >= n_rows) return;
+  const bool real = (row & 31) < __ldg(group_ntok + (row >> 5));
+  const uint32_t bits = q_bits[row * 16 + b];
+  uint32_t lo = 0, hi = 0;  // elements 8b..8b+3 and 8b+4..8b+7 as int8 (MSB of the byte = first element)
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    lo |= (real ? (((bits >> (7 - e)) & 1u) ? 0x01u : 0xffu) : 0u) << (8 * e);
+    hi |= (real ? (((bits >> (3 - e)) & 1u) ? 0x01u : 0xffu) : 0u) << (8 * e);
+  }
+  reinterpret_cast<uint2*>(out)[row * 16 + b] = make_uint2(lo, hi);
+  if (b == 0) {
+    const uint4 w = *reinterpret_cast<const uint4*>(q_bits + row * 16);
+    tok_const[row] = real ? 128 - (__popc(w.x) + __popc(w.y) + __popc(w.z) + __popc(w.w)) : 0;
+  }
+}
+
+// ------------------------------------------------------------------ tile iterator shared by all warp roles
+struct TileIter {
+  int u, t, n_tiles, c0, c1;
+  __device__ __forceinline__ void load(const int32_t* us, const int32_t* ue, int n_units) {
+    n_tiles = 0;
+    while (u < n_units) {
+      c0 = __ldg(us + u);
+      c1 = __ldg(ue + u);
+      n_tiles = (c1 - c0 + 3) >> 2;
+      if (n_tiles > 0) break;
+      u += gridDim.x;
+    }
+    t = 0;
+  }
+  __device__ __forceinline__ bool valid(int n_units) const { return u < n_units; }
+  __device__ __forceinline__ void next(const int32_t* us, const int32_t* ue, int n_units) {
+    if (++t == n_tiles) {
+      u += gridDim.x;
+      load(us, ue, n_units);
+    }
+  }
+  __device__ __forceinline__ int64_t row0() const { return int64_t(c0 + 4 * t) * kGroup; }
+};
+
+template <int KIND>
+__device__ __forceinline__ void mma_chain(typename Kind<KIND>::Acc (&d)[64], uint32_t a_addr, uint32_t b_addr) {
+  const uint64_t ad = wgmma_desc_kmajor_sw128(a_addr);
+  const uint64_t bd = wgmma_desc_kmajor_sw128(b_addr);
+#pragma unroll
+  for (int ks = 0; ks < Kind<KIND>::kKSteps; ++ks) {  // 32 B of K per step; 4 steps per 128 B panel
+    const uint32_t off = ((ks >> 2) * kSubtileBytes + (ks & 3) * 32) >> 4;
+    if constexpr (KIND == 0) {
+      wgmma_m64n128k16_bf16(d, ad + off, bd + off, ks != 0);
+    } else if constexpr (KIND == 1) {
+      wgmma_m64n128k32_s8(d, ad + off, bd + off, ks != 0);
+    } else {
+      wgmma_m64n128k16_f16(d, ad + off, bd + off, ks != 0);
+    }
+  }
+  wgmma_commit();
+}
+
+// group sum of one warp: 4 token values per thread (the quad's four lanes hold the same ones), 8 quads
+template <typename Acc>
+__device__ __forceinline__ Acc group_sum(const Acc (&v)[4]) {
+  Acc s = (v[0] + v[1]) + (v[2] + v[3]);
+  s += __shfl_xor_sync(0xffffffffu, s, 4);
+  s += __shfl_xor_sync(0xffffffffu, s, 8);
+  s += __shfl_xor_sync(0xffffffffu, s, 16);
+  return s;
+}
+
+// e4m3 x 8 (one 8-byte word) -> 8 f16 (exact)
+__device__ __forceinline__ uint4 e4m3x8_to_f16x8(uint32_t lo, uint32_t hi) {
+  uint4 o;
+  asm("{\n\t.reg .b16 a, b, c, d;\n\t"
+      "mov.b32 {a, b}, %4;\n\tmov.b32 {c, d}, %5;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, a;\n\tcvt.rn.f16x2.e4m3x2 %1, b;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %2, c;\n\tcvt.rn.f16x2.e4m3x2 %3, d;\n\t}"
+      : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+      : "r"(lo), "r"(hi));
+  return o;
+}
+
+// e4m3 query rows -> f16 rows (the A operand of the KIND 2 kernel)
+__global__ void __launch_bounds__(256)
+f8_query_widen_kernel(const uint2* __restrict__ q, int64_t n_words, uint4* __restrict__ out) {
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n_words; i += int64_t(gridDim.x) * blockDim.x) {
+    const uint2 v = __ldg(q + i);
+    out[i] = e4m3x8_to_f16x8(v.x, v.y);
+  }
+}
+
+// KIND 0 bf16, 1 int8 (BITS: 1-bit corpus expanded to int8), 2 fp8 e4m3 (widened to f16 by the producer warpgroup);
+// NM = resident query tiles (1, 2, 4 or 8).
+template <int KIND, int NM, bool BITS>
+__global__ void __launch_bounds__(kThreads, 1)
+maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_constant__ CUtensorMap tmap_q,
+                    const uint4* __restrict__ bit_rows, int64_t n_rows, const int32_t* __restrict__ tok_const,
+                    const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start,
+                    const int32_t* __restrict__ unit_end, int slot_mode, int n_units, int m_tile_base, int n_groups_real,
+                    const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
+                    int num_stages) {
+  using K = Kind<KIND>;
+  using Acc = typename K::Acc;
+  static_assert(!BITS || KIND == 1, "1-bit corpora run on the int8 MMA");
+  constexpr int NWG = NM >= 2 ? 2 : 1;   // consumer warpgroups with work
+  constexpr int MPW = (NM + 1) / 2;      // query tiles per consumer warpgroup
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_q = smem;                                            // NM query tiles
+  uint8_t* smem_st = smem + NM * K::kTileBytes;                      // num_stages patch tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_st + size_t(num_stages) * K::kTileBytes);
+  uint64_t* full = bars;                     // [num_stages] producer -> MMA
+  uint64_t* empty = bars + 16;               // [num_stages] MMA -> producer
+  uint64_t* qfull = bars + 32;               // query tiles landed
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  constexpr bool kExpand = BITS || KIND == 2;  // the producer warpgroup writes the patch tiles itself
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_q);
+    if constexpr (!kExpand) prefetch_tmap(&tmap_rows);
+    for (int i = 0; i < num_stages; ++i) {
+      mbar_init(&full[i], kExpand ? 4 : 1);  // expanding producers: one arrival per warp
+      mbar_init(&empty[i], 4 * NWG);      // one arrival per consumer warp
+    }
+    mbar_init(qfull, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ================================================================ producer warpgroup
+    if (threadIdx.x == 0) {
+      // query tile m, block h, group g: rows 32g + 16h .. +16 of the tile -> rows 16g .. 16g+15 of A block h
+      const uint64_t pol_q = policy_evict_last();
+      mbar_expect_tx(qfull, NM * K::kTileBytes);
+      for (int m = 0; m < NM; ++m)
+        for (int p = 0; p < K::kPanels; ++p)
+          for (int hb = 0; hb < 2; ++hb)
+            for (int g = 0; g < 4; ++g)
+              tma_load_2d(&tmap_q, qfull, smem_q + m * K::kTileBytes + p * kSubtileBytes + hb * kQBlockBytes + g * 2048,
+                          p * K::kPanelElems, (m_tile_base + m) * kTileM + 32 * g + 16 * hb, pol_q);
+    }
+    if constexpr (!kExpand) {
+      if (threadIdx.x == 0) {
+        const uint64_t pol_rows = policy_evict_first();
+        int stage = 0;
+        uint32_t phase = 0;
+        TileIter it;
+        it.u = blockIdx.x;
+        it.load(unit_start, unit_end, n_units);
+        for (; it.valid(n_units); it.next(unit_start, unit_end, n_units)) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_expect_tx(&full[stage], K::kTileBytes);
+          uint8_t* dst = smem_st + size_t(stage) * K::kTileBytes;
+#pragma unroll
+          for (int p = 0; p < K::kPanels; ++p)
+            tma_load_2d(&tmap_rows, &full[stage], dst + p * kSubtileBytes, p * K::kPanelElems, int32_t(it.row0()), pol_rows);
+          if (++stage == num_stages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    } else if constexpr (KIND == 2) {
+      // widening: e4m3 rows -> f16, swizzled K-major, two 64-element panels; thread r owns row r of the tile and keeps the
+      // loads of the next tile in flight while it converts the current one
+      const int r = threadIdx.x;
+      const uint32_t row_off = uint32_t(r >> 3) * 1024u + uint32_t(r & 7) * 128u;
+      const uint32_t sw = uint32_t(r & 7);
+      const uint4* rows16 = reinterpret_cast<const uint4*>(bit_rows);  // [n_rows, 8] x 16 B
+      TileIter cur, pf;
+      cur.u = blockIdx.x;
+      cur.load(unit_start, unit_end, n_units);
+      pf = cur;
+      uint4 nxt[8];
+      auto fetch = [&](uint4 (&v)[8]) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = make_uint4(0, 0, 0, 0);
+        if (pf.valid(n_units)) {
+          const int64_t row = pf.row0() + r;
+          if (row < n_rows) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = __ldg(rows16 + row * 8 + i);
+          }
+          pf.next(unit_start, unit_end, n_units);
+        }
+      };
+      fetch(nxt);
+      int stage = 0;
+      uint32_t phase = 0;
+      while (cur.valid(n_units)) {
+        uint4 mine[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) mine[i] = nxt[i];
+        fetch(nxt);
+        mbar_wait(&empty[stage], phase ^ 1);
+        const uint32_t tile = smem_u32(smem_st) + uint32_t(stage) * K::kTileBytes + row_off;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {  // elements 16i .. 16i+15 -> f16 chunks 2i, 2i+1 (panel 2i / 8)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const uint32_t c = uint32_t(2 * i + hh);
+            const uint4 o = hh == 0 ? e4m3x8_to_f16x8(mine[i].x, mine[i].y) : e4m3x8_to_f16x8(mine[i].z, mine[i].w);
+            st_shared_v4(tile + (c >> 3) * kSubtileBytes + (((c & 7) ^ sw) << 4), o);
+          }
+        }
+        fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&full[stage]);
+        if (++stage == num_stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+        cur.next(unit_start, unit_end, n_units);
+      }
+    } else {
+      // expanders: packed bits -> {0,1} int8, swizzled K-major; loads of the next 8 tiles stay in flight meanwhile
+      const int r = threadIdx.x;  // row of the tile this thread owns
+      const uint32_t row_off = uint32_t(r >> 3) * 1024u + uint32_t(r & 7) * 128u;
+      const uint32_t sw = uint32_t(r & 7);
+      TileIter cur, pf;
+      cur.u = blockIdx.x;
+      cur.load(unit_start, unit_end, n_units);
+      pf = cur;
+      constexpr int kRing = 8;
+      uint4 ring[kRing];
+#pragma unroll
+      for (int i = 0; i < kRing; ++i) {
+        ring[i] = make_uint4(0, 0, 0, 0);
+        if (pf.valid(n_units)) {
+          const int64_t row = pf.row0() + r;
+          if (row < n_rows) ring[i] = __ldg(bit_rows + row);
+          pf.next(unit_start, unit_end, n_units);
+        }
+      }
+      int stage = 0;
+      uint32_t phase = 0;
+      while (cur.valid(n_units)) {
+#pragma unroll
+        for (int i = 0; i < kRing; ++i) {
+          if (!cur.valid(n_units)) break;
+          const uint4 mine = ring[i];
+          ring[i] = make_uint4(0, 0, 0, 0);
+          if (pf.valid(n_units)) {
+            const int64_t row = pf.row0() + r;
+            if (row < n_rows) ring[i] = __ldg(bit_rows + row);
+            pf.next(unit_start, unit_end, n_units);
+          }
+          mbar_wait(&empty[stage], phase ^ 1);
+          const uint32_t tile = smem_u32(smem_st) + uint32_t(stage) * K::kTileBytes + row_off;
+          const uint32_t words[4] = {mine.x, mine.y, mine.z, mine.w};
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            // __brev: bit e%8 of (reversed) byte 3-b now holds element 8b + e%8 of this word's 32 elements
+            const uint32_t rev = __brev(words[w]);
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {  // 16-byte chunk c = 2w + hh  <-  source bytes 2hh, 2hh+1 of the word
+              // nibble n (bit e = element e) * 0x204081 puts bit k at k, k+7, k+14, k+21; masked with 0x01010101 that is
+              // one element per byte.  (Only valid for 4-bit inputs: with 8 bits the shifted copies overlap and carry.)
+              const uint32_t b0 = (rev >> (8 * (3 - 2 * hh))) & 0xffu, b1 = (rev >> (8 * (2 - 2 * hh))) & 0xffu;
+              uint4 o;
+              o.x = ((b0 & 0xfu) * 0x00204081u) & 0x01010101u;
+              o.y = ((b0 >> 4) * 0x00204081u) & 0x01010101u;
+              o.z = ((b1 & 0xfu) * 0x00204081u) & 0x01010101u;
+              o.w = ((b1 >> 4) * 0x00204081u) & 0x01010101u;
+              const uint32_t c = uint32_t(2 * w + hh);
+              st_shared_v4(tile + ((c ^ sw) << 4), o);
+            }
+          }
+          fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&full[stage]);
+          if (++stage == num_stages) {
+            stage = 0;
+            phase ^= 1;
+          }
+          cur.next(unit_start, unit_end, n_units);
+        }
+      }
+    }
+    return;
+  }
+
+  // ================================================================ consumer warpgroups: MMA + epilogue
+  const int wg = (warp >> 2) - 1;
+  const int w = warp & 3;  // group w of every query tile this warpgroup owns
+  if (wg >= NWG) return;
+  mbar_wait(qfull, 0);
+  const uint32_t q_addr = smem_u32(smem_q);
+  const uint32_t st_addr = smem_u32(smem_st);
+
+  Acc runmax[MPW][4];
+  Acc cnst[MPW][4];
+  int cur_page[MPW];
+#pragma unroll
+  for (int i = 0; i < MPW; ++i) {
+    const int mt = m_tile_base + wg + 2 * i;
+    const bool active = (wg + 2 * i) < NM && mt * 4 + w < n_groups_real;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      runmax[i][k] = Acc(0);
+      cnst[i][k] = Acc(0);
+      if constexpr (BITS) {  // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w
+        if (active) cnst[i][k] = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2));
+      }
+    }
+    cur_page[i] = -1;
+  }
+
+  auto flush = [&](int i, int u) {
+    const int mt = m_tile_base + wg + 2 * i;
+    const int group = mt * 4 + w;
+    if (group < n_groups_real && cur_page[i] >= 0) {
+      const int o = slot_mode ? u : cur_page[i];
+      Acc v[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) v[k] = clamp_token_max(clamp_bits, o, runmax[i][k]) + cnst[i][k];
+      const Acc s = group_sum(v);
+      if (lane == 0) group_scores[int64_t(group) * ld + o] = s;
+    }
+  };
+
+  int stage = 0;
+  uint32_t phase = 0;
+  int last_u = -1;
+  TileIter it;
+  it.u = blockIdx.x;
+  it.load(unit_start, unit_end, n_units);
+  for (; it.valid(n_units); it.next(unit_start, unit_end, n_units)) {
+    if (it.u != last_u) {  // new unit: units end on page boundaries
+      if (last_u >= 0) {
+#pragma unroll
+        for (int i = 0; i < MPW; ++i) flush(i, last_u);
+      }
+#pragma unroll
+      for (int i = 0; i < MPW; ++i) cur_page[i] = -1;
+      last_u = it.u;
+    }
+    const int cb = it.c0 + 4 * it.t;
+    int pg[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) pg[j] = (cb + j < it.c1) ? __ldg(chunk_page + cb + j) : -1;
+    mbar_wait(&full[stage], phase);
+    const uint32_t b_addr = st_addr + uint32_t(stage) * K::kTileBytes;
+#pragma unroll
+    for (int i = 0; i < MPW; ++i) {
+      const int m = wg + 2 * i;
+      if (m >= NM) break;
+      const uint32_t a_addr = q_addr + uint32_t(m) * K::kTileBytes;
+      Acc d0[64], d1[64];
+      wgmma_fence();
+      mma_chain<KIND>(d0, a_addr, b_addr);
+      mma_chain<KIND>(d1, a_addr + kQBlockBytes, b_addr);
+      Acc cm[4][4];  // [token k][chunk]
+      {
+        wgmma_wait<1>();
+        reg_fence_all(d0);
+        Acc c2[2][4];
+        chunk_maxima(d0, c2);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          cm[0][c] = c2[0][c];
+          cm[1][c] = c2[1][c];
+        }
+      }
+      {
+        wgmma_wait<0>();
+        reg_fence_all(d1);
+        if (i == MPW - 1 || m + 2 >= NM) {  // every read of this stage has completed
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[stage]);
+        }
+        Acc c2[2][4];
+        chunk_maxima(d1, c2);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          cm[2][c] = c2[0][c];
+          cm[3][c] = c2[1][c];
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (pg[j] < 0) continue;  // chunk belongs to the next unit
+        if (pg[j] != cur_page[i]) {
+          flush(i, it.u);
+          cur_page[i] = pg[j];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) runmax[i][k] = cm[k][j];
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) runmax[i][k] = acc_max(runmax[i][k], cm[k][j]);
+        }
+      }
+    }
+    if (++stage == num_stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  if (last_u >= 0) {
+#pragma unroll
+    for (int i = 0; i < MPW; ++i) flush(i, last_u);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------- host side
+template <int KIND, int NM, bool BITS>
+static int launch_one(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const, int m_tile_base,
+                      int n_groups_real, void* scores, int64_t ld, cudaStream_t s) {
+  using K = Kind<KIND>;
+  const Corpus& c = h->corpus;
+  const uint32_t avail = kSmemLimit - 1024 /*align*/ - kBarrierBytes - NM * K::kTileBytes;
+  int stages = int(avail / K::kTileBytes);
+  if (stages > 8) stages = 8;
+  if (stages < 2) return set_error(h, B200MS_EINVAL, "maxsim_wgmma: not enough shared memory for 2 stages");
+  const uint32_t smem = 1024 + NM * K::kTileBytes + uint32_t(stages) * K::kTileBytes + kBarrierBytes;
+  auto kern = maxsim_wgmma_kernel<KIND, NM, BITS>;
+  if (int e = ensure_smem(h, reinterpret_cast<const void*>(kern), int(smem), "cudaFuncSetAttribute(maxsim_wgmma)"))
+    return e;
+  int grid = h->max_ctas > 0 ? h->max_ctas : h->num_sms;
+  if (grid > up.n_units) grid = up.n_units;
+  if (grid < 1) return B200MS_OK;
+  kern<<<grid, kThreads, smem, s>>>(c.tmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
+                                   static_cast<const int32_t*>(h->chunk_page.p), up.start, up.end, up.slot_mode, up.n_units,
+                                   m_tile_base, n_groups_real, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
+                                   stages);
+  h->launches++;
+  return check_cuda(h, cudaGetLastError(), "launch maxsim_wgmma");
+}
+
+// Query tiles [base, base + nm) in one pass over the corpus.  nm is rounded up to a power of two: a phantom (all-zero) tile
+// costs less than a second pass over the corpus.
+template <int KIND, bool BITS>
+static int launch_tiles(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const, int n_groups_real,
+                        int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
+  constexpr int kMaxNM = Kind<KIND>::kMaxNM;
+  for (int base = m_lo; base < m_hi;) {
+    const int rem = m_hi - base;
+    int nm = 1;
+    while (nm < rem && nm < kMaxNM) nm <<= 1;
+    int e;
+    switch (nm) {
+      case 1: e = launch_one<KIND, 1, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 2: e = launch_one<KIND, 2, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 4: e = launch_one<KIND, 4, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      default:
+        if constexpr (kMaxNM >= 8) {
+          e = launch_one<KIND, 8, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s);
+        } else {
+          e = set_error(h, B200MS_EINVAL, "maxsim_wgmma: bad NM");
+        }
+    }
+    if (e) return e;
+    base += nm;
+  }
+  return B200MS_OK;
+}
+
+// query rows as 16-row TMA boxes (two per group and A block, see the kernel); re-encoded only when (pointer, dtype, rows) change
+static int query_tmap(b200ms_t* h, const void* q, int dtype, int n_q_rows) {
+  if (h->tmap_q_base == q && h->tmap_q_dtype == dtype && h->tmap_q_rows == n_q_rows) return B200MS_OK;
+  if (int e = make_tmap_rows(h, &h->tmap_q, q, dtype, int64_t(n_q_rows), 16)) return e;
+  h->tmap_q_base = q;
+  h->tmap_q_dtype = dtype;
+  h->tmap_q_rows = n_q_rows;
+  return B200MS_OK;
+}
+
+// m_tile_lo / m_tile_hi: score only query tiles [m_tile_lo, m_tile_hi) (hi < 0: all) -- the batched rerank walks the query
+// tiles one launch at a time, each against its own candidate units.
+int launch_score_wgmma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, int n_groups_real, void* group_scores,
+                       int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
+  const Corpus& c = h->corpus;
+  UnitPlan up;
+  if (plan) {
+    up = *plan;
+  } else {  // full scan: unit u = [unit_start[u], unit_start[u+1])
+    up.start = static_cast<const int32_t*>(h->unit_start.p);
+    up.end = up.start + 1;
+    up.n_units = c.n_units;
+    up.slot_mode = 0;
+  }
+  if (!c.has_tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
+  const int n_groups_padded = (n_groups_real + 3) & ~3;
+  const int n_mtiles = n_groups_padded / 4;
+  const int n_q_rows = n_groups_padded * kGroup;
+  if (c.dtype == B200MS_F8) {  // the A operand of the f16 MMA: the e4m3 query rows widened to f16
+    if (int e = reserve(h, h->f8_q_f16, size_t(n_q_rows) * 256 + 1024)) return e;
+    void* wide = reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(h->f8_q_f16.p) + 1023) & ~uintptr_t(1023));
+    const int64_t n_words = int64_t(n_q_rows) * 16;
+    f8_query_widen_kernel<<<int((n_words + 255) / 256 < 4 * h->num_sms ? (n_words + 255) / 256 : 4 * h->num_sms), 256, 0, s>>>(
+        static_cast<const uint2*>(q_packed), n_words, static_cast<uint4*>(wide));
+    h->launches++;
+    if (int e = check_cuda(h, cudaGetLastError(), "launch f8_query_widen")) return e;
+    if (int e = query_tmap(h, wide, B200MS_BF16, n_q_rows)) return e;  // any 2-byte element type: TMA only copies
+  } else if (int e = query_tmap(h, q_packed, c.dtype, n_q_rows)) {
+    return e;
+  }
+  int lo = 0, hi = n_mtiles;
+  if (m_tile_hi >= 0) {
+    lo = m_tile_lo;
+    hi = m_tile_hi < n_mtiles ? m_tile_hi : n_mtiles;
+  }
+  switch (kind_of_dtype(c.dtype)) {
+    case 0: return launch_tiles<0, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 1: return launch_tiles<1, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 2: return launch_tiles<2, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    default: return set_error(h, B200MS_ESTATE, "score: corpus dtype has no wgmma scorer");
+  }
+}
+
+// 1-bit full scan: the query bits become +-1 int8 rows (b1_q_i8) and per-token constants, then the int8 kernel with the
+// expanding producer.
+int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
+                          void* group_scores, int64_t ld, cudaStream_t s) {
+  const Corpus& c = h->corpus;
+  const int n_groups_padded = (n_groups_real + 3) & ~3;
+  const int n_rows = n_groups_padded * kGroup;
+  if (int e = reserve(h, h->b1_q_i8, size_t(n_rows) * 128 + 1024)) return e;
+  if (int e = reserve(h, h->b1_tok_const, size_t(n_rows) * 4)) return e;
+  int8_t* q_i8 = reinterpret_cast<int8_t*>((reinterpret_cast<uintptr_t>(h->b1_q_i8.p) + 1023) & ~uintptr_t(1023));
+  int32_t* tok_const = static_cast<int32_t*>(h->b1_tok_const.p);
+  b1_query_expand_kernel<<<(n_rows * 16 + 255) / 256, 256, 0, s>>>(static_cast<const uint8_t*>(q_bits), group_ntok_dev, n_rows,
+                                                                  q_i8, tok_const);
+  h->launches++;
+  if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
+  if (int e = query_tmap(h, q_i8, B200MS_I8, n_rows)) return e;
+  UnitPlan up;
+  up.start = static_cast<const int32_t*>(h->unit_start.p);
+  up.end = up.start + 1;
+  up.n_units = c.n_units;
+  up.slot_mode = 0;
+  return launch_tiles<1, true>(h, up, h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
+}
+
+}  // namespace bms

@@ -358,7 +358,7 @@ class TwoStageIndex:
     def search_device(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
                       id_base: int = 0):
         """Two-stage search, everything on the device and asynchronous: query FDEs -> ONE scan of the FDE matrix for the
-        whole batch (tcgen05) -> top-n_candidates per query -> ONE batched rerank call (each query against its own list)
+        whole batch (wgmma) -> top-n_candidates per query -> ONE batched rerank call (each query against its own list)
         -> top-k.  Returns device tensors (scores [n_q,kk], page ids + id_base [n_q,kk], counts [n_q]) and the CUDA events
         that bracket the stages (for last_timing_ms)."""
         n_q = len(queries)

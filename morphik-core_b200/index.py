@@ -37,7 +37,7 @@ def _aligned_bytes(nbytes: int, device: torch.device, align: int = 1024) -> torc
 class MaxSimIndex:
     """Packed corpus of pages (each a [P_i, 128] matrix of patch embeddings) on one GPU.
 
-    Layout in HBM (see DESIGN.md): rows of ``row_bytes`` (bf16 256 B / int8 128 B / sign bits 16 B), every page padded to a
+    Layout in HBM: rows of ``row_bytes`` (bf16 256 B / int8 128 B / sign bits 16 B), every page padded to a
     multiple of 32 rows by repeating its last row, pages back to back in insertion order.  ``page id`` = insertion index.
     """
 
@@ -45,7 +45,7 @@ class MaxSimIndex:
         if dtype not in nat.DTYPE_NAMES or nat.DTYPE_NAMES[dtype] == nat.F32:
             raise ValueError(f"dtype must be one of bf16/int8/fp8/binary, got {dtype!r}")
         if not torch.cuda.is_available():
-            raise nat.NativeError("MaxSimIndex needs a CUDA device (B200); there is no CPU fallback")
+            raise nat.NativeError("MaxSimIndex needs a CUDA device (H100); there is no CPU fallback")
         self.device = torch.device("cuda", int(device))
         self.dtype = nat.DTYPE_NAMES[dtype]
         self.dtype_name = dtype

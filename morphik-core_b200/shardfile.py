@@ -3,8 +3,8 @@
 The reference keeps multivectors as one object per page: ``numpy.save`` of float32 ``[P,128]`` under
 ``multivector/{document_id}/{chunk_number}.npy`` (core/vector_store/fast_multivector_store.py:673-707, read back one by one
 at :713-774 through a disk LRU cache), or as ``BIT(128)[]`` rows in Postgres (multi_vector_store.py:240-251).  Rebuilding a
-GPU corpus from those costs one object fetch / row decode per page.  A shard file is the packed HBM layout itself
-(DESIGN.md section 3), so loading is a sequence of large sequential reads + H2D copies and nothing else:
+GPU corpus from those costs one object fetch / row decode per page.  A shard file is the packed HBM layout itself,
+so loading is a sequence of large sequential reads + H2D copies and nothing else:
 
     offset 0     : 4096-byte header  = magic "B2MSHARD", version, dtype, n_pages, n_rows_padded, row_bytes, i8_scale (JSON, NUL padded)
     offset 4096  : page_lens  int32[n_pages]   (true lengths), zero padded to a 4096-byte boundary

@@ -175,7 +175,7 @@ class QueryCoalescer:
 
 
 class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
-    """Exhaustive ColPali MaxSim store on one B200 (see module docstring)."""
+    """Exhaustive ColPali MaxSim store on one H100 (see module docstring)."""
 
     def __init__(self, uri: str = "b200://0", device: int = 0, mode: str = "bf16", storage: Any = None,
                  auto_initialize: bool = True, compact_dead_fraction: float = 0.3, index: Any = None,

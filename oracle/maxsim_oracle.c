@@ -5,7 +5,7 @@
  * product (morphik-core_b200/) may link, import or call this file; it is the checker used by
  * tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs.
  *
- * Every function cites the reference lines it restates (paths relative to /root/reference):
+ * Every function cites the reference lines it restates (paths relative to the morphik-core repository root):
  *   - sign quantise + MSB-first pack : core/utils/fast_ops.py:191-227 (authoritative pure-Python
  *                                      fallback), morphik_rust/src/binary_ops.rs:147-222
  *   - Hamming distance               : core/utils/fast_ops.py:230-248, binary_ops.rs:237-292

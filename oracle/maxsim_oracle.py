@@ -5,7 +5,7 @@ loader for the C restatement in ``maxsim_oracle.c``.  Only ``tests/``, ``__graft
 ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import this module; the product package
 (``morphik-core_b200/``) must never do so.
 
-Reference lines restated (relative to /root/reference):
+Reference lines restated (relative to the morphik-core repository root):
   * sign quantise + MSB-first pack : core/utils/fast_ops.py:191-227, morphik_rust/src/binary_ops.rs:147-222
   * Hamming                        : core/utils/fast_ops.py:230-248, morphik_rust/src/binary_ops.rs:237-292
   * binary MaxSim                  : core/vector_store/multi_vector_store.py:287-311 (SQL max_sim), :759 (ORDER BY)

@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and puts the repo root on sys.path.
 
 `-m "not gpu"` runs on the build container (no GPU): oracle-vs-golden, host logic, C-ABI symbol checks, gloo tests.
-`-m gpu` runs on a B200 box: parity of the CUDA path (through the C-ABI) against the oracle.
+`-m gpu` runs on an H100: parity of the CUDA path (through the C-ABI) against the oracle.
 """
 import os
 import sys
@@ -16,7 +16,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

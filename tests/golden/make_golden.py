@@ -1,11 +1,10 @@
 """Generate the golden fixtures under tests/golden/ by EXECUTING reference code in the build container.
 
-Run from the repo root:  python tests/golden/make_golden.py
-Needs /root/reference (read-only) and transformers; neither exists on the GPU box, which is why the outputs
-(small .npz files) are committed next to this script.
+Run from the repo root:  MORPHIK_REFERENCE=<a morphik-core checkout> python tests/golden/make_golden.py
+Needs that checkout and transformers, which is why the outputs (small .npz files) are committed next to this script.
 
 What is executed:
-  * /root/reference/core/utils/fast_ops.py (loaded by file path; HAS_RUST is False here so the authoritative
+  * core/utils/fast_ops.py of the checkout (loaded by file path; HAS_RUST is False here so the authoritative
     pure-Python fallbacks run): binary_quantize, binary_quantize_packed, hamming_distance(_batch).
   * transformers.models.colpali.processing_colpali.ColPaliProcessor.score_retrieval -- the port of
     colpali_engine v0.3.13 ``score_multi_vector`` that the reference calls at
@@ -19,7 +18,7 @@ import os
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("MORPHIK_REFERENCE", "")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -97,7 +96,9 @@ def gen_float_maxsim():
                                                        output_dtype=torch.float32)[0] for q in qe])
     out.update(e_rows=torch.cat(pe).numpy(), e_lens=np.array(lens_e), e_cand=cand_e.astype(np.int64), e_q0=qe[0].numpy(),
                e_q1=qe[1].numpy(), e_scores=se.numpy())
-    np.savez_compressed(os.path.join(OUT, "float_maxsim.npz"), **out)
+    # split by case so that no fixture file exceeds 1 MB
+    for name, cases in (("float_maxsim.npz", "abc"), ("float_maxsim_d.npz", "d"), ("float_maxsim_e.npz", "e")):
+        np.savez_compressed(os.path.join(OUT, name), **{k: v for k, v in out.items() if k[0] in cases})
 
 
 def gen_binary_known_answers():

@@ -76,15 +76,17 @@ def test_fails_loudly_without_gpu():
     assert nat.lib.b200ms_set_corpus(None, None, nat.BF16, None, 0) == -1
 
 
-def test_sass_has_blackwell_tensor_and_tma_instructions():
-    """Static evidence that the hot kernel is tcgen05 + TMA code (B200_PROFILING.md 'What proves a Blackwell-native kernel')."""
+def test_sass_has_hopper_tensor_and_tma_instructions():
+    """Static evidence that the hot kernels are sm_90a warpgroup-MMA + TMA code: bf16, int8 and f16 (the widened e4m3 corpora) wgmma,
+    TMA loads."""
     from morphik_core_b200 import _native as nat
 
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", nat.LIB_PATH], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTCIMMA", "LDTM", "UTMALDG", "FMNMX3", "POPC"):
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "IGMMA.64x128x32.S8.S8", "HGMMA.64x128x16.F32 ", "HGMMA.64x64x16",
+                     "UTMALDG", "POPC"):
         assert mnemonic in sass, mnemonic
     assert "HMMA.16816" not in sass  # no legacy mma.sync path
 
@@ -112,7 +114,7 @@ def test_every_named_option_is_documented_in_the_header():
     body = api[api.index("B200MS_API int b200ms_set_option"):]
     body = body[:body.index("\n}\n")]
     names = set(re.findall(r'n == "([a-z0-9_]+)"', body))
-    assert {"pair_cta", "b1_tensor", "rowm", "zero_pad_compat"} <= names
+    assert {"b1_tensor", "fde_gemm", "zero_pad_compat"} <= names
     header = open(os.path.join(ROOT, "include", "b200ms.h")).read()
     missing = sorted(n for n in names if f'"{n}"' not in header)
     assert not missing, f"options without a line in include/b200ms.h: {missing}"

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path, called through the C-ABI (ctypes), against the oracle.
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C-ABI (ctypes), against the oracle.
 
 Bars (SURVEY 8d "Parity gates"): sign bits / Hamming / int8 bit-exact; bf16 scores within 1e-3 relative of the fp32
 oracle evaluated on the same bf16-rounded inputs (measured: ~1e-6); top-k id lists identical to the oracle's
@@ -108,7 +108,7 @@ def test_bf16_config0_shape_single_query():
 
 
 def test_bf16_golden_fixture_from_score_multi_vector(golden_dir):
-    fm = np.load(os.path.join(golden_dir, "float_maxsim.npz"))
+    fm = {k: v for f in ("float_maxsim.npz", "float_maxsim_d.npz", "float_maxsim_e.npz") for k, v in np.load(os.path.join(golden_dir, f)).items()}
     # case D is bf16-valued (what ColQwen emits), so bf16 storage is lossless and the port's scores are the target
     idx = MaxSimIndex(dtype="bf16")
     idx.add_pages(list(fm["d_pages"]))
@@ -141,8 +141,8 @@ def test_bf16_ragged_pages_empty_pages_unit_boundaries(unit_rows_):
 
 @pytest.mark.parametrize("dtype", ["bf16", "int8"])
 def test_one_cta_forms_match_oracle(dtype):
-    """pair_cta = 0 (what a partition without whole TPCs falls back to): NM = 1 / 2 two-warpgroup kernel and the NM = 4 / 8
-    four-warpgroup kernel against the oracle -- bf16 within rounding, int8 bit-exact."""
+    """NM = 1 / 2 / 4 / 8 resident query tiles (one and two busy consumer warpgroups) and a second pass over the corpus
+    against the oracle -- bf16 within rounding, int8 bit-exact."""
     rng = np.random.default_rng(808)
     lens = [1, 33, 0, 64, 700, 1030, 2] + list(rng.integers(1, 300, size=50))
     pages = make_pages(rng, lens)
@@ -150,7 +150,7 @@ def test_one_cta_forms_match_oracle(dtype):
     off = orc.page_offsets(lens)
     for n_q in (1, 5, 13, 32, 40):  # 1, 2, 4, 8 (int8: NM=8), 10 query tiles
         queries = [unit_rows(rng, 32 if i % 2 else 29) for i in range(n_q)]
-        a = MaxSimIndex(dtype=dtype); a.set_option("pair_cta", 0); a.set_option("unit_rows", 400); a.add_pages(pages)
+        a = MaxSimIndex(dtype=dtype); a.set_option("unit_rows", 400); a.add_pages(pages)
         got = a.score_matrix(queries)
         if dtype == "bf16":
             assert_close_rel(got, oracle_float(queries, pages), 3e-5)
@@ -163,40 +163,51 @@ def test_one_cta_forms_match_oracle(dtype):
 @pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8"])
 @pytest.mark.parametrize("unit_rows_,n_pages", [(400, 57), (64, 9), (4096, 3), (400, 1)])
 def test_cta_pair_form_agrees(dtype, unit_rows_, n_pages):
-    """The CTA-pair kernel (tcgen05 cta_group::2, two unit streams per pair) is bit-identical to the one-CTA kernels:
-    odd/even unit counts, fewer units than CTAs, a single page, phantom query tiles, int8 with NM = 8."""
+    """One CTA walking every unit (persistent loop, stage ring wrap) is bit-identical to the full grid: odd/even unit counts,
+    fewer units than CTAs, a single page, phantom query tiles, int8 with NM = 8; both against the oracle of the dtype.
+    (The name dates from a CTA-pair kernel; the same edge cases are checked here.)"""
     rng = np.random.default_rng(909 + n_pages)
     lens = ([1, 33, 0, 64, 700, 1030, 2] + list(rng.integers(1, 300, size=50)))[:n_pages]
     pages = make_pages(rng, lens)
-    for n_q in (5, 9, 13, 32, 40, 70):  # 2 (pair_cta = 2 only), 3, 4, 8, 10, 18 query tiles
+    for n_q in (5, 9, 13, 32, 40, 70):  # 2, 3, 4, 8, 10, 18 query tiles
         queries = [unit_rows(rng, 32 if i % 2 else 29) for i in range(n_q)]
-        a = MaxSimIndex(dtype=dtype); a.set_option("pair_cta", 2); a.set_option("unit_rows", unit_rows_); a.add_pages(pages)
-        b = MaxSimIndex(dtype=dtype); b.set_option("pair_cta", 0); b.set_option("unit_rows", unit_rows_); b.add_pages(pages)
+        a = MaxSimIndex(dtype=dtype); a.set_option("unit_rows", unit_rows_); a.add_pages(pages)
+        b = MaxSimIndex(dtype=dtype); b.set_option("unit_rows", unit_rows_); b.set_option("max_ctas", 1); b.add_pages(pages)
         ga, gb = a.score_matrix(queries), b.score_matrix(queries)
         assert np.array_equal(ga, gb), (dtype, n_q, np.abs(ga - gb).max())
-        if dtype == "bf16" and n_q == 13:
-            assert_close_rel(ga, oracle_float(queries, pages), 3e-5)
+        if n_q in (13, 70):  # one pass of 4 resident tiles, and several passes
+            if dtype == "bf16":
+                assert_close_rel(ga, oracle_float(queries, pages), 3e-5)
+            elif dtype == "fp8":
+                assert_close_rel(ga, oracle_fp8(queries, pages), 1e-4)
+            else:
+                rows = np.concatenate(pages)
+                rq, off = orc.quantize_int8_np(rows, 127.0), orc.page_offsets(lens)
+                want = np.stack([orc.int8_maxsim_c(orc.quantize_int8_np(q, 127.0), rq, off) for q in queries])
+                assert np.array_equal(np.rint(ga * 127.0 * 127.0).astype(np.int64), want), n_q
 
 
 @pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8", "binary"])
 @pytest.mark.parametrize("unit_rows_,n_pages", [(400, 70), (64, 9), (4096, 70), (400, 1), (0, 400)])
 def test_rows_as_m_kernel_is_bit_identical_to_query_as_m(dtype, unit_rows_, n_pages):
-    """maxsim_rowm_kernel (lone query: patch rows = M operand, four epilogue warps, cross-warp page combine in shared memory)
-    against the query-as-M kernels it replaces for scans of <= 2 query groups: 1 and 2 groups, short last groups, pages of
-    1 .. 1030 rows (pages inside one chunk, pages crossing tiles and units), empty pages, one page only, more units than SMs."""
+    """Scans of <= 2 query groups (one busy consumer warpgroup) under a given unit size against one CTA walking the default
+    units (1-bit: against the POPC kernel, an independent formulation): 1 and 2 groups, short last groups, pages of
+    1 .. 1030 rows (pages inside one chunk, pages crossing tiles and units), empty pages, one page only, more units than SMs;
+    bf16, int8 and fp8 also against the oracle.  (The name dates from a rows-as-M kernel; the same edge cases are checked.)"""
     rng = np.random.default_rng(1234 + n_pages)
     base = [1, 31, 32, 33, 0, 64, 127, 128, 129, 5, 700, 1030, 0, 2, 96, 255, 256, 257, 40, 1]
     lens = (base + list(rng.integers(1, 300, size=400)))[:n_pages] if n_pages > 1 else [333]
     if n_pages == 400:
         lens = list(rng.integers(1, 1100, size=400))
     pages = make_pages(rng, lens)
-    a = MaxSimIndex(dtype=dtype); a.set_option("rowm", 1)
-    b = MaxSimIndex(dtype=dtype); b.set_option("rowm", 0)
+    a = MaxSimIndex(dtype=dtype)
+    b = MaxSimIndex(dtype=dtype); b.set_option("max_ctas", 1)
     if dtype == "binary":
+        a.set_option("b1_tensor", 1)  # the wgmma kernel (the default sends one or two groups to POPC)
         b.set_option("b1_tensor", 0)  # the POPC kernel: an independent formulation
+    if unit_rows_:
+        a.set_option("unit_rows", unit_rows_)
     for ix in (a, b):
-        if unit_rows_:
-            ix.set_option("unit_rows", unit_rows_)
         ix.add_pages(pages)
     for qs in ([unit_rows(rng, 32)], [unit_rows(rng, 7)], [-np.abs(unit_rows(rng, 20))], [unit_rows(rng, 64)],
                [unit_rows(rng, 45)], [unit_rows(rng, 32), unit_rows(rng, 3)]):
@@ -211,34 +222,50 @@ def test_rows_as_m_kernel_is_bit_identical_to_query_as_m(dtype, unit_rows_, n_pa
             ix.set_option("zero_pad_compat", 16)
         q1 = [-np.abs(unit_rows(rng, 20))]
         assert np.array_equal(a.score_matrix(q1), b.score_matrix(q1))
+    elif dtype == "fp8":
+        qs = [unit_rows(rng, 32), unit_rows(rng, 30)]
+        assert_close_rel(a.score_matrix(qs), oracle_fp8(qs, pages), 1e-4)
+    elif dtype == "int8":
+        qs = [unit_rows(rng, 32), unit_rows(rng, 30)]
+        rq, off = orc.quantize_int8_np(np.concatenate(pages), 127.0), orc.page_offsets([len(p) for p in pages])
+        want = np.stack([orc.int8_maxsim_c(orc.quantize_int8_np(q, 127.0), rq, off) for q in qs])
+        assert np.array_equal(np.rint(a.score_matrix(qs) * 127.0 * 127.0).astype(np.int64), want)
 
 
 @pytest.mark.parametrize("dtype", ["bf16", "binary"])
 def test_rows_as_m_kernel_flushes_finished_pages_early(dtype):
-    """One CTA, 64-row work units: a 128-row page gives lane quadrants 2 and 3 a partial maximum, then 400 pages of <= 64 rows
-    follow whose tiles only fill quadrants 0 and 1 -- those warps must hand the finished page over at the next block, not at
-    their next chunk (which never comes), or the 128-slot page table wraps around under them."""
+    """One CTA, 64-row work units: a 128-row page, then 400 pages of <= 64 rows (several page ends inside one 128-row tile,
+    tiles that straddle units), then more of both -- every finished page must be written exactly once with its own maximum.
+    1-bit: against the POPC kernel; bf16: against the oracle."""
     rng = np.random.default_rng(99)
     lens = [128] + [int(x) for x in rng.integers(33, 65, size=400)] + [128] + [40] * 300
     pages = make_pages(rng, lens)
-    a = MaxSimIndex(dtype=dtype); a.set_option("rowm", 1)
-    b = MaxSimIndex(dtype=dtype); b.set_option("rowm", 0)
+    a = MaxSimIndex(dtype=dtype)
     if dtype == "binary":
+        a.set_option("b1_tensor", 1)
+    a.set_tuning(unit_rows=64, max_ctas=1)
+    a.add_pages(pages)
+    b = None
+    if dtype == "binary":
+        b = MaxSimIndex(dtype=dtype)
         b.set_option("b1_tensor", 0)
-    for ix in (a, b):
-        ix.set_tuning(unit_rows=64, max_ctas=1)
-        ix.add_pages(pages)
+        b.set_tuning(unit_rows=64, max_ctas=1)
+        b.add_pages(pages)
     for qs in ([unit_rows(rng, 32)], [unit_rows(rng, 9)]):
-        ga, gb = a.score_matrix(qs), b.score_matrix(qs)
-        assert np.array_equal(ga, gb), (dtype, np.argwhere(ga != gb)[:5])
+        ga = a.score_matrix(qs)
+        if b is not None:
+            gb = b.score_matrix(qs)
+            assert np.array_equal(ga, gb), (dtype, np.argwhere(ga != gb)[:5])
+        else:
+            assert_close_rel(ga, oracle_float(qs, pages), 3e-5)
 
 
 def test_rows_as_m_kernel_binary_matches_oracle_on_uniform_pages():
-    """1024-row pages (the BASELINE shape): every page spans 8 tiles and all four epilogue warps; exact integers."""
+    """1024-row pages (the BASELINE shape), one query group on the wgmma kernel: every page spans 8 tiles; exact integers."""
     rng = np.random.default_rng(77)
     lens = [1024] * 300
     pages = make_pages(rng, lens)
-    idx = MaxSimIndex(dtype="binary"); idx.add_pages(pages)
+    idx = MaxSimIndex(dtype="binary"); idx.set_option("b1_tensor", 1); idx.add_pages(pages)
     q = [unit_rows(rng, 32)]
     got = idx.score_matrix(q)
     want, _ = orc.binary_maxsim_c(orc.sign_pack_c(q[0]), orc.sign_pack_c(np.concatenate(pages)), orc.page_offsets(lens))
@@ -246,13 +273,13 @@ def test_rows_as_m_kernel_binary_matches_oracle_on_uniform_pages():
 
 
 def test_cta_pair_form_large_and_topk():
-    """Pair kernel on a corpus that gives every pair many units (persistent loop, stage ring wrap, dummy tail tiles)."""
+    """A corpus that gives every CTA many units (persistent loop, stage ring wrap) against one CTA walking all of them."""
     rng = np.random.default_rng(4242)
     lens = list(rng.integers(900, 1100, size=700))
     pages = make_pages(rng, lens)
     queries = [unit_rows(rng, 32) for _ in range(32)]
-    a = MaxSimIndex(dtype="bf16"); a.set_option("pair_cta", 1); a.add_pages(pages)
-    b = MaxSimIndex(dtype="bf16"); b.set_option("pair_cta", 0); b.add_pages(pages)
+    a = MaxSimIndex(dtype="bf16"); a.add_pages(pages)
+    b = MaxSimIndex(dtype="bf16"); b.set_option("max_ctas", 1); b.add_pages(pages)
     assert np.array_equal(a.score_matrix(queries), b.score_matrix(queries))
     ta, tb = a.search_host(queries, k=10), b.search_host(queries, k=10)
     assert np.array_equal(ta[1], tb[1]) and np.array_equal(ta[0], tb[0])
@@ -331,7 +358,7 @@ def test_binary_known_answers_from_reference_tests(golden_dir):
         assert ti[0][0] == j and ts[0][0] == 3.0 and np.all(np.diff(ts[0]) <= 0)
 
 
-@pytest.mark.parametrize("path", [0, 1, 2])  # 0 = POPC kernel, 1 = tcgen05 kernel (incl. the replicated-query form), 2 = auto
+@pytest.mark.parametrize("path", [0, 1, 2])  # 0 = POPC kernel, 1 = wgmma kernel, 2 = auto by group count
 @pytest.mark.parametrize("n_q", [1, 3, 8, 13])
 def test_binary_bit_exact(n_q, path):
     rng = np.random.default_rng(50 + n_q)
@@ -543,8 +570,9 @@ def oracle_fp8(queries, pages, scale=64.0):
 
 @pytest.mark.parametrize("n_q", [1, 5, 13, 40])
 def test_fp8_matches_oracle(n_q):
-    """B200MS_F8: e4m3(x * 64) rows and queries, tcgen05 kind::f8f6f4 with fp32 accumulation.  The packed bytes equal the
-    oracle's round-to-nearest-even e4m3 codes; scores match the oracle's fp32 MaxSim of the dequantised values."""
+    """B200MS_F8: e4m3(x * 64) rows and queries, widened to f16 in shared memory (exact) and multiplied with wgmma .f16 into
+    fp32 accumulators.  The packed bytes equal the oracle's round-to-nearest-even e4m3 codes; scores match the oracle's fp32
+    MaxSim of the dequantised values."""
     rng = np.random.default_rng(300 + n_q)
     lens = [1, 33, 0, 64, 200, 1024, 17, 96] + list(rng.integers(1, 260, size=30))
     pages = make_pages(rng, lens)
@@ -579,7 +607,7 @@ def test_zero_pad_compat_matches_score_multi_vector_golden(golden_dir, case, bat
     """Product option zero_pad_compat=<batch size> reproduces colpali_engine score_multi_vector's padding quirk (a page
     shorter than the longest of its batch scores max(true, 0) per token): golden cases B (one 128-batch) and C
     (batch_size=3) were produced by the transformers port of score_multi_vector (tests/golden/make_golden.py)."""
-    fm = np.load(os.path.join(golden_dir, "float_maxsim.npz"))
+    fm = {k: v for f in ("float_maxsim.npz", "float_maxsim_d.npz", "float_maxsim_e.npz") for k, v in np.load(os.path.join(golden_dir, f)).items()}
     lens = fm["b_lens"].tolist()
     off = orc.page_offsets(lens)
     pages = [fm["b_rows"][off[i]:off[i + 1]] for i in range(len(lens))]
@@ -593,13 +621,13 @@ def test_zero_pad_compat_matches_score_multi_vector_golden(golden_dir, case, bat
     # the quirk is visible: the all-negative query's clean MaxSim differs on the short pages
     clean = MaxSimIndex(dtype="bf16"); clean.add_pages(pages)
     assert np.abs(clean.score_matrix(queries)[0] - want[0]).max() > 0.1
-    # and against the oracle's own switch on bf16-rounded inputs (tight tolerance), batches of queries too (pair kernel)
+    # and against the oracle's own switch on bf16-rounded inputs (tight tolerance), batches of queries too
     many = queries + [unit_rows(np.random.default_rng(5), 32) * (-1 if i % 2 else 1) for i in range(11)]
     rr = orc.bf16_round_np(fm["b_rows"])
     want2 = np.stack([orc.float_maxsim_c(orc.bf16_round_np(q), rr, off, zero_pad_compat=True, batch=batch) for q in many])
     assert_close_rel(idx.score_matrix(many), want2, 3e-5)
-    for pc in (0, 2):  # one-CTA and CTA-pair forms agree bit for bit
-        alt = MaxSimIndex(dtype="bf16"); alt.set_option("zero_pad_compat", batch); alt.set_option("pair_cta", pc); alt.add_pages(pages)
+    for mc in (1, 3):  # narrower grids agree bit for bit
+        alt = MaxSimIndex(dtype="bf16"); alt.set_option("zero_pad_compat", batch); alt.set_option("max_ctas", mc); alt.add_pages(pages)
         assert np.array_equal(alt.score_matrix(many), idx.score_matrix(many))
 
 
@@ -634,7 +662,7 @@ def test_zero_pad_compat_rerank_batches_candidates_like_the_reference():
 def test_zero_pad_compat_rerank_matches_port_golden(golden_dir):
     """Golden case E (produced by the transformers port of score_multi_vector): the reference's rerank call, candidates in
     first-stage order -- b200ms_rerank_batch_device with zero_pad_compat=128 returns the port's scores and ranking."""
-    fm = np.load(os.path.join(golden_dir, "float_maxsim.npz"))
+    fm = {k: v for f in ("float_maxsim.npz", "float_maxsim_d.npz", "float_maxsim_e.npz") for k, v in np.load(os.path.join(golden_dir, f)).items()}
     lens = fm["e_lens"].tolist()
     off = orc.page_offsets(lens)
     pages = [fm["e_rows"][off[i]:off[i + 1]] for i in range(len(lens))]

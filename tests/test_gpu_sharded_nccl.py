@@ -1,4 +1,4 @@
-"""2-GPU (NCCL) test of the document-sharded search: every rank scans only its shard on its own B200, one all-gather of
+"""2-GPU (NCCL) test of the document-sharded search: every rank scans only its shard on its own GPU, one all-gather of
 the per-shard top-k, merge on the device -- and every rank must end up with the oracle's global top-k.
 Skipped on boxes with fewer than 2 GPUs (the host logic is covered on CPU by tests/test_sharded_gloo.py)."""
 import os

@@ -20,7 +20,7 @@ def sp(golden_dir):
 
 @pytest.fixture(scope="module")
 def fm(golden_dir):
-    return np.load(os.path.join(golden_dir, "float_maxsim.npz"))
+    return {k: v for f in ("float_maxsim.npz", "float_maxsim_d.npz", "float_maxsim_e.npz") for k, v in np.load(os.path.join(golden_dir, f)).items()}
 
 
 def test_sign_pack_matches_reference_fast_ops(sp):

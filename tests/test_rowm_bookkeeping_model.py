@@ -1,7 +1,9 @@
-"""CPU model of the page bookkeeping of maxsim_rowm_kernel's epilogue (morphik-core_b200/csrc/maxsim_rowm.cu).
+"""CPU model of the page bookkeeping of a rows-as-M MaxSim epilogue (patch rows as the MMA M operand, eight epilogue warps
+that each see one chunk of a tile and meet in a page-slot table).
 
-The CUDA kernel is tested on the GPU against the oracle (tests/test_gpu_parity.py::test_rows_as_m_*).  This file pins the
-ALGORITHM its eight epilogue warps run -- independent of CUDA -- so that a change of the invariants shows up on a CPU box:
+This file guards no shipped code: the CUDA kernel (maxsim_wgmma.cu) holds whole query groups per warp and has no slot table.
+It pins the ALGORITHM of the rows-as-M design -- a pure-Python model, independent of CUDA -- for anyone who brings that
+orientation back (it pays off where the MMA's smallest M is larger than one query's 32 tokens).  Its invariants:
 
   * every 8-tile block, a warp derives from two 32-bit masks (chunk exists / chunk starts a page) the ordinal of each page
     in the CTA's page sequence and the extent [start, end) of the page it is accumulating -- no page_start lookups;

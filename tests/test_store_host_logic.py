@@ -256,65 +256,3 @@ def test_batch_query_mask_search_and_chunks_are_one_critical_section():
         stop.set()
         t.join()
     assert idx.bad == 0
-
-
-@pytest.mark.skipif(not __import__("os").path.exists("/root/reference/core/vector_store/dual_multivector_store.py"),
-                    reason="needs the reference checkout (build container only)")
-def test_reference_dual_multivector_store_runs_unmodified_over_this_store():
-    """SURVEY row a-11: the reference's own DualMultiVectorStore (core/vector_store/dual_multivector_store.py), executed
-    unmodified, with two B200MultiVectorStore instances as its fast / slow members.  Only its sibling imports -- the Postgres and
-    Turbopuffer stores, which need psycopg / turbopuffer -- are replaced by empty placeholder classes (they are used as type
-    annotations there); every method the dual store calls on its members is this repo's."""
-    import importlib.util
-    import sys
-    import types
-
-    ref = "/root/reference"
-    saved = {k: sys.modules.get(k) for k in ("core", "core.vector_store", "core.vector_store.base_vector_store",
-                                             "core.vector_store.fast_multivector_store", "core.vector_store.multi_vector_store",
-                                             "core.models", "core.models.chunk", "core.vector_store.dual_multivector_store")}
-    try:
-        def load(name, path, is_pkg=False):
-            spec = importlib.util.spec_from_file_location(name, path, submodule_search_locations=[path.rsplit("/", 1)[0]] if is_pkg else None)
-            mod = importlib.util.module_from_spec(spec)
-            sys.modules[name] = mod
-            spec.loader.exec_module(mod)
-            return mod
-
-        for pkg in ("core", "core.vector_store", "core.models"):
-            m = types.ModuleType(pkg)
-            m.__path__ = [f"{ref}/{pkg.replace('.', '/')}"]
-            sys.modules[pkg] = m
-        load("core.models.chunk", f"{ref}/core/models/chunk.py")
-        load("core.vector_store.base_vector_store", f"{ref}/core/vector_store/base_vector_store.py")
-        for name, cls in (("fast_multivector_store", "FastMultiVectorStore"), ("multi_vector_store", "MultiVectorStore")):
-            stub = types.ModuleType(f"core.vector_store.{name}")
-            setattr(stub, cls, type(cls, (), {}))
-            sys.modules[f"core.vector_store.{name}"] = stub
-        dual_mod = load("core.vector_store.dual_multivector_store", f"{ref}/core/vector_store/dual_multivector_store.py")
-        RefChunk = sys.modules["core.models.chunk"].DocumentChunk
-
-        fast = B200MultiVectorStore(index=OracleIndex(), mode="binary", auto_initialize=False, uri="b200://fast")
-        slow = B200MultiVectorStore(index=OracleIndex(), mode="binary", auto_initialize=False, uri="b200://slow", storage="the-storage")
-        dual = dual_mod.DualMultiVectorStore(fast_store=fast, slow_store=slow)
-        assert dual.initialize() is True and dual.uri == "b200://slow" and dual.storage == "the-storage"
-        rng = np.random.default_rng(8)
-        chunks = [RefChunk(document_id=f"d{i // 2}", content=f"c{i}", embedding=rng.standard_normal((3, 128)).astype(np.float32),
-                           chunk_number=i % 2, metadata={"i": i}) for i in range(8)]
-        ok, ids, metrics = run(dual.store_embeddings(chunks, app_id="app"))
-        assert ok and ids == [f"d{i // 2}-{i % 2}" for i in range(8)] and metrics["mode"] == "dual" and {"fast", "slow"} <= set(metrics)
-        assert len(fast.catalog) == len(slow.catalog) == 8
-        res = run(dual.query_similar(chunks[5].embedding, 3, None, "app"))
-        assert (res[0].document_id, res[0].chunk_number) == ("d2", 1) and res[0].metadata == {"i": 5}
-        got = run(dual.get_chunks_by_id([("d1", 0), ("zz", 0)], "app"))
-        assert [(c.document_id, c.chunk_number) for c in got] == [("d1", 0)]
-        assert run(dual.delete_chunks_by_document_id("d2", "app")) is True
-        assert fast.catalog.pages_of("d2") == [] and slow.catalog.pages_of("d2") == []
-        assert all(r.document_id != "d2" for r in run(dual.query_similar(chunks[5].embedding, 8, None, "app")))
-        dual.close()
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v

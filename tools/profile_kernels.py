@@ -2,11 +2,11 @@
 
 Builds a synthetic shard (default 32768 pages x 1024 x 128, 8.6 GB bf16) and launches each scoring kernel a few times
 in a fixed order so that `ncu -k regex:<name> -s <skip> -c <count>` picks a warm launch:
-  (default)     bf16: 4x bq=32 (maxsim_umma_pair<0,4>), then 4x bq=1 (maxsim_umma<0,1>)
-  --only int8   int8 sub-shard: 4x bq=32 (maxsim_umma_pair<1,4>), 4x bq=1
+  (default)     bf16: 4x bq=32 (maxsim_wgmma<0,4>), then 4x bq=1 (maxsim_wgmma<0,1>)
+  --only int8   int8 sub-shard: 4x bq=32 (maxsim_wgmma<1,4>), 4x bq=1
   --only fp8    fp8 sub-shard, same
-  --only binary 1-bit sub-shard: 4x bq=8 (tcgen05 path), 4x bq=1 (POPC path)
-  --only fde    FDE matrix of the shard: 4x scan with 1 query, 4x with 32 queries (fde_scan_umma_kernel)
+  --only binary 1-bit sub-shard: 4x bq=8 (wgmma path), 4x bq=1 (POPC path)
+  --only fde    FDE matrix of the shard: 4x scan with 1 query, 4x with 32 queries (fde_scan_wgmma_kernel)
 """
 import argparse
 import os

@@ -1,10 +1,10 @@
-"""A/B timing of the scoring kernels, CUDA events, outside any profiler (developer aid; not a bench.py leg).
+"""Timing of the scoring kernels, CUDA events, outside any profiler (developer aid; not a bench.py leg).
 
-  python tools/time_scan.py [--pages 65536] [--dtypes bf16,int8,fp8] [--variants base,exact,...]
+  python tools/time_scan.py [--pages 65536] [--dtypes bf16,int8,fp8] [--b1-groups 1,2,3,4,8]
 
-With --variants it re-runs itself once per morphik-core_b200/lib/ab/libb200ms_<name>.so (tools/build_variants.py) with
-B200MS_LIB set, so every variant is timed in a fresh process on the same box.  Prints one JSON line per run:
-scoring-kernel ms and GB/s for ONE 32-token query, ms for a 32-query batch.
+Prints one JSON line: the GPU's name and power limit, scoring-kernel ms and GB/s for ONE 32-token query and ms for a
+32-query batch per dtype, and with --b1-groups the 1-bit full-scan ms on the POPC kernel (b1_tensor 0) and on the wgmma
+kernel (b1_tensor 1) for each number of 32-token query groups -- the measurement behind the b1_tensor = 2 crossover.
 """
 import argparse
 import json
@@ -18,20 +18,9 @@ sys.path.insert(0, ROOT)
 ap = argparse.ArgumentParser()
 ap.add_argument("--pages", type=int, default=65536)
 ap.add_argument("--dtypes", default="bf16,int8,fp8")
-ap.add_argument("--variants", default="")
+ap.add_argument("--b1-groups", default="", help="comma-separated query-group counts for the 1-bit POPC / wgmma comparison")
 ap.add_argument("--steps", type=int, default=30)
 args = ap.parse_args()
-
-if args.variants:
-    for name in args.variants.split(","):
-        env = dict(os.environ)
-        if name != "product":
-            env["B200MS_LIB"] = os.path.join(ROOT, "morphik-core_b200", "lib", "ab", f"libb200ms_{name}.so")
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--pages", str(args.pages), "--dtypes", args.dtypes,
-                            "--steps", str(args.steps)], env=env, capture_output=True, text=True, timeout=600)
-        line = r.stdout.strip().splitlines()[-1] if r.stdout.strip() else json.dumps({"error": r.stderr[-400:]})
-        print(json.dumps({"variant": name, **json.loads(line)}), flush=True)
-    raise SystemExit(0)
 
 import torch  # noqa: E402
 
@@ -42,8 +31,10 @@ dev = torch.device("cuda", 0)
 q_host = bench.make_queries(32)
 packed, _ = bench.build_shard(args.pages, dev, 1234, q_host)
 q_dev = q_host.to(dev)
-out = {"pages": args.pages}
-for dt in args.dtypes.split(","):
+gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                     text=True).stdout.strip()
+out = {"gpu": gpu, "pages": args.pages}
+for dt in [d for d in args.dtypes.split(",") if d]:
     if dt == "bf16":
         idx = MaxSimIndex(device=0, dtype="bf16")
         idx.adopt_packed(packed, [bench.P_PATCH] * args.pages)
@@ -54,5 +45,17 @@ for dt in args.dtypes.split(","):
     _, b32 = bench.time_search(idx, q_dev, [32] * 32, 10, args.steps, 3)
     out[dt] = {"one_query_ms": round(one, 4), "one_query_gbs": round(args.pages * bench.P_PATCH * rb / one / 1e6, 1),
                "batch32_ms": round(b32, 4)}
+    idx.close()
+if args.b1_groups:
+    idx = bench.quantised_subshard(packed, args.pages, "binary", 0)
+    b1 = {}
+    for ng in [int(x) for x in args.b1_groups.split(",")]:
+        row = {}
+        for path, name in ((0, "popc_ms"), (1, "wgmma_ms")):
+            idx.set_option("b1_tensor", path)
+            _, ms = bench.time_search(idx, q_dev[: ng * 32].contiguous(), [32] * ng, 10, args.steps, 3)
+            row[name] = round(ms, 3)
+        b1[ng] = row
+    out["binary_full_scan_by_groups"] = b1
     idx.close()
 print(json.dumps(out))
