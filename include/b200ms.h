@@ -166,8 +166,9 @@ int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int src_dtype, c
                                 int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream);
 
 /* MaxSim over an explicit candidate list (the "rerank" half of a two-stage search, fast_multivector_store.py:545-557):
- * cand_ids_dev = device array of n_cand page ids (-1 = unused slot).  Only those pages are scanned; ties break towards
- * the earlier candidate slot (= better first-stage rank).  Outputs as b200ms_search_device. */
+ * cand_ids_dev = device array of n_cand page ids (-1, or any id outside [0, n_pages) = unused slot; a page may appear in
+ * several slots).  Only those pages are scanned; ties break towards the earlier candidate slot (= better first-stage rank),
+ * for every n_cand.  Outputs as b200ms_search_device. */
 int b200ms_rerank_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
                          const int64_t* cand_ids_dev, int n_cand, int k, float i8_q_scale, float score_scale,
                          float* top_scores_dev, int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream);

@@ -24,6 +24,7 @@ template <int G>
 __global__ void __launch_bounds__(kB1Warps * 32)
 maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ page_start, int64_t n_pages,
                  const int64_t* __restrict__ cand_ids /* NULL: every page; else n_pages candidates, output slot = index */,
+                 int64_t corpus_pages /* candidate ids outside [0, corpus_pages) are unused slots */,
                  const uint4* __restrict__ q_bits /*[n_groups*32]*/, const int32_t* __restrict__ group_ntok, int g_base,
                  int n_groups, int32_t* __restrict__ group_scores, int64_t ld) {
   __shared__ uint4 slab[kB1Warps][32];
@@ -47,7 +48,8 @@ maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ pag
   const int64_t warp_stride = int64_t(gridDim.x) * kB1Warps;
   for (int64_t p = warp_global; p < n_pages; p += warp_stride) {
     const int64_t pg = cand_ids ? __ldg(cand_ids + p) : p;
-    const int64_t r0 = pg >= 0 ? __ldg(page_start + pg) : 0, r1 = pg >= 0 ? __ldg(page_start + pg + 1) : 0;
+    const bool live_page = pg >= 0 && pg < corpus_pages;
+    const int64_t r0 = live_page ? __ldg(page_start + pg) : 0, r1 = live_page ? __ldg(page_start + pg + 1) : 0;
     int best[G];
 #pragma unroll
     for (int g = 0; g < G; ++g) best[g] = 129;  // min Hamming so far (129 = none)
@@ -98,16 +100,16 @@ int launch_score_b1(b200ms_t* h, const int64_t* cand_ids, int64_t n_cand, const 
   for (int base = g_lo; base < g_hi;) {
     const int rem = g_hi - base;
     if (rem >= 8) {
-      maxsim_b1_kernel<8><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<8><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 8;
     } else if (rem >= 4) {
-      maxsim_b1_kernel<4><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<4><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 4;
     } else if (rem >= 2) {
-      maxsim_b1_kernel<2><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<2><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 2;
     } else {
-      maxsim_b1_kernel<1><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<1><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 1;
     }
     h->launches++;

@@ -216,9 +216,11 @@ topk_kernel(const T* __restrict__ gs, int64_t n_pages, int64_t ld, const int32_t
     const int64_t slot = int64_t(0xffffffffu - uint32_t(w));
     const int64_t id = live ? (id_map ? __ldg(id_map + slot) : slot + id_base) : int64_t(-1);
     if (part_keys) {
+      // candidate mode hands the merge SLOTS, not page ids: ties must come out in slot order, and the merge maps the winners'
+      // slots to page ids itself
       const int64_t o = (int64_t(q) * gridDim.y + blockIdx.y) * k + i;
       part_keys[o] = uint32_t(w >> 32);
-      part_ids[o] = id;
+      part_ids[o] = (live && id_map) ? slot : id;
     } else {
       top_scores[int64_t(q) * k + i] = live ? score_of_key(uint32_t(w >> 32), T(0)) * scale : -CUDART_INF_F;
       top_ids[int64_t(q) * k + i] = id;
@@ -287,12 +289,14 @@ __device__ __forceinline__ bool cand_before(uint32_t ka, int64_t ia, uint32_t kb
 // gathered != NULL: candidates come straight from the all-gather buffer -- `world` blocks (one per rank) of
 // [n_q*kx int64 ids | n_q*kx f32 scores] (the exchange layout the local top-k is written in, include/b200ms.h); candidate
 // i of query q is entry q*kx + i%kx of rank i/kx.  No repacking kernels between the collective and the merge.
+// id_map != NULL: the candidate ids are slots of a rerank (second level of topk_kernel in candidate mode); they are ordered
+// as slots and reported as id_map[slot].
 template <typename T>
 __global__ void __launch_bounds__(1024)
 merge_topk_kernel(const float* __restrict__ cand_scores, const uint32_t* __restrict__ cand_keys,
                   const int64_t* __restrict__ cand_ids, int m, int n2, int k, float scale, float* __restrict__ top_scores,
                   int64_t* __restrict__ top_ids, int32_t* __restrict__ top_counts, const uint8_t* __restrict__ gathered,
-                  int kx, int64_t rank_stride, int64_t scores_off) {
+                  int kx, int64_t rank_stride, int64_t scores_off, const int64_t* __restrict__ id_map) {
   extern __shared__ uint8_t msm[];
   int64_t* ids = reinterpret_cast<int64_t*>(msm);
   uint32_t* keys = reinterpret_cast<uint32_t*>(ids + n2);
@@ -345,7 +349,7 @@ merge_topk_kernel(const float* __restrict__ cand_scores, const uint32_t* __restr
   for (int i = threadIdx.x; i < k; i += blockDim.x) {
     const bool live = uint32_t(i) < kk;
     top_scores[int64_t(q) * k + i] = live ? score_of_key(keys[i], T(0)) * scale : -CUDART_INF_F;
-    top_ids[int64_t(q) * k + i] = live ? ids[i] : int64_t(-1);
+    top_ids[int64_t(q) * k + i] = live ? (id_map ? __ldg(id_map + ids[i]) : ids[i]) : int64_t(-1);
   }
   if (threadIdx.x == 0) top_counts[q] = int32_t(kk);
 }
@@ -354,7 +358,7 @@ template <typename T>
 static int launch_merge_impl(b200ms_t* h, const float* cand_scores, const uint32_t* cand_keys, const int64_t* cand_ids, int n_q,
                              int m, int k, float scale, float* top_scores, int64_t* top_ids, int32_t* top_counts,
                              cudaStream_t s, const uint8_t* gathered = nullptr, int kx = 1, int64_t rank_stride = 0,
-                             int64_t scores_off = 0) {
+                             int64_t scores_off = 0, const int64_t* id_map = nullptr) {
   int n2 = 2;
   while (n2 < m) n2 <<= 1;
   const size_t smem = size_t(n2) * (sizeof(int64_t) + sizeof(uint32_t));
@@ -362,7 +366,7 @@ static int launch_merge_impl(b200ms_t* h, const float* cand_scores, const uint32
   if (int e = ensure_smem(h, reinterpret_cast<const void*>(kern), int(smem), "cudaFuncSetAttribute(merge_topk)"))
     return e;
   kern<<<n_q, 1024, smem, s>>>(cand_scores, cand_keys, cand_ids, m, n2, k, scale, top_scores, top_ids, top_counts, gathered, kx,
-                               rank_stride, scores_off);
+                               rank_stride, scores_off, id_map);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch merge_topk");
 }
@@ -420,8 +424,10 @@ int launch_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t 
   if (slices == 1) return B200MS_OK;
   const int m = int(slices) * k;
   return score_dtype == B200MS_F32
-             ? launch_merge_impl<float>(h, nullptr, part_keys, part_ids, n_q, m, k, scale, top_scores, top_ids, top_counts, s)
-             : launch_merge_impl<int>(h, nullptr, part_keys, part_ids, n_q, m, k, scale, top_scores, top_ids, top_counts, s);
+             ? launch_merge_impl<float>(h, nullptr, part_keys, part_ids, n_q, m, k, scale, top_scores, top_ids, top_counts, s,
+                                        nullptr, 1, 0, 0, id_map)
+             : launch_merge_impl<int>(h, nullptr, part_keys, part_ids, n_q, m, k, scale, top_scores, top_ids, top_counts, s,
+                                      nullptr, 1, 0, 0, id_map);
 }
 
 int launch_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand_ids, int n_q, int m, int k,

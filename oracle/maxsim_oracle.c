@@ -150,17 +150,31 @@ ORACLE_API void oracle_float_maxsim(const float* q, int n_tok, const float* rows
 /* ------------------------------------------------------------------------------------------------
  * int8 MaxSim (no reference counterpart, SURVEY F5 / 8d "bit-exact mode"): pure integer
  *   S[p] = sum_t max_s sum_d q_i8[t,d] * p_i8[s,d]      (int32 dot, int64 sum; empty page -> 0)
+ * zero_pad_compat / batch: the same switch as oracle_float_maxsim -- a page shorter than the longest page of its
+ * batch of `batch` pages (page-id order) scores sum_t max(max_s dot, 0).
  * ---------------------------------------------------------------------------------------------- */
 ORACLE_API void oracle_int8_maxsim(const int8_t* q, int n_tok, const int8_t* rows, const int64_t* page_off,
-                                   int64_t n_pages, int dim, int64_t* scores_out) {
+                                   int64_t n_pages, int dim, int zero_pad_compat, int batch, int64_t* scores_out) {
+  if (batch <= 0) batch = 128;
 #pragma omp parallel for schedule(dynamic, 4)
   for (int64_t p = 0; p < n_pages; ++p) {
     const int64_t r0 = page_off[p], r1 = page_off[p + 1];
+    int padded = 0;
+    if (zero_pad_compat) {
+      const int64_t b0 = (p / batch) * batch;
+      const int64_t b1 = (b0 + batch < n_pages) ? b0 + batch : n_pages;
+      int64_t longest = 0;
+      for (int64_t j = b0; j < b1; ++j) {
+        const int64_t len = page_off[j + 1] - page_off[j];
+        if (len > longest) longest = len;
+      }
+      padded = (r1 - r0) < longest;
+    }
     int64_t total = 0;
-    if (r1 > r0) {
+    if (r1 > r0 || padded) {
       for (int t = 0; t < n_tok; ++t) {
         const int8_t* qt = q + (int64_t)t * dim;
-        int32_t best = INT32_MIN;
+        int32_t best = padded ? 0 : INT32_MIN;
         for (int64_t r = r0; r < r1; ++r) {
           const int8_t* pr = rows + r * dim;
           int32_t acc = 0;

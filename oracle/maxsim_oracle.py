@@ -53,7 +53,7 @@ def c_oracle() -> ctypes.CDLL:
         lib.oracle_hamming.restype = ctypes.c_uint32
         lib.oracle_binary_maxsim.argtypes = [vp, i32, vp, vp, i64, i32, vp, vp]
         lib.oracle_float_maxsim.argtypes = [vp, i32, vp, vp, i64, i32, i32, i32, vp]
-        lib.oracle_int8_maxsim.argtypes = [vp, i32, vp, vp, i64, i32, vp]
+        lib.oracle_int8_maxsim.argtypes = [vp, i32, vp, vp, i64, i32, i32, i32, vp]
         lib.oracle_topk.argtypes = [vp, i64, vp, i64, vp, vp]
         lib.oracle_topk.restype = i64
         lib.oracle_fde_encode.argtypes = [vp, i64, i32, i32, i32, i32, ctypes.c_float, vp, vp, vp, i32, vp]
@@ -132,15 +132,25 @@ def float_maxsim_np(q: np.ndarray, rows: np.ndarray, off: np.ndarray, zero_pad_c
     return out
 
 
-def int8_maxsim_np(q: np.ndarray, rows: np.ndarray, off: np.ndarray) -> np.ndarray:
+def int8_maxsim_np(q: np.ndarray, rows: np.ndarray, off: np.ndarray, zero_pad_compat: bool = False,
+                   batch: int = 128) -> np.ndarray:
+    """Integer MaxSim (int64 sums); zero_pad_compat / batch as in float_maxsim_np."""
     n_pages = len(off) - 1
+    lens = np.diff(off)
     out = np.zeros(n_pages, dtype=np.int64)
     q32 = q.astype(np.int32)
     for p in range(n_pages):
         d = rows[off[p]:off[p + 1]].astype(np.int32)
-        if d.shape[0] == 0:
+        padded = False
+        if zero_pad_compat:
+            b0 = (p // batch) * batch
+            padded = lens[p] < lens[b0:b0 + batch].max()
+        if d.shape[0] == 0 and not padded:
             continue
-        out[p] = (q32 @ d.T).max(axis=1).sum()
+        best = (q32 @ d.T).max(axis=1) if d.shape[0] else np.zeros(q.shape[0], dtype=np.int64)
+        if padded:
+            best = np.maximum(best, 0)
+        out[p] = best.astype(np.int64).sum()
     return out
 
 
@@ -206,13 +216,15 @@ def float_maxsim_c(q: np.ndarray, rows: np.ndarray, off: np.ndarray, zero_pad_co
     return out
 
 
-def int8_maxsim_c(q: np.ndarray, rows: np.ndarray, off: np.ndarray) -> np.ndarray:
+def int8_maxsim_c(q: np.ndarray, rows: np.ndarray, off: np.ndarray, zero_pad_compat: bool = False,
+                  batch: int = 128) -> np.ndarray:
     q = np.ascontiguousarray(q, dtype=np.int8)
     rows = np.ascontiguousarray(rows, dtype=np.int8)
     off = np.ascontiguousarray(off, dtype=np.int64)
     n_pages = len(off) - 1
     out = np.zeros(n_pages, dtype=np.int64)
-    c_oracle().oracle_int8_maxsim(_ptr(q), q.shape[0], _ptr(rows), _ptr(off), n_pages, q.shape[1], _ptr(out))
+    c_oracle().oracle_int8_maxsim(_ptr(q), q.shape[0], _ptr(rows), _ptr(off), n_pages, q.shape[1],
+                                  int(zero_pad_compat), batch, _ptr(out))
     return out
 
 

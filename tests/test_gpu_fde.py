@@ -16,6 +16,7 @@ if not torch.cuda.is_available():  # pragma: no cover
 from morphik_core_b200 import fde  # noqa: E402
 from morphik_core_b200.index import MaxSimIndex  # noqa: E402
 from oracle import maxsim_oracle as orc  # noqa: E402
+from oracle.scoring import oracle_scores  # noqa: E402
 
 
 def unit_rows(rng, n):
@@ -74,7 +75,7 @@ def test_fde_dot_approximates_chamfer():
     assert len(rel & set(np.argsort(-approx)[:30].tolist())) >= 8
 
 
-@pytest.mark.parametrize("dtype", ["bf16", "int8", "binary"])
+@pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8", "binary"])
 def test_two_stage_search_matches_oracle_on_candidates(dtype):
     rng = np.random.default_rng(5)
     lens = [int(x) for x in rng.integers(20, 200, size=300)]
@@ -108,16 +109,11 @@ def test_two_stage_search_matches_oracle_on_candidates(dtype):
     rows = np.concatenate(pages)
     off = orc.page_offsets(lens)
     for qi, q in enumerate(queries):
-        if dtype == "bf16":
-            full = orc.float_maxsim_c(orc.bf16_round_np(q), orc.bf16_round_np(rows), off).astype(np.float64)
-        elif dtype == "int8":
-            full = orc.int8_maxsim_c(orc.quantize_int8_np(q, 127.0), orc.quantize_int8_np(rows, 127.0), off) / (127.0 * 127.0)
-        else:
-            full = orc.binary_maxsim_c(orc.sign_pack_c(q), orc.sign_pack_c(rows), off)[0]
+        full = oracle_scores(dtype, [q], pages)[0]
         cs = full[cand[qi]]
         order = np.lexsort((np.arange(n_cand), -cs))[:k]
         assert got_i[qi].tolist() == cand[qi][order].tolist(), (dtype, qi)
-        np.testing.assert_allclose(got_s[qi], cs[order], rtol=3e-5)
+        np.testing.assert_allclose(got_s[qi], cs[order], rtol=1e-4 if dtype == "fp8" else 3e-5)
         # (iv) the planted pages are found through the two stages
         planted = {17 * (qi + 1) + 31 * j for j in range(6)}
         assert len(planted & set(got_i[qi].tolist())) >= 4

@@ -18,6 +18,7 @@ if not torch.cuda.is_available():  # pragma: no cover - the gpu marker normally 
 from morphik_core_b200 import _native as nat  # noqa: E402
 from morphik_core_b200.index import MaxSimIndex  # noqa: E402
 from oracle import maxsim_oracle as orc  # noqa: E402
+from oracle.scoring import assert_candidate_ranking, oracle_scores, slot_scores_of  # noqa: E402
 
 BF16_RTOL = 1e-3  # north-star tolerance for bf16 storage
 
@@ -32,10 +33,10 @@ def make_pages(rng, lens):
 
 
 def oracle_float(queries, pages, bf16=True):
+    if bf16:
+        return oracle_scores("bf16", queries, pages)
     rows = np.concatenate(pages) if sum(len(p) for p in pages) else np.zeros((0, 128), np.float32)
-    off = orc.page_offsets([len(p) for p in pages])
-    rr = orc.bf16_round_np(rows) if bf16 else rows
-    return np.stack([orc.float_maxsim_c(orc.bf16_round_np(q) if bf16 else q, rr, off) for q in queries])
+    return np.stack([orc.float_maxsim_c(q, rows, orc.page_offsets([len(p) for p in pages])) for q in queries])
 
 
 def assert_close_rel(got, want, rtol):
@@ -311,8 +312,8 @@ def test_int8_bit_exact(n_q):
     lens = [1, 33, 0, 64, 200, 1024, 17, 96] + list(rng.integers(1, 260, size=30))
     pages = make_pages(rng, lens)
     queries = [unit_rows(rng, 32 if i % 3 else 19) for i in range(n_q)]
-    # every dot product of these tokens is negative (all-negative query x all-positive pages below): the per-chunk maximum
-    # is negative, which the epilogue's float-datapath max cannot order -> its exact integer fallback must kick in
+    # every dot product of these tokens is negative (all-negative query x all-positive pages below): every per-chunk and
+    # per-page maximum is negative, so a running max that starts at 0 instead of the first chunk's value would show here
     queries[0] = -np.abs(queries[0])
     for j in (3, 4, 9):
         pages[j] = np.abs(pages[j])
@@ -561,11 +562,8 @@ def test_properties_at_scale_int8_binary(dtype):
 
 
 # ------------------------------------------------------------------------------------------------ fp8 e4m3 corpora (config-2 sweep point)
-def oracle_fp8(queries, pages, scale=64.0):
-    rows = np.concatenate(pages) if sum(len(p) for p in pages) else np.zeros((0, 128), np.float32)
-    off = orc.page_offsets([len(p) for p in pages])
-    rr = orc.dequantize_e4m3_np(orc.quantize_e4m3_np(rows, scale))
-    return np.stack([orc.float_maxsim_c(orc.dequantize_e4m3_np(orc.quantize_e4m3_np(q, scale)), rr, off) for q in queries]) / (scale * scale)
+def oracle_fp8(queries, pages):
+    return oracle_scores("fp8", queries, pages)
 
 
 @pytest.mark.parametrize("n_q", [1, 5, 13, 40])
@@ -682,7 +680,7 @@ def test_zero_pad_compat_rerank_matches_port_golden(golden_dir):
 
 
 # ------------------------------------------------------------------------------------------------ batched rerank (per-query lists)
-@pytest.mark.parametrize("dtype", ["bf16", "int8", "binary"])
+@pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8", "binary"])
 def test_rerank_batch_per_query_candidate_lists(dtype):
     rng = np.random.default_rng(71)
     lens = [int(x) for x in rng.integers(1, 200, size=120)] + [0, 1024]
@@ -704,6 +702,10 @@ def test_rerank_batch_per_query_candidate_lists(dtype):
         order = sorted(valid, key=lambda j: (-full[qi, cand[qi, j]], j))[:k]
         assert tc[qi] == len(order) and ti[qi][:len(order)].tolist() == [int(cand[qi, j]) for j in order], (dtype, qi)
         np.testing.assert_allclose(ts[qi][:len(order)], [full[qi, cand[qi, j]] for j in order], rtol=1e-6)
+    want = oracle_scores(dtype, queries, pages)  # and against the oracle, not only against the full scan
+    for qi in range(len(queries)):
+        assert_candidate_ranking(dtype, ts[qi], ti[qi], tc[qi], slot_scores_of(want[qi], cand[qi]), cand[qi], len(pages), k,
+                                 f"{dtype} q{qi}")
 
 
 # ------------------------------------------------------------------------------------------------ pipelined sharded search, world = 1
@@ -746,7 +748,7 @@ def test_sharded_search_pipeline_world1_matches_search():
     assert np.array_equal(o[1].numpy(), prev[1][1]) and np.array_equal(o[2].numpy(), prev[1][2])
 
 
-@pytest.mark.parametrize("dtype", ["bf16", "binary"])
+@pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8", "binary"])
 def test_host_graph_replay_matches_plain_launches(dtype):
     """Small unmasked host searches of a repeated shape are captured into a CUDA graph on their second call and replayed
     afterwards; results equal the plain launches, and a corpus change / option change invalidates the graph."""
@@ -765,7 +767,7 @@ def test_host_graph_replay_matches_plain_launches(dtype):
     for q in qs[:4]:
         ra, rb = a.search_host(q, k=7), b.search_host(q, k=7)
         assert all(np.array_equal(x, y) for x, y in zip(ra, rb))
-    if dtype == "bf16":
+    if dtype != "binary":
         a.set_option("zero_pad_compat", 128); b.set_option("zero_pad_compat", 128)
         for q in qs[:4]:
             ra, rb = a.search_host(q, k=7), b.search_host(q, k=7)
