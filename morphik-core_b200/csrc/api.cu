@@ -157,43 +157,44 @@ DeviceGuard::~DeviceGuard() {
   if (prev >= 0 && cur != prev) cudaSetDevice(prev);
 }
 
-// ---- per-call metadata: ONE block (host-built) -> one upload, or read in place when the block is mapped pinned memory
-struct SearchMeta {
-  std::vector<uint8_t> host;  // [ss int64 (n_q+1) | ds int64 (n_q+1) | goff int32 (n_q+1) | ntok int32 (groups_padded)]
-  size_t off_ss = 0, off_ds = 0, off_goff = 0, off_ntok = 0;
-  int64_t rows = 0, groups = 0, groups_padded = 0;
-  std::vector<int32_t> goff;
-};
-
-static void build_search_meta(const int32_t* q_lens, int n_q, SearchMeta* m) {
-  const int64_t groups = b200ms_query_groups(q_lens, n_q);
-  m->groups = groups;
-  m->groups_padded = (groups + 3) & ~int64_t(3);
-  const size_t n1 = size_t(n_q) + 1;
-  m->off_ss = 0;
-  m->off_ds = n1 * 8;
-  m->off_goff = 2 * n1 * 8;
-  m->off_ntok = m->off_goff + ((n1 * 4 + 15) & ~size_t(15));
-  m->host.assign(m->off_ntok + size_t(m->groups_padded > 0 ? m->groups_padded : 4) * 4, 0);
-  int64_t* ss = reinterpret_cast<int64_t*>(m->host.data() + m->off_ss);
-  int64_t* ds = reinterpret_cast<int64_t*>(m->host.data() + m->off_ds);
-  int32_t* goff = reinterpret_cast<int32_t*>(m->host.data() + m->off_goff);
-  int32_t* ntok = reinterpret_cast<int32_t*>(m->host.data() + m->off_ntok);
-  ss[0] = ds[0] = 0;
-  goff[0] = 0;
-  for (int i = 0; i < n_q; ++i) {
-    const int64_t len = q_lens[i] > 0 ? q_lens[i] : 0;
-    ss[i + 1] = ss[i] + len;
-    ds[i + 1] = ds[i] + b200ms_padded_len(len);
-    goff[i + 1] = int32_t(ds[i + 1] / kGroup);
-    int64_t left = len;
-    for (int g = goff[i]; g < goff[i + 1]; ++g) {
+void group_tokens(const int32_t* lens, int64_t n, const int32_t* goff, int64_t n_groups, int32_t* ntok) {
+  for (int64_t i = 0; i < n; ++i) {
+    int64_t left = lens[i];
+    for (int64_t g = goff[i]; g < goff[i + 1] && g < n_groups; ++g) {
       ntok[g] = int32_t(left > kGroup ? kGroup : left);
       left -= ntok[g];
     }
   }
-  m->rows = ss[n_q];
-  m->goff.assign(goff, goff + n1);
+}
+
+SearchMeta build_search_meta(const int32_t* lens, int64_t n, bool with_groups) {
+  SearchMeta m;
+  if (!lens || n < 0) n = 0;
+  const size_t n1 = size_t(n) + 1;
+  m.n = n;
+  m.off_ds = n1 * 8;
+  m.off_goff = 2 * n1 * 8;
+  m.off_ntok = m.off_goff + ((n1 * 4 + 15) & ~size_t(15));
+  if (with_groups) {
+    m.groups = b200ms_query_groups(lens, int(n));
+    m.groups_padded = groups_padded(m.groups);
+  }
+  m.host.assign(with_groups ? m.off_ntok + size_t(m.groups_padded > 0 ? m.groups_padded : 4) * 4 : m.off_goff, 0);
+  int64_t* ss = reinterpret_cast<int64_t*>(m.host.data());
+  int64_t* ds = reinterpret_cast<int64_t*>(m.host.data() + m.off_ds);
+  for (int64_t i = 0; i < n; ++i) {
+    const int64_t len = lens[i] > 0 ? lens[i] : 0;
+    ss[i + 1] = ss[i] + len;
+    ds[i + 1] = ds[i] + b200ms_padded_len(len);
+  }
+  m.rows = ss[n];
+  m.padded_rows = ds[n];
+  if (with_groups) {
+    int32_t* goff = reinterpret_cast<int32_t*>(m.host.data() + m.off_goff);
+    for (int64_t i = 0; i <= n; ++i) goff[i] = int32_t(ds[i] / kGroup);
+    group_tokens(lens, n, goff, m.groups, reinterpret_cast<int32_t*>(m.host.data() + m.off_ntok));
+  }
+  return m;
 }
 
 }  // namespace bms
@@ -307,13 +308,6 @@ B200MS_API int64_t b200ms_query_groups(const int32_t* q_lens, int n_q) {
 
 B200MS_API int64_t b200ms_launch_count(const b200ms_t* h) { return h ? h->launches : 0; }
 
-B200MS_API int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas) {
-  if (!h) return B200MS_EINVAL;
-  if (unit_rows > 0) h->unit_rows = unit_rows;
-  if (max_ctas >= 0) h->max_ctas = max_ctas;
-  return B200MS_OK;
-}
-
 B200MS_API int b200ms_set_option(b200ms_t* h, const char* name, int64_t value) {
   if (!h || !name) return B200MS_EINVAL;
   const std::string n(name);
@@ -338,31 +332,26 @@ B200MS_API int b200ms_set_option(b200ms_t* h, const char* name, int64_t value) {
   return B200MS_OK;
 }
 
+B200MS_API int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas) {
+  if (!h) return B200MS_EINVAL;
+  if (unit_rows > 0)
+    if (int e = b200ms_set_option(h, "unit_rows", unit_rows)) return e;
+  if (max_ctas >= 0) return b200ms_set_option(h, "max_ctas", max_ctas);
+  return B200MS_OK;
+}
+
 B200MS_API int64_t b200ms_corpus_pages(const b200ms_t* h) { return h ? h->corpus.n_pages : 0; }
 B200MS_API int64_t b200ms_corpus_rows(const b200ms_t* h) { return h ? h->corpus.n_rows : 0; }
 
 // ------------------------------------------------------------------------------------------------ quantise / pack
-static int pack_items(b200ms_t* h, const void* src, int src_dtype, const int32_t* lens, int64_t n, bool queries,
-                      void* dst, int dst_dtype, int64_t dst_rows_total, float i8_scale, cudaStream_t s,
-                      std::vector<int64_t>* dst_start_out) {
-  // one metadata block [ss | ds], one upload
-  std::vector<int64_t> sd(2 * (size_t(n) + 1));
-  int64_t* ss = sd.data();
-  int64_t* ds = sd.data() + n + 1;
-  ss[0] = ds[0] = 0;
-  for (int64_t i = 0; i < n; ++i) {
-    const int64_t len = lens[i] > 0 ? lens[i] : 0;
-    ss[i + 1] = ss[i] + len;
-    ds[i + 1] = ds[i] + b200ms_padded_len(len);
-  }
-  const int64_t dst_rows = dst_rows_total >= 0 ? dst_rows_total : ds[n];
-  if (int e = upload(h, h->meta_b, sd.data(), sd.size() * 8, s)) return e;
+// Pack the items of m (queries: up to groups_padded * 32 rows, tail rows zeroed; pages: m.padded_rows) with one upload of
+// m's [ss | ds] part.  m is pageable host memory: cudaMemcpyAsync staged it before returning, so it may die afterwards.
+static int pack_items(b200ms_t* h, const void* src, int src_dtype, const SearchMeta& m, bool queries, void* dst, int dst_dtype,
+                      float i8_scale, cudaStream_t s) {
+  if (int e = upload(h, h->meta_b, m.host.data(), m.off_goff, s)) return e;
   const int64_t* dev = static_cast<const int64_t*>(h->meta_b.p);
-  if (int e = launch_pack_rows(h, src, src_dtype, dev, dev + n + 1, n, dst_rows, queries ? 1 : 0, dst, dst_dtype, i8_scale, s))
-    return e;
-  // sd is pageable host memory: cudaMemcpyAsync staged it before returning, so it may die here
-  if (dst_start_out) dst_start_out->assign(ds, ds + n + 1);
-  return B200MS_OK;
+  return launch_pack_rows(h, src, src_dtype, dev, dev + m.n + 1, m.n, queries ? m.groups_padded * kGroup : m.padded_rows,
+                          queries ? 1 : 0, dst, dst_dtype, i8_scale, s);
 }
 
 B200MS_API int b200ms_sign_pack(b200ms_t* h, const void* x, int src_dtype, int64_t rows, uint8_t* out, void* stream) {
@@ -395,8 +384,8 @@ B200MS_API int b200ms_pack_pages(b200ms_t* h, const void* src, int src_dtype, co
     return set_error(h, B200MS_EINVAL, "pack_pages: bad arguments");
   if (n_pages == 0) return B200MS_OK;
   DeviceGuard g(h->device);
-  return pack_items(h, src, src_dtype, page_lens, n_pages, false, dst, dst_dtype, -1, i8_scale,
-                    static_cast<cudaStream_t>(stream), nullptr);
+  return pack_items(h, src, src_dtype, build_search_meta(page_lens, n_pages, false), false, dst, dst_dtype, i8_scale,
+                    static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t* q_lens, int n_q,
@@ -406,19 +395,11 @@ B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, co
   if (!src_dtype_ok(src_dtype) || !corpus_dtype_ok(dst_dtype) || n_q < 0 || (n_q > 0 && (!q_lens || !q_packed)))
     return set_error(h, B200MS_EINVAL, "pack_queries: bad arguments");
   DeviceGuard g(h->device);
-  const int64_t groups = b200ms_query_groups(q_lens, n_q);
-  const int64_t groups_padded = (groups + 3) & ~int64_t(3);
-  std::vector<int64_t> ds;
-  if (groups_padded > 0) {
-    if (int e = pack_items(h, q, src_dtype, q_lens, n_q, true, q_packed, dst_dtype, groups_padded * kGroup, i8_scale,
-                           static_cast<cudaStream_t>(stream), &ds))
-      return e;
-  } else {
-    ds.assign(size_t(n_q) + 1, 0);
-  }
-  if (group_offsets_out)
-    for (int i = 0; i <= n_q; ++i) group_offsets_out[i] = int32_t(ds[i] / kGroup);
-  if (n_groups_out) *n_groups_out = int(groups);
+  const SearchMeta m = build_search_meta(q_lens, n_q);
+  if (m.groups_padded > 0)
+    if (int e = pack_items(h, q, src_dtype, m, true, q_packed, dst_dtype, i8_scale, static_cast<cudaStream_t>(stream))) return e;
+  if (group_offsets_out) memcpy(group_offsets_out, m.goff(), (size_t(n_q) + 1) * 4);
+  if (n_groups_out) *n_groups_out = int(m.groups);
   return B200MS_OK;
 }
 
@@ -506,18 +487,51 @@ static int ensure_clamp_pages(b200ms_t* h, cudaStream_t s, const uint32_t** out)
 }
 
 // ------------------------------------------------------------------------------------------------ hot path
-// Candidate description for score_impl / search_impl.
-//   ids == NULL           : scan the whole corpus, scores indexed by page id.
-//   ids, per_query == 0   : ONE list of n_cand page ids (-1 = unused slot) scored by every query, scores indexed by slot.
-//   ids, per_query == 1   : one list PER QUERY, ids = [n_q, stride] with stride = roundup(n_cand, 32); query q owns slots
-//                           [q*stride, q*stride + n_cand) and only its own groups are scored against them.
-struct CandSpec {
-  const int64_t* ids = nullptr;
-  int n_cand = 0;
-  int per_query = 0;
-  int64_t stride = 0;
-  int64_t n_slots(int n_q) const { return per_query ? stride * n_q : n_cand; }
-};
+// Candidate mode of the wgmma scorers: unit j = the chunk range of candidate slot j, scores indexed by j.
+static int candidate_plan(b200ms_t* h, const CandSpec& cs, int n_q, cudaStream_t s, UnitPlan* plan) {
+  const int n_slots = int(cs.n_slots(n_q));
+  if (int e = reserve(h, h->cand_start, size_t(n_slots) * 4)) return e;
+  if (int e = reserve(h, h->cand_end, size_t(n_slots) * 4)) return e;
+  if (int e = launch_cand_units(h, cs.ids, n_slots, static_cast<int32_t*>(h->cand_start.p),
+                                static_cast<int32_t*>(h->cand_end.p), nullptr, s))
+    return e;
+  plan->start = static_cast<const int32_t*>(h->cand_start.p);
+  plan->end = static_cast<const int32_t*>(h->cand_end.p);
+  plan->n_units = n_slots;
+  plan->slot_mode = 1;
+  if (h->zero_pad_batch > 0) {  // the reference's quirk, exactly: batches of zero_pad_batch candidates in first-stage order
+    if (int e = reserve(h, h->clamp_slots, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
+    if (int e = launch_clamp_slots(h, cs.ids, cs.n_cand, cs.per_query ? n_q : 1, cs.stride(), h->zero_pad_batch,
+                                   static_cast<uint32_t*>(h->clamp_slots.p), s))
+      return e;
+    plan->clamp_bits = static_cast<const uint32_t*>(h->clamp_slots.p);
+  }
+  return B200MS_OK;
+}
+
+// Per-query candidate lists on wgmma: one launch per 128-token query tile, the tile's queries against THEIR candidate
+// lists only (a contiguous slot range).
+static int score_wgmma_per_query(b200ms_t* h, const UnitPlan& plan, const CandSpec& cs, const void* q_packed, int n_groups,
+                                 const int32_t* goff, int n_q, void* group_scores, int64_t ld, cudaStream_t s) {
+  const int n_mtiles = int(groups_padded(n_groups)) / 4;
+  int q_lo = 0;
+  for (int m = 0; m < n_mtiles; ++m) {
+    const int g0 = 4 * m, g1 = 4 * m + 4;
+    while (q_lo < n_q && goff[q_lo + 1] <= g0) ++q_lo;  // first query with a group in this tile
+    int q_hi = q_lo;
+    while (q_hi < n_q && goff[q_hi] < g1) ++q_hi;        // one past the last
+    if (q_hi <= q_lo) continue;
+    UnitPlan sub = plan;
+    const int64_t s0 = int64_t(q_lo) * cs.stride();
+    sub.start += s0;
+    sub.end += s0;
+    sub.n_units = int(int64_t(q_hi - q_lo) * cs.stride());
+    if (sub.clamp_bits) sub.clamp_bits += s0 / 32;
+    void* sc = static_cast<uint8_t*>(group_scores) + size_t(s0) * 4;
+    if (int e = launch_score_wgmma(h, sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
+  }
+  return B200MS_OK;
+}
 
 static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* goff, int n_q, const int32_t* ntok_dev,
                       void* group_scores, int64_t ld, const CandSpec& cs, cudaStream_t s) {
@@ -527,96 +541,47 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   if (n_groups < 0 || ld < n_items || cs.n_cand < 0 || (n_groups > 0 && (!q_packed || !group_scores)))
     return set_error(h, B200MS_EINVAL, "score: bad arguments");
   if (n_groups == 0 || n_items == 0 || c.n_pages == 0) return B200MS_OK;
-  const int slot = int(h->ev_count % b200ms_t::kEvRing);
-  const int n_groups_padded = (n_groups + 3) & ~3;
-  if (c.dtype == B200MS_B1) {
-    if (!goff || !ntok_dev || n_q <= 0) return set_error(h, B200MS_EINVAL, "score: B1 needs the per-group token counts");
-    // b1_tensor: 0 = POPC kernel, 1 = wgmma kernel (bits expanded to int8, maxsim_wgmma.cu), 2 (default) = by group count:
-    // the POPC pipe costs one pass per 32-token group, the wgmma kernel about the same for up to 4 groups.  Full scans of
-    // 65 536 pages x 1024 rows (tools/time_scan.py --b1-groups) on an NVIDIA H100 80GB HBM3 at a 700 W power limit: 1 group
-    // 1.65 ms POPC vs 3.80 ms wgmma, 2 groups 3.16 vs 3.81, 3 groups 4.85 vs 3.81, 8 groups 12.76 vs 4.75.  Rerank of a
-    // candidate list stays on the POPC kernel.
-    const bool tensor_path = !cs.ids && (h->b1_tensor == 1 || (h->b1_tensor == 2 && n_groups >= 3));
-    if ((tensor_path && c.has_empty) || cs.per_query)
-      if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(n_groups_padded) * size_t(ld) * 4, s), "score: memset")) return e;
-    if (!h->capturing)
-      if (int e = check_cuda(h, cudaEventRecord(h->ev0[slot], s), "score: event record")) return e;
-    if (tensor_path) {
-      if (int e = launch_score_b1_wgmma(h, q_packed, ntok_dev, n_groups, group_scores, ld, s)) return e;
-    } else if (cs.per_query) {
-      for (int q = 0; q < n_q; ++q) {
-        if (goff[q + 1] <= goff[q]) continue;
-        if (int e = launch_score_b1(h, cs.ids + int64_t(q) * cs.stride, cs.n_cand, q_packed, n_groups, ntok_dev,
-                                    static_cast<int32_t*>(group_scores) + int64_t(q) * cs.stride, ld, s, goff[q], goff[q + 1]))
-          return e;
-      }
-    } else {
-      if (int e = launch_score_b1(h, cs.ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups)) return e;
-    }
-    if (!h->capturing) {
-      if (int e = check_cuda(h, cudaEventRecord(h->ev1[slot], s), "score: event record")) return e;
-      h->ev_count++;
-    }
-    return B200MS_OK;
-  }
-  // pages with zero rows (and unused candidate slots) are never touched by the tile kernel: they score 0
-  if (c.has_empty || cs.ids) {
-    if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(n_groups_padded) * size_t(ld) * 4, s), "score: memset")) return e;
-  }
-  UnitPlan plan;
-  if (cs.ids) {
-    const int n_slots = int(cs.n_slots(n_q));
-    if (int e = reserve(h, h->cand_start, size_t(n_slots) * 4)) return e;
-    if (int e = reserve(h, h->cand_end, size_t(n_slots) * 4)) return e;
-    if (int e = launch_cand_units(h, cs.ids, n_slots, static_cast<int32_t*>(h->cand_start.p),
-                                  static_cast<int32_t*>(h->cand_end.p), nullptr, s))
+  const bool b1 = c.dtype == B200MS_B1;
+  if (b1 && (!goff || !ntok_dev || n_q <= 0)) return set_error(h, B200MS_EINVAL, "score: B1 needs the per-group token counts");
+  // b1_tensor: 0 = POPC kernel, 1 = wgmma kernel (bits expanded to int8, maxsim_wgmma.cu), 2 (default) = by group count:
+  // the POPC pipe costs one pass per 32-token group, the wgmma kernel about the same for up to 4 groups.  Full scans of
+  // 65 536 pages x 1024 rows (tools/time_scan.py --b1-groups) on an NVIDIA H100 80GB HBM3 at a 700 W power limit: 1 group
+  // 1.65 ms POPC vs 3.80 ms wgmma, 2 groups 3.16 vs 3.81, 3 groups 4.85 vs 3.81, 8 groups 12.76 vs 4.75.  Rerank of a
+  // candidate list stays on the POPC kernel.
+  const bool b1_wgmma = b1 && !cs.ids && (h->b1_tensor == 1 || (h->b1_tensor == 2 && n_groups >= 3));
+  // zero-fill what no launch writes: the tile kernels skip pages with zero rows and unused candidate slots; the per-query
+  // POPC launches write only their own query's groups and slots
+  const bool zero_fill = b1 ? (b1_wgmma && c.has_empty) || cs.per_query : c.has_empty || cs.ids;
+  if (zero_fill)
+    if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(groups_padded(n_groups)) * size_t(ld) * 4, s), "score: memset"))
       return e;
-    plan.start = static_cast<const int32_t*>(h->cand_start.p);
-    plan.end = static_cast<const int32_t*>(h->cand_end.p);
-    plan.n_units = n_slots;
-    plan.slot_mode = 1;
-    if (h->zero_pad_batch > 0) {  // the reference's quirk, exactly: batches of zero_pad_batch candidates in first-stage order
-      if (int e = reserve(h, h->clamp_slots, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
-      const int lists = cs.per_query ? n_q : 1;
-      const int64_t stride = cs.per_query ? cs.stride : 0;
-      if (int e = launch_clamp_slots(h, cs.ids, cs.n_cand, lists, stride, h->zero_pad_batch,
-                                     static_cast<uint32_t*>(h->clamp_slots.p), s))
-        return e;
-      plan.clamp_bits = static_cast<const uint32_t*>(h->clamp_slots.p);
-    }
-  } else {  // full scan: unit u = [unit_start[u], unit_start[u+1])
-    plan.start = static_cast<const int32_t*>(h->unit_start.p);
-    plan.end = plan.start + 1;
-    plan.n_units = c.n_units;
-    plan.slot_mode = 0;
-    if (int e = ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
+  UnitPlan plan = full_scan_plan(h);
+  if (!b1) {
+    if (int e = cs.ids ? candidate_plan(h, cs, n_q, s, &plan) : ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
   }
+  // ev0 / ev1 bracket the scoring launches only (b200ms_score_times_ms): bench.py derives the roofline's achieved figure
+  // from this time
+  const int slot = int(h->ev_count % b200ms_t::kEvRing);
   if (!h->capturing)
     if (int e = check_cuda(h, cudaEventRecord(h->ev0[slot], s), "score: event record")) return e;
-  if (cs.ids && cs.per_query) {
-    // one launch per 128-token query tile: the tile's queries against THEIR candidate lists only (a contiguous slot range)
-    const int n_mtiles = n_groups_padded / 4;
-    int q_lo = 0;
-    for (int m = 0; m < n_mtiles; ++m) {
-      const int g0 = 4 * m, g1 = 4 * m + 4;
-      while (q_lo < n_q && goff[q_lo + 1] <= g0) ++q_lo;  // first query with a group in this tile
-      int q_hi = q_lo;
-      while (q_hi < n_q && goff[q_hi] < g1) ++q_hi;        // one past the last
-      if (q_hi <= q_lo) continue;
-      UnitPlan sub = plan;
-      const int64_t s0 = int64_t(q_lo) * cs.stride;
-      sub.start += s0;
-      sub.end += s0;
-      sub.n_units = int(int64_t(q_hi - q_lo) * cs.stride);
-      if (sub.clamp_bits) sub.clamp_bits += s0 / 32;
-      void* sc = static_cast<uint8_t*>(group_scores) + size_t(s0) * 4;
-      if (int e = launch_score_wgmma(h, &sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
-    }
+  int e = B200MS_OK;
+  if (b1_wgmma) {
+    e = launch_score_b1_wgmma(h, q_packed, ntok_dev, n_groups, group_scores, ld, s);
+  } else if (b1 && cs.per_query) {
+    for (int q = 0; q < n_q && !e; ++q)
+      if (goff[q + 1] > goff[q])
+        e = launch_score_b1(h, cs.ids + int64_t(q) * cs.stride(), cs.n_cand, q_packed, n_groups, ntok_dev,
+                            static_cast<int32_t*>(group_scores) + int64_t(q) * cs.stride(), ld, s, goff[q], goff[q + 1]);
+  } else if (b1) {
+    e = launch_score_b1(h, cs.ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups);
+  } else if (cs.per_query) {
+    e = score_wgmma_per_query(h, plan, cs, q_packed, n_groups, goff, n_q, group_scores, ld, s);
   } else {
-    if (int e = launch_score_wgmma(h, &plan, q_packed, n_groups, group_scores, ld, s)) return e;
+    e = launch_score_wgmma(h, plan, q_packed, n_groups, group_scores, ld, s);
   }
+  if (e) return e;
   if (!h->capturing) {
-    if (int e = check_cuda(h, cudaEventRecord(h->ev1[slot], s), "score: event record")) return e;
+    if (int e2 = check_cuda(h, cudaEventRecord(h->ev1[slot], s), "score: event record")) return e2;
     h->ev_count++;
   }
   return B200MS_OK;
@@ -630,15 +595,9 @@ B200MS_API int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, con
   const int32_t* ntok_dev = nullptr;
   if (h->corpus.dtype == B200MS_B1) {
     if (!q_lens || !group_offsets || n_q <= 0) return set_error(h, B200MS_EINVAL, "score: B1 needs q_lens and group_offsets");
-    const int n_groups_padded = (n_groups + 3) & ~3;
-    std::vector<int32_t> ntok(size_t(n_groups_padded > 0 ? n_groups_padded : 4), 0);
-    for (int q = 0; q < n_q; ++q) {
-      int left = q_lens[q];
-      for (int gi = group_offsets[q]; gi < group_offsets[q + 1] && gi < n_groups; ++gi) {
-        ntok[gi] = left > kGroup ? kGroup : left;
-        left -= ntok[gi];
-      }
-    }
+    const int64_t gp = groups_padded(n_groups);
+    std::vector<int32_t> ntok(size_t(gp > 0 ? gp : 4), 0);
+    group_tokens(q_lens, n_q, group_offsets, n_groups, ntok.data());
     if (int e = upload(h, h->meta, ntok.data(), ntok.size() * 4, s)) return e;
     ntok_dev = static_cast<const int32_t*>(h->meta.p);
   }
@@ -701,82 +660,56 @@ B200MS_API int b200ms_merge_topk(b200ms_t* h, const float* cand_scores, const in
 
 namespace bms {
 
-// The search step shared by every entry point: pack queries -> score -> top-k, all enqueued on `s`.
-//   q_src           rows [sum q_lens,128] F32|BF16, device memory or (zero-copy path) mapped pinned host memory
-//   meta_in_place   != NULL: the SearchMeta block already sits in device-readable memory at this address (mapped pinned
-//                   staging) -- no upload; else the block is uploaded with ONE cudaMemcpyAsync
-int search_core(b200ms_t* h, const void* q_src, int src_dtype, const int32_t* q_lens, int n_q, int k,
-                const uint32_t* allow_dev, float i8_q_scale, float score_scale, int64_t id_base, float* ts, int64_t* ti,
-                int32_t* tc, cudaStream_t s, const SearchCand* cand, const int32_t* mask_index_dev, int64_t mask_stride,
-                const void* meta_in_place, const void* meta_host_block) {
+int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "search: no corpus attached (call b200ms_set_corpus first)");
-  if (n_q < 1 || !q_lens || !q_src || k < 1 || k > B200MS_MAX_K || !ts || !ti || !tc)
+  const int n_q = r.n_q;
+  if (n_q < 1 || !r.q_lens || !r.q || r.k < 1 || r.k > B200MS_MAX_K || !r.top_scores || !r.top_ids || !r.top_counts)
     return set_error(h, B200MS_EINVAL, "search: bad arguments (n_q >= 1, 1 <= k <= 4096)");
-  SearchMeta local;
-  const SearchMeta* m = static_cast<const SearchMeta*>(meta_host_block);
-  if (!m) {
-    build_search_meta(q_lens, n_q, &local);
-    m = &local;
+  CandSpec cs = r.cand;
+  if (cs.per_query && cs.stride() != cs.n_cand) {  // caller's lists are [n_q, n_cand]: give every list a 32-slot-aligned stride
+    if (int e = reserve(h, h->cand_pad, size_t(cs.stride()) * size_t(n_q) * 8)) return e;
+    if (int e = launch_pad_cands(h, r.cand.ids, cs.n_cand, n_q, cs.stride(), static_cast<int64_t*>(h->cand_pad.p), s)) return e;
+    cs.ids = static_cast<const int64_t*>(h->cand_pad.p);
   }
-  CandSpec cs;
-  if (cand && cand->ids) {
-    cs.ids = cand->ids;
-    cs.n_cand = cand->n_cand;
-    cs.per_query = cand->per_query;
-    cs.stride = cand->per_query ? ((int64_t(cand->n_cand) + 31) & ~int64_t(31)) : 0;
-    if (cs.per_query && cs.stride != cs.n_cand) {  // caller's lists are [n_q, n_cand]: give every list a 32-slot-aligned stride
-      if (int e = reserve(h, h->cand_pad, size_t(cs.stride) * size_t(n_q) * 8)) return e;
-      if (int e = launch_pad_cands(h, cand->ids, cs.n_cand, n_q, cs.stride, static_cast<int64_t*>(h->cand_pad.p), s)) return e;
-      cs.ids = static_cast<const int64_t*>(h->cand_pad.p);
-    }
-  }
-  const int64_t gp = m->groups_padded > 0 ? m->groups_padded : 4;
+  const int64_t gp = m.groups_padded > 0 ? m.groups_padded : 4;
   const int64_t n_items = cs.ids ? cs.n_slots(n_q) : c.n_pages;
   const int64_t ld = ((n_items + 31) & ~int64_t(31)) > 0 ? ((n_items + 31) & ~int64_t(31)) : 32;
   if (int e = reserve(h, h->q_packed, size_t(gp) * kGroup * size_t(b200ms_row_bytes(c.dtype)))) return e;
   if (int e = reserve(h, h->scores, size_t(gp) * size_t(ld) * 4)) return e;
-  const uint8_t* meta_dev = static_cast<const uint8_t*>(meta_in_place);
   if (!meta_dev) {
-    if (int e = upload(h, h->meta, m->host.data(), m->host.size(), s)) return e;
-    meta_dev = static_cast<const uint8_t*>(h->meta.p);
+    if (int e = upload(h, h->meta, m.host.data(), m.host.size(), s)) return e;
+    meta_dev = h->meta.p;
   }
-  const int64_t* ss_dev = reinterpret_cast<const int64_t*>(meta_dev + m->off_ss);
-  const int64_t* ds_dev = reinterpret_cast<const int64_t*>(meta_dev + m->off_ds);
-  const int32_t* goff_dev = reinterpret_cast<const int32_t*>(meta_dev + m->off_goff);
-  const int32_t* ntok_dev = reinterpret_cast<const int32_t*>(meta_dev + m->off_ntok);
-  if (m->groups_padded > 0)
-    if (int e = launch_pack_rows(h, q_src, src_dtype, ss_dev, ds_dev, n_q, m->groups_padded * kGroup, 1, h->q_packed.p, c.dtype,
-                                 i8_q_scale, s))
+  const uint8_t* md = static_cast<const uint8_t*>(meta_dev);
+  const int64_t* ss_dev = reinterpret_cast<const int64_t*>(md);
+  const int64_t* ds_dev = reinterpret_cast<const int64_t*>(md + m.off_ds);
+  const int32_t* goff_dev = reinterpret_cast<const int32_t*>(md + m.off_goff);
+  const int32_t* ntok_dev = reinterpret_cast<const int32_t*>(md + m.off_ntok);
+  if (m.groups_padded > 0)
+    if (int e = launch_pack_rows(h, r.q, r.q_dtype, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, 1, h->q_packed.p, c.dtype,
+                                 r.i8_q_scale, s))
       return e;
-  const int ng = int(m->groups);
-  if (int e = score_impl(h, h->q_packed.p, ng, m->goff.data(), n_q, ntok_dev, h->scores.p, ld, cs, s)) return e;
+  const int ng = int(m.groups);
+  if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s)) return e;
   if (ng == 0 || n_items == 0) {
     // nothing scored: every page (if any) has score 0 -- still a defined ranking
     if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "search: memset")) return e;
   }
   const int sdt = (c.dtype == B200MS_BF16 || c.dtype == B200MS_F8) ? B200MS_F32 : B200MS_I32;
   if (!cs.ids) {
-    return launch_topk(h, h->scores.p, sdt, c.n_pages, ld, goff_dev, n_q, allow_dev, k, score_scale, id_base, nullptr, ts, ti,
-                       tc, s, mask_index_dev, mask_stride);
+    return launch_topk(h, h->scores.p, sdt, c.n_pages, ld, goff_dev, n_q, r.allow, r.k, r.score_scale, r.id_base, nullptr,
+                       r.top_scores, r.top_ids, r.top_counts, s, r.mask_index, (c.n_pages + 31) / 32);
   }
   // candidate mode: rank the slots (ties -> lower slot = better first-stage rank), report the page ids; unused slots masked
   const int n_slots = int(cs.n_slots(n_q));
   if (int e = reserve(h, h->cand_mask, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
   if (int e = launch_cand_units(h, cs.ids, n_slots, nullptr, nullptr, static_cast<uint32_t*>(h->cand_mask.p), s)) return e;
-  return launch_topk(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, static_cast<const uint32_t*>(h->cand_mask.p), k,
-                     score_scale, 0, cs.ids, ts, ti, tc, s, nullptr, 0, cs.per_query ? cs.stride : 0);
+  return launch_topk(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, static_cast<const uint32_t*>(h->cand_mask.p), r.k,
+                     r.score_scale, 0, cs.ids, r.top_scores, r.top_ids, r.top_counts, s, nullptr, 0, cs.stride());
 }
 
 }  // namespace bms
-
-static int search_impl(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
-                       const uint32_t* allow_dev, float i8_q_scale, float score_scale, int64_t id_base, float* ts,
-                       int64_t* ti, int32_t* tc, cudaStream_t s, const SearchCand* cand = nullptr,
-                       const int32_t* mask_index_dev = nullptr, int64_t mask_stride = 0) {
-  return search_core(h, q_dev, src_dtype, q_lens, n_q, k, allow_dev, i8_q_scale, score_scale, id_base, ts, ti, tc, s, cand,
-                     mask_index_dev, mask_stride, nullptr, nullptr);
-}
 
 B200MS_API int b200ms_rerank_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
                                     const int64_t* cand_ids_dev, int n_cand, int k, float i8_q_scale, float score_scale,
@@ -785,22 +718,22 @@ B200MS_API int b200ms_rerank_device(b200ms_t* h, const void* q_dev, int src_dtyp
   if (!src_dtype_ok(src_dtype) || !cand_ids_dev || n_cand < 1)
     return set_error(h, B200MS_EINVAL, "rerank_device: bad arguments (F32/BF16 queries, n_cand >= 1)");
   DeviceGuard g(h->device);
-  SearchCand cand{cand_ids_dev, n_cand, 0};
-  return search_impl(h, q_dev, src_dtype, q_lens, n_q, k, nullptr, i8_q_scale, score_scale, 0, top_scores_dev, top_ids_dev,
-                     top_counts_dev, static_cast<cudaStream_t>(stream), &cand);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev};
+  r.cand = CandSpec{cand_ids_dev, n_cand, 0};
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
                                           const int64_t* cand_ids_dev, int n_cand, int k, float i8_q_scale, float score_scale,
                                           float* top_scores_dev, int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream) {
   if (!h) return B200MS_EINVAL;
-  if (!src_dtype_ok(src_dtype) || !cand_ids_dev || n_cand < 1 || n_q < 1 ||
-      ((int64_t(n_cand) + 31) & ~int64_t(31)) * n_q >= (int64_t(1) << 30))
+  const CandSpec cand{cand_ids_dev, n_cand, 1};
+  if (!src_dtype_ok(src_dtype) || !cand_ids_dev || n_cand < 1 || n_q < 1 || cand.n_slots(n_q) >= (int64_t(1) << 30))
     return set_error(h, B200MS_EINVAL, "rerank_batch_device: bad arguments (F32/BF16 queries, n_cand >= 1, n_q*n_cand < 2^30)");
   DeviceGuard g(h->device);
-  SearchCand cand{cand_ids_dev, n_cand, 1};
-  return search_impl(h, q_dev, src_dtype, q_lens, n_q, k, nullptr, i8_q_scale, score_scale, 0, top_scores_dev, top_ids_dev,
-                     top_counts_dev, static_cast<cudaStream_t>(stream), &cand);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev};
+  r.cand = cand;
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_search_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
@@ -809,8 +742,9 @@ B200MS_API int b200ms_search_device(b200ms_t* h, const void* q_dev, int src_dtyp
   if (!h) return B200MS_EINVAL;
   if (!src_dtype_ok(src_dtype)) return set_error(h, B200MS_EINVAL, "search_device: src dtype must be F32 or BF16");
   DeviceGuard g(h->device);
-  return search_impl(h, q_dev, src_dtype, q_lens, n_q, k, allow_mask_dev, i8_q_scale, score_scale, id_base, top_scores_dev,
-                     top_ids_dev, top_counts_dev, static_cast<cudaStream_t>(stream));
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev, id_base};
+  r.allow = allow_mask_dev;
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
@@ -823,9 +757,86 @@ B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int s
   if (n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
     return set_error(h, B200MS_EINVAL, "search_device_masked: n_masks > 0 needs the mask matrix and one index per query");
   DeviceGuard g(h->device);
-  return search_impl(h, q_dev, src_dtype, q_lens, n_q, k, n_masks > 0 ? allow_masks_dev : nullptr, i8_q_scale, score_scale,
-                     id_base, top_scores_dev, top_ids_dev, top_counts_dev, static_cast<cudaStream_t>(stream), nullptr,
-                     n_masks > 0 ? mask_index_dev : nullptr, (h->corpus.n_pages + 31) / 32);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev, id_base};
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+}
+
+// Small unmasked zero-copy calls repeat with the same shapes (interactive queries): the second call of a shape is captured
+// into a CUDA graph -- pack -> score -> top-k become ONE launch, the third call onwards replays it.  Everything the kernels
+// read or write sits at fixed addresses (mapped staging block, handle scratch); h->generation changes when any moves.
+// enqueue() puts the search on stream s; it runs plainly on the first use of a shape and whenever capture fails.
+template <class Enqueue>
+static int run_host_graph(b200ms_t* h, uint64_t key, cudaStream_t s, Enqueue&& enqueue) {
+  b200ms::HostGraph* hg = nullptr;  // NOLINT
+  for (auto& g : h->host_graphs)
+    if (g.key == key) hg = &g;
+  if (!hg) {
+    if (h->host_graphs.size() >= 16) {  // evict the least recently used shape
+      size_t lru = 0;
+      for (size_t i = 1; i < h->host_graphs.size(); ++i)
+        if (h->host_graphs[i].last_use < h->host_graphs[lru].last_use) lru = i;
+      if (h->host_graphs[lru].exec) cudaGraphExecDestroy(h->host_graphs[lru].exec);
+      h->host_graphs.erase(h->host_graphs.begin() + long(lru));
+    }
+    h->host_graphs.emplace_back();
+    hg = &h->host_graphs.back();
+    hg->key = key;
+  }
+  hg->last_use = ++h->graph_clock;
+  if (hg->exec && hg->generation != h->generation) {  // a buffer moved / corpus or option changed: start over
+    cudaGraphExecDestroy(hg->exec);
+    hg->exec = nullptr;
+    hg->seen = 0;
+  }
+  if (hg->exec) {
+    if (int e = check_cuda(h, cudaGraphLaunch(hg->exec, s), "search_host: graph launch")) return e;
+    h->launches += hg->launches;
+    return B200MS_OK;
+  }
+  if (hg->seen < 1) {
+    hg->seen++;
+    return enqueue();
+  }
+  const uint64_t gen0 = h->generation;
+  const int64_t l0 = h->launches;
+  if (int e = check_cuda(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal), "search_host: begin capture")) return e;
+  h->capturing = true;
+  const int e = enqueue();
+  h->capturing = false;
+  cudaGraph_t graph = nullptr;
+  const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+  bool ok = !e && ce == cudaSuccess && graph && gen0 == h->generation;
+  if (ok) ok = cudaGraphInstantiate(&hg->exec, graph, 0) == cudaSuccess;
+  if (graph) cudaGraphDestroy(graph);
+  if (!ok) {
+    cudaGetLastError();
+    hg->exec = nullptr;
+    hg->seen = -1000000;  // this shape does not capture: plain launches from now on
+    return enqueue();
+  }
+  hg->generation = h->generation;
+  hg->launches = int(h->launches - l0);
+  return check_cuda(h, cudaGraphLaunch(hg->exec, s), "search_host: graph launch");
+}
+
+// the shape of a host search: everything a captured graph bakes in besides the staging and scratch addresses
+static uint64_t host_graph_key(const SearchRequest& r) {
+  uint64_t key = 1469598103934665603ull;
+  auto mix = [&](uint64_t v) { key = (key ^ v) * 1099511628211ull; };
+  mix(uint64_t(r.n_q));
+  mix(uint64_t(r.k));
+  for (int i = 0; i < r.n_q; ++i) mix(uint64_t(uint32_t(r.q_lens[i])));
+  mix(uint64_t(r.id_base));
+  uint32_t fb;
+  memcpy(&fb, &r.score_scale, 4);
+  mix(fb);
+  memcpy(&fb, &r.i8_q_scale, 4);
+  mix(fb);
+  return key;
 }
 
 // Host entry point.  Two transports, same kernels:
@@ -833,7 +844,7 @@ B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int s
 //     per-call metadata are written into ONE handle-owned mapped pinned block that the pack / top-k kernels read in
 //     place, and the top-k kernel writes its results straight into the same block -- no copy-engine operation and no
 //     metadata upload on the critical path (round 1 spent ~12 driver calls, 4 of them pageable uploads, around a 15 us scan).
-//   copy engine (batches): one H2D of the rows, one upload of the metadata block, one fused D2H of [scores|ids|counts].
+//   copy engine (batches): one H2D of the rows, one upload of the metadata block, one fused D2H of the result block.
 static int search_host_impl(b200ms_t* h, const float* q_host, const int32_t* q_lens, int n_q, int k,
                             const uint32_t* masks_host, int n_masks, const int32_t* mask_index_host, float i8_q_scale,
                             float score_scale, int64_t id_base, float* top_scores_host, int64_t* top_ids_host,
@@ -842,133 +853,51 @@ static int search_host_impl(b200ms_t* h, const float* q_host, const int32_t* q_l
     return set_error(h, B200MS_EINVAL, "search_host: bad arguments (n_q >= 1, 1 <= k <= 4096)");
   DeviceGuard g(h->device);
   cudaStream_t s = h->stream;
-  SearchMeta m;
-  build_search_meta(q_lens, n_q, &m);
-  const size_t q_bytes = size_t(m.rows > 0 ? m.rows : 0) * kDim * 4;
-  const size_t nk = size_t(n_q) * size_t(k);
-  const size_t out_ids_off = 0, out_scores_off = nk * 8, out_counts_off = nk * 12;
-  const size_t out_bytes = (nk * 12 + size_t(n_q) * 4 + 15) & ~size_t(15);
-  const uint32_t* allow_dev = nullptr;
-  const int32_t* index_dev = nullptr;
-  const int64_t words = (h->corpus.n_pages + 31) / 32;
+  const SearchMeta m = build_search_meta(q_lens, n_q);
+  const ResultBlock rb(n_q, k);
+  const size_t q_bytes = size_t(m.rows) * kDim * 4;
+  SearchRequest r{nullptr, B200MS_F32, q_lens, n_q, k, i8_q_scale, score_scale};
+  r.id_base = id_base;
   if (masks_host && n_masks > 0 && h->corpus.n_pages > 0) {
     if (mask_index_host)
       for (int i = 0; i < n_q; ++i)
         if (mask_index_host[i] < -1 || mask_index_host[i] >= n_masks)
           return set_error(h, B200MS_EINVAL, "search_host_masked: mask_index out of range");
-    if (int e = upload(h, h->mask, masks_host, size_t(n_masks) * size_t(words) * 4, s)) return e;
-    allow_dev = static_cast<const uint32_t*>(h->mask.p);
+    if (int e = upload(h, h->mask, masks_host, size_t(n_masks) * size_t((h->corpus.n_pages + 31) / 32) * 4, s)) return e;
+    r.allow = static_cast<const uint32_t*>(h->mask.p);
     if (mask_index_host) {
       if (int e = upload(h, h->mask_index, mask_index_host, size_t(n_q) * 4, s)) return e;
-      index_dev = static_cast<const int32_t*>(h->mask_index.p);
+      r.mask_index = static_cast<const int32_t*>(h->mask_index.p);
     }
   }
-  const bool zc = h->zero_copy && m.rows <= 256 && out_bytes <= (64u << 10);
-  const size_t meta_off = 0, q_off = (m.host.size() + 255) & ~size_t(255), out_off = (q_off + q_bytes + 255) & ~size_t(255);
-  if (int e = reserve_pinned(h, h->stage, out_off + out_bytes)) return e;
+  const bool zc = h->zero_copy && m.rows <= 256 && rb.bytes() <= (64u << 10);
+  const size_t q_off = (m.host.size() + 255) & ~size_t(255), out_off = (q_off + q_bytes + 255) & ~size_t(255);
+  if (int e = reserve_pinned(h, h->stage, out_off + rb.bytes())) return e;
   uint8_t* st = static_cast<uint8_t*>(h->stage.p);
-  int e = 0;
-  if (zc) {
-    memcpy(st + meta_off, m.host.data(), m.host.size());
+  void* out = st + out_off;  // where the kernels write the result block
+  const void* meta_dev = nullptr;
+  if (zc) {  // [metadata | query rows | results], all read and written in place
+    memcpy(st, m.host.data(), m.host.size());
     if (q_bytes) memcpy(st + q_off, q_host, q_bytes);
-    float* ts = reinterpret_cast<float*>(st + out_off + out_scores_off);
-    int64_t* ti = reinterpret_cast<int64_t*>(st + out_off + out_ids_off);
-    int32_t* tc = reinterpret_cast<int32_t*>(st + out_off + out_counts_off);
-    // Small unmasked calls repeat with the same shapes (interactive queries): the second call of a shape is captured into
-    // a CUDA graph -- pack -> score -> top-k become ONE launch, the third call onwards replays it.  Everything the kernels
-    // read or write sits at fixed addresses (mapped staging block, handle scratch); h->generation changes when any moves.
-    b200ms::HostGraph* hg = nullptr;  // NOLINT
-    if (h->host_graph && !allow_dev) {
-      uint64_t key = 1469598103934665603ull;
-      auto mix = [&](uint64_t v) { key = (key ^ v) * 1099511628211ull; };
-      mix(uint64_t(n_q));
-      mix(uint64_t(k));
-      for (int i = 0; i < n_q; ++i) mix(uint64_t(uint32_t(q_lens[i])));
-      mix(uint64_t(id_base));
-      uint32_t fb;
-      memcpy(&fb, &score_scale, 4);
-      mix(fb);
-      memcpy(&fb, &i8_q_scale, 4);
-      mix(fb);
-      for (auto& g2 : h->host_graphs)
-        if (g2.key == key) hg = &g2;
-      if (!hg) {
-        if (h->host_graphs.size() >= 16) {  // evict the least recently used shape
-          size_t lru = 0;
-          for (size_t i = 1; i < h->host_graphs.size(); ++i)
-            if (h->host_graphs[i].last_use < h->host_graphs[lru].last_use) lru = i;
-          if (h->host_graphs[lru].exec) cudaGraphExecDestroy(h->host_graphs[lru].exec);
-          h->host_graphs.erase(h->host_graphs.begin() + long(lru));
-        }
-        h->host_graphs.emplace_back();
-        hg = &h->host_graphs.back();
-        hg->key = key;
-      }
-      hg->last_use = ++h->graph_clock;
-      if (hg->exec && hg->generation != h->generation) {  // a buffer moved / corpus or option changed: start over
-        cudaGraphExecDestroy(hg->exec);
-        hg->exec = nullptr;
-        hg->seen = 0;
-      }
-    }
-    if (hg && hg->exec) {
-      if (int e2 = check_cuda(h, cudaGraphLaunch(hg->exec, s), "search_host: graph launch")) return e2;
-      h->launches += hg->launches;
-    } else if (hg && hg->seen >= 1) {
-      const uint64_t gen0 = h->generation;
-      const int64_t l0 = h->launches;
-      if (int e2 = check_cuda(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal), "search_host: begin capture")) return e2;
-      h->capturing = true;
-      e = search_core(h, st + q_off, B200MS_F32, q_lens, n_q, k, nullptr, i8_q_scale, score_scale, id_base, ts, ti, tc, s, nullptr,
-                      nullptr, words, st + meta_off, &m);
-      h->capturing = false;
-      cudaGraph_t graph = nullptr;
-      const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-      if (e || ce != cudaSuccess || !graph || gen0 != h->generation) {
-        if (graph) cudaGraphDestroy(graph);
-        cudaGetLastError();
-        hg->seen = -1000000;  // this shape does not capture: plain launches from now on
-        e = search_core(h, st + q_off, B200MS_F32, q_lens, n_q, k, nullptr, i8_q_scale, score_scale, id_base, ts, ti, tc, s,
-                        nullptr, nullptr, words, st + meta_off, &m);
-        if (e) return e;
-      } else {
-        const cudaError_t ie = cudaGraphInstantiate(&hg->exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) {
-          cudaGetLastError();
-          hg->exec = nullptr;
-          hg->seen = -1000000;
-          e = search_core(h, st + q_off, B200MS_F32, q_lens, n_q, k, nullptr, i8_q_scale, score_scale, id_base, ts, ti, tc, s,
-                          nullptr, nullptr, words, st + meta_off, &m);
-          if (e) return e;
-        } else {
-          hg->generation = h->generation;
-          hg->launches = int(h->launches - l0);
-          if (int e2 = check_cuda(h, cudaGraphLaunch(hg->exec, s), "search_host: graph launch")) return e2;
-        }
-      }
-    } else {
-      if (hg) hg->seen++;
-      e = search_core(h, st + q_off, B200MS_F32, q_lens, n_q, k, allow_dev, i8_q_scale, score_scale, id_base, ts, ti, tc, s,
-                      nullptr, index_dev, words, st + meta_off, &m);
-      if (e) return e;
-    }
+    r.q = st + q_off;
+    meta_dev = st;
   } else {
-    if (int e2 = reserve(h, h->q_raw, q_bytes ? q_bytes : 512)) return e2;
-    if (int e2 = reserve(h, h->out_all, out_bytes)) return e2;
+    if (int e = reserve(h, h->q_raw, q_bytes ? q_bytes : 512)) return e;
+    if (int e = reserve(h, h->out_all, rb.bytes())) return e;
     if (q_bytes)
-      if (int e2 = check_cuda(h, cudaMemcpyAsync(h->q_raw.p, q_host, q_bytes, cudaMemcpyHostToDevice, s), "search_host: H2D queries")) return e2;
-    uint8_t* od = static_cast<uint8_t*>(h->out_all.p);
-    e = search_core(h, h->q_raw.p, B200MS_F32, q_lens, n_q, k, allow_dev, i8_q_scale, score_scale, id_base,
-                    reinterpret_cast<float*>(od + out_scores_off), reinterpret_cast<int64_t*>(od + out_ids_off),
-                    reinterpret_cast<int32_t*>(od + out_counts_off), s, nullptr, index_dev, words, nullptr, &m);
-    if (e) return e;
-    if (int e2 = check_cuda(h, cudaMemcpyAsync(st + out_off, od, out_bytes, cudaMemcpyDeviceToHost, s), "search_host: D2H results")) return e2;
+      if (int e = check_cuda(h, cudaMemcpyAsync(h->q_raw.p, q_host, q_bytes, cudaMemcpyHostToDevice, s), "search_host: H2D queries")) return e;
+    r.q = h->q_raw.p;
+    out = h->out_all.p;
   }
-  if (int e2 = check_cuda(h, cudaStreamSynchronize(s), "search_host: stream sync")) return e2;
-  memcpy(top_ids_host, st + out_off + out_ids_off, nk * 8);
-  memcpy(top_scores_host, st + out_off + out_scores_off, nk * 4);
-  memcpy(top_counts_host, st + out_off + out_counts_off, size_t(n_q) * 4);
+  r.top_scores = rb.scores(out);
+  r.top_ids = rb.ids(out);
+  r.top_counts = rb.counts(out);
+  auto enqueue = [&] { return search_core(h, r, m, s, meta_dev); };
+  if (int e = zc && h->host_graph && !r.allow ? run_host_graph(h, host_graph_key(r), s, enqueue) : enqueue()) return e;
+  if (!zc)
+    if (int e = check_cuda(h, cudaMemcpyAsync(st + out_off, out, rb.bytes(), cudaMemcpyDeviceToHost, s), "search_host: D2H results")) return e;
+  if (int e = check_cuda(h, cudaStreamSynchronize(s), "search_host: stream sync")) return e;
+  rb.unpack(st + out_off, top_scores_host, top_ids_host, top_counts_host);
   return B200MS_OK;
 }
 

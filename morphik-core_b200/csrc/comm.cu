@@ -85,11 +85,6 @@ static int check_nccl(b200ms_t* h, ncclResult_t r, const char* what) {
                                         (a.GetErrorString ? a.GetErrorString(r) : "?") + ")");
 }
 
-// Exchange layout of one rank's top-k list (what the all-gather moves, and what launch_merge_gathered reads):
-//   [n_q*k int64 global page ids][n_q*k float32 scores], padded to a multiple of 16 bytes so that every rank's block of the
-//   gathered buffer starts 8-byte aligned (n_q*k*12 alone is not: 1 query x 7 entries = 84 bytes);  unused entries: id -1, -inf.
-static inline size_t xchg_bytes(int n_q, int k) { return (size_t(n_q) * size_t(k) * 12 + 15) & ~size_t(15); }
-
 constexpr int kSlots = 2;
 
 struct Comm {
@@ -286,35 +281,33 @@ B200MS_API int b200ms_allgather_topk(b200ms_t* h, void* nccl_comm, const void* x
 }
 
 // ---- pipelined sharded search ----------------------------------------------------------------------------------------
-static int sharded_begin(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
-                         const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev, float i8_q_scale,
-                         float score_scale, int64_t id_base, float* ts, int64_t* ti, int32_t* tc, cudaStream_t s, int* slot_out) {
+// r's outputs receive the merged result (on the communication stream)
+static int sharded_begin(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, int* slot_out) {
   if (int e = ensure_comm_state(h)) return e;
   Comm* c = h->comm;
   const int world = c->world;
-  if (n_q < 1 || k < 1 || k > B200MS_MAX_K || int64_t(world) * k > 2 * B200MS_MAX_K)
+  if (r.n_q < 1 || r.k < 1 || r.k > B200MS_MAX_K || int64_t(world) * r.k > 2 * B200MS_MAX_K)
     return set_error(h, B200MS_EINVAL, "sharded_search: bad arguments (n_q >= 1, world * k <= 8192)");
   if (world > 1 && !c->comm) return set_error(h, B200MS_ESTATE, "sharded_search: call b200ms_comm_init first");
   const int slot = int(c->ticket % kSlots);
-  const size_t xb = xchg_bytes(n_q, k);
+  const size_t xb = xchg_bytes(r.n_q, r.k);
   if (c->used[slot]) {
     // the slot's previous exchange must have left the send buffer before the local top-k overwrites it
     if (int e = check_cuda(h, cudaStreamWaitEvent(s, c->ev_gathered[slot], 0), "sharded_search: wait gathered")) return e;
   }
   if (int e = reserve(h, c->xchg[slot], xb)) return e;
   if (int e = reserve(h, c->gath[slot], xb * size_t(world))) return e;
-  if (int e = reserve(h, c->lcount[slot], size_t(n_q) * 4)) return e;
-  uint8_t* x = static_cast<uint8_t*>(c->xchg[slot].p);
-  int64_t* xi = reinterpret_cast<int64_t*>(x);
-  float* xs = reinterpret_cast<float*>(x + size_t(n_q) * k * 8);
+  if (int e = reserve(h, c->lcount[slot], size_t(r.n_q) * 4)) return e;
+  void* x = c->xchg[slot].p;
   // local scan + top-k with global ids, written straight into the exchange layout (the local counts are not exchanged:
   // unused entries carry id -1; they go to scratch so that a caller reusing its output buffers across pipelined steps
   // never has two streams writing top_counts)
-  const uint32_t* allow = n_masks > 0 ? allow_masks_dev : nullptr;
-  const int32_t* mi = n_masks > 0 ? mask_index_dev : nullptr;
-  if (int e = search_core(h, q_dev, src_dtype, q_lens, n_q, k, allow, i8_q_scale, score_scale, id_base, xs, xi,
-                          static_cast<int32_t*>(c->lcount[slot].p), s, nullptr, mi, (h->corpus.n_pages + 31) / 32, nullptr, nullptr))
-    return e;
+  const ResultBlock xl(r.n_q, r.k);
+  SearchRequest local = r;
+  local.top_ids = xl.ids(x);
+  local.top_scores = xl.scores(x);
+  local.top_counts = static_cast<int32_t*>(c->lcount[slot].p);
+  if (int e = search_core(h, local, m, s)) return e;
   if (int e = check_cuda(h, cudaEventRecord(c->ev_local[slot], s), "sharded_search: record local")) return e;
   if (int e = check_cuda(h, cudaStreamWaitEvent(c->cstream, c->ev_local[slot], 0), "sharded_search: wait local")) return e;
   if (world > 1) {
@@ -322,7 +315,9 @@ static int sharded_begin(b200ms_t* h, const void* q_dev, int src_dtype, const in
     h->launches++;
   }
   if (int e = check_cuda(h, cudaEventRecord(c->ev_gathered[slot], c->cstream), "sharded_search: record gathered")) return e;
-  if (int e = launch_merge_gathered(h, world > 1 ? c->gath[slot].p : x, world, n_q, k, ts, ti, tc, c->cstream)) return e;
+  if (int e = launch_merge_gathered(h, world > 1 ? c->gath[slot].p : x, world, r.n_q, r.k, r.top_scores, r.top_ids,
+                                    r.top_counts, c->cstream))
+    return e;
   c->used[slot] = true;
   *slot_out = slot;
   return B200MS_OK;
@@ -337,10 +332,13 @@ B200MS_API int64_t b200ms_sharded_search_begin(b200ms_t* h, const void* q_dev, i
       n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
     return set_error(h, B200MS_EINVAL, "sharded_search_begin: bad arguments");
   DeviceGuard g(h->device);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev, id_base};
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
   int slot = 0;
-  if (int e = sharded_begin(h, q_dev, src_dtype, q_lens, n_q, k, allow_masks_dev, n_masks, mask_index_dev, i8_q_scale, score_scale,
-                            id_base, top_scores_dev, top_ids_dev, top_counts_dev, static_cast<cudaStream_t>(stream), &slot))
-    return e;
+  if (int e = sharded_begin(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream), &slot)) return e;
   Comm* c = h->comm;
   if (int e = check_cuda(h, cudaEventRecord(c->ev_done[slot], c->cstream), "sharded_search: record done")) return e;
   return c->ticket++;
@@ -370,24 +368,25 @@ B200MS_API int64_t b200ms_sharded_search_host_begin(b200ms_t* h, const float* q_
     return set_error(h, B200MS_ESTATE, "sharded_search_host_begin: two searches are in flight -- collect the older one with "
                                        "b200ms_sharded_search_host_end first");
   cudaStream_t s = h->stream;
-  int64_t rows = 0;
-  for (int i = 0; i < n_q; ++i) rows += q_lens[i] > 0 ? q_lens[i] : 0;
-  const size_t nk = size_t(n_q) * size_t(k > 0 ? k : 0);
-  const size_t out_bytes = (nk * 12 + size_t(n_q) * 4 + 15) & ~size_t(15);
-  if (int e = reserve(h, c->q_raw[slot], size_t(rows > 0 ? rows : 1) * kDim * 4)) return e;
-  if (int e = reserve(h, c->out_dev[slot], out_bytes)) return e;
-  if (int e = reserve_pinned(h, c->out_pin[slot], out_bytes)) return e;
-  if (rows > 0)
-    if (int e = check_cuda(h, cudaMemcpyAsync(c->q_raw[slot].p, q_host, size_t(rows) * kDim * 4, cudaMemcpyHostToDevice, s),
+  const SearchMeta m = build_search_meta(q_lens, n_q);
+  const ResultBlock rb(n_q, k);
+  if (int e = reserve(h, c->q_raw[slot], size_t(m.rows > 0 ? m.rows : 1) * kDim * 4)) return e;
+  if (int e = reserve(h, c->out_dev[slot], rb.bytes())) return e;
+  if (int e = reserve_pinned(h, c->out_pin[slot], rb.bytes())) return e;
+  if (m.rows > 0)
+    if (int e = check_cuda(h, cudaMemcpyAsync(c->q_raw[slot].p, q_host, size_t(m.rows) * kDim * 4, cudaMemcpyHostToDevice, s),
                            "sharded_search_host: H2D queries"))
       return e;
-  uint8_t* od = static_cast<uint8_t*>(c->out_dev[slot].p);
+  void* od = c->out_dev[slot].p;
+  SearchRequest r{c->q_raw[slot].p, B200MS_F32, q_lens, n_q, k, i8_q_scale, score_scale, rb.scores(od), rb.ids(od), rb.counts(od),
+                  id_base};
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
   int sl = 0;
-  if (int e = sharded_begin(h, c->q_raw[slot].p, B200MS_F32, q_lens, n_q, k, allow_masks_dev, n_masks, mask_index_dev, i8_q_scale,
-                            score_scale, id_base, reinterpret_cast<float*>(od + nk * 8), reinterpret_cast<int64_t*>(od),
-                            reinterpret_cast<int32_t*>(od + nk * 12), s, &sl))
-    return e;
-  if (int e = check_cuda(h, cudaMemcpyAsync(c->out_pin[slot].p, od, out_bytes, cudaMemcpyDeviceToHost, c->cstream),
+  if (int e = sharded_begin(h, r, m, s, &sl)) return e;
+  if (int e = check_cuda(h, cudaMemcpyAsync(c->out_pin[slot].p, od, rb.bytes(), cudaMemcpyDeviceToHost, c->cstream),
                          "sharded_search_host: D2H results"))
     return e;
   if (int e = check_cuda(h, cudaEventRecord(c->ev_done[slot], c->cstream), "sharded_search_host: record done")) return e;
@@ -406,11 +405,7 @@ B200MS_API int b200ms_sharded_search_host_end(b200ms_t* h, int64_t ticket, float
   DeviceGuard g(h->device);
   const int slot = int(ticket % kSlots);
   if (int e = check_cuda(h, cudaEventSynchronize(c->ev_done[slot]), "sharded_search_host_end: sync")) return e;
-  const size_t nk = size_t(c->out_nq[slot]) * size_t(c->out_k[slot]);
-  const uint8_t* o = static_cast<const uint8_t*>(c->out_pin[slot].p);
-  memcpy(top_ids_host, o, nk * 8);
-  memcpy(top_scores_host, o + nk * 8, nk * 4);
-  memcpy(top_counts_host, o + nk * 12, size_t(c->out_nq[slot]) * 4);
+  ResultBlock(c->out_nq[slot], c->out_k[slot]).unpack(c->out_pin[slot].p, top_scores_host, top_ids_host, top_counts_host);
   c->host_pending[slot] = false;
   return B200MS_OK;
 }

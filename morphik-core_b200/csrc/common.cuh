@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstring>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -30,14 +31,80 @@ struct DeviceGuard {  // switch to the handle's device for the duration of a cal
   explicit DeviceGuard(int dev);
   ~DeviceGuard();
 };
-// candidate list(s) of a rerank call: ids (device int64, -1 = unused slot); per_query = 0: one list of n_cand ids shared by
-// every query; 1: [n_q, roundup(n_cand,32)] -- one list per query
-struct SearchCand {
+struct Comm;  // comm.cu: NCCL communicator + the exchange pipeline of the sharded search
+
+// query groups rounded up to whole 128-row MMA tiles: the row count of a packed query block and of a group-score matrix
+inline int64_t groups_padded(int64_t groups) { return (groups + 3) & ~int64_t(3); }
+
+// Candidate list(s) of a search (ids: device int64, -1 = unused slot).
+//   ids == NULL           : scan the whole corpus, scores indexed by page id.
+//   ids, per_query == 0   : ONE list of n_cand page ids scored by every query, scores indexed by slot.
+//   ids, per_query == 1   : one list PER QUERY laid out as [n_q, stride()]: query q owns slots [q*stride, q*stride + n_cand)
+//                           and only its own groups are scored against them.
+struct CandSpec {
   const int64_t* ids = nullptr;
   int n_cand = 0;
   int per_query = 0;
+  int64_t stride() const { return per_query ? (int64_t(n_cand) + 31) & ~int64_t(31) : 0; }
+  int64_t n_slots(int n_q) const { return per_query ? stride() * n_q : n_cand; }
 };
-struct Comm;  // comm.cu: NCCL communicator + the exchange pipeline of the sharded search
+
+// Layout of n items (queries, or pages) of lens[i] rows, each padded to whole 32-row groups, as ONE host block that is
+// uploaded with one copy or read in place from mapped pinned memory:
+//   [ss int64 (n+1) true-row offsets | ds int64 (n+1) padded-row offsets | goff int32 (n+1) group offsets, 16 B aligned |
+//    ntok int32 (groups_padded, at least 4) true tokens per group]
+// Without groups (pages) the block ends after ds.
+struct SearchMeta {
+  std::vector<uint8_t> host;
+  size_t off_ds = 0, off_goff = 0, off_ntok = 0;  // ss is at offset 0
+  int64_t n = 0, rows = 0, padded_rows = 0, groups = 0, groups_padded = 0;
+  const int32_t* goff() const { return reinterpret_cast<const int32_t*>(host.data() + off_goff); }
+};
+// NULL lens or n < 0 give the empty layout (search_core rejects such a request)
+SearchMeta build_search_meta(const int32_t* lens, int64_t n, bool with_groups = true);
+// true tokens of every group: item i's lens[i] tokens fill groups [goff[i], goff[i+1]) 32 at a time; groups at or past
+// n_groups are skipped
+void group_tokens(const int32_t* lens, int64_t n, const int32_t* goff, int64_t n_groups, int32_t* ntok);
+
+// One search: pack queries -> score -> top-k.  Device pointers, except that q and the outputs may be mapped pinned memory.
+struct SearchRequest {
+  const void* q = nullptr;  // rows [sum q_lens,128] of q_dtype (F32 | BF16)
+  int q_dtype = B200MS_F32;
+  const int32_t* q_lens = nullptr;  // HOST
+  int n_q = 0;
+  int k = 0;
+  float i8_q_scale = 1.f;
+  float score_scale = 1.f;
+  float* top_scores = nullptr;   // [n_q, k]
+  int64_t* top_ids = nullptr;    // [n_q, k]
+  int32_t* top_counts = nullptr; // [n_q]
+  int64_t id_base = 0;
+  const uint32_t* allow = nullptr;       // allow-mask bits over the pages (NULL = all); with mask_index: [n_masks, words]
+  const int32_t* mask_index = nullptr;   // per query: row of `allow` (-1 = no mask); NULL = the one mask for every query
+  CandSpec cand;                         // ids == NULL: full scan
+};
+
+// Results of a search as one block: [n_q*k int64 ids | n_q*k f32 scores | n_q int32 counts], padded to 16 bytes, so that
+// a host entry point copies them back with one D2H.  Its first two parts are the exchange layout of the sharded search.
+struct ResultBlock {
+  size_t n_q, nk;
+  ResultBlock(int n_q_, int k) : n_q(size_t(n_q_)), nk(size_t(n_q_) * size_t(k > 0 ? k : 0)) {}
+  size_t bytes() const { return (nk * 12 + n_q * 4 + 15) & ~size_t(15); }
+  int64_t* ids(void* b) const { return static_cast<int64_t*>(b); }
+  float* scores(void* b) const { return reinterpret_cast<float*>(static_cast<uint8_t*>(b) + nk * 8); }
+  int32_t* counts(void* b) const { return reinterpret_cast<int32_t*>(static_cast<uint8_t*>(b) + nk * 12); }
+  void unpack(const void* b, float* ts, int64_t* ti, int32_t* tc) const {  // -> host arrays
+    const uint8_t* p = static_cast<const uint8_t*>(b);
+    memcpy(ti, p, nk * 8);
+    memcpy(ts, p + nk * 8, nk * 4);
+    memcpy(tc, p + nk * 12, n_q * 4);
+  }
+};
+
+// Exchange layout of one rank's top-k list (what the all-gather moves, and what launch_merge_gathered reads):
+//   [n_q*k int64 global page ids][n_q*k float32 scores], padded to a multiple of 16 bytes so that every rank's block of the
+//   gathered buffer starts 8-byte aligned (n_q*k*12 alone is not: 1 query x 7 entries = 84 bytes);  unused entries: id -1, -inf.
+inline size_t xchg_bytes(int n_q, int k) { return (size_t(n_q) * size_t(k) * 12 + 15) & ~size_t(15); }
 
 // Which chunk ranges a scoring launch walks.  Full scan: the corpus' own unit plan, scores indexed by page id.
 // Candidate ("slot") mode: unit j = the chunk range of candidate page j, scores indexed by j.
@@ -142,14 +209,21 @@ int ensure_smem(b200ms_t* h, const void* kernel, int smem, const char* what);
 int make_tmap_rows(b200ms_t* h, CUtensorMap* out, const void* base, int dtype, int64_t n_rows, int box_rows,
                    int64_t row_bytes = 0);
 void comm_teardown(b200ms_t* h);
-// pack -> score -> top-k on stream s (api.cu); meta_in_place / meta_host_block: see the definition
-int search_core(b200ms_t* h, const void* q_src, int src_dtype, const int32_t* q_lens, int n_q, int k,
-                const uint32_t* allow_dev, float i8_q_scale, float score_scale, int64_t id_base, float* ts, int64_t* ti,
-                int32_t* tc, cudaStream_t s, const SearchCand* cand, const int32_t* mask_index_dev, int64_t mask_stride,
-                const void* meta_in_place, const void* meta_host_block);
+// pack -> score -> top-k of r on stream s (api.cu); m = build_search_meta(r.q_lens, r.n_q).  meta_dev != NULL: m's block
+// already sits in device-readable memory at this address (mapped pinned staging) -- no upload; else ONE cudaMemcpyAsync.
+int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev = nullptr);
+
+// Full scan: unit u = chunks [unit_start[u], unit_start[u+1]) of the attached corpus, scores indexed by page id
+inline UnitPlan full_scan_plan(const b200ms_t* h) {
+  UnitPlan p;
+  p.start = static_cast<const int32_t*>(h->unit_start.p);
+  p.end = p.start + 1;
+  p.n_units = h->corpus.n_units;
+  return p;
+}
 
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
-int launch_score_wgmma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, int n_groups_real, void* group_scores,
+int launch_score_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_packed, int n_groups_real, void* group_scores,
                        int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
 int launch_score_b1(b200ms_t* h, const int64_t* cand_ids, int64_t n_cand, const void* q_packed, int n_groups,
                     const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo, int g_hi);
@@ -161,7 +235,6 @@ int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_
 int launch_cand_units(b200ms_t* h, const int64_t* cand_ids, int n_cand, int32_t* unit_start, int32_t* unit_end,
                       uint32_t* slot_mask, cudaStream_t s);
 int launch_hamming_batch(b200ms_t* h, const void* q, const void* cand, int64_t n, uint32_t* out, cudaStream_t s);
-int launch_sign_pack(b200ms_t* h, const void* x, int src_dtype, int64_t rows, uint8_t* out, cudaStream_t s);
 int launch_chunk_page(b200ms_t* h, const int64_t* page_start_dev, int64_t n_pages, int32_t* chunk_page, cudaStream_t s);
 int launch_pack_rows(b200ms_t* h, const void* src, int src_dtype, const int64_t* src_start_dev,
                      const int64_t* dst_start_dev, int64_t n_items, int64_t dst_rows, int pad_mode, void* dst,

@@ -513,20 +513,11 @@ static int query_tmap(b200ms_t* h, const void* q, int dtype, int n_q_rows) {
 
 // m_tile_lo / m_tile_hi: score only query tiles [m_tile_lo, m_tile_hi) (hi < 0: all) -- the batched rerank walks the query
 // tiles one launch at a time, each against its own candidate units.
-int launch_score_wgmma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, int n_groups_real, void* group_scores,
+int launch_score_wgmma(b200ms_t* h, const UnitPlan& up, const void* q_packed, int n_groups_real, void* group_scores,
                        int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
   const Corpus& c = h->corpus;
-  UnitPlan up;
-  if (plan) {
-    up = *plan;
-  } else {  // full scan: unit u = [unit_start[u], unit_start[u+1])
-    up.start = static_cast<const int32_t*>(h->unit_start.p);
-    up.end = up.start + 1;
-    up.n_units = c.n_units;
-    up.slot_mode = 0;
-  }
   if (!c.has_tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
-  const int n_groups_padded = (n_groups_real + 3) & ~3;
+  const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_mtiles = n_groups_padded / 4;
   const int n_q_rows = n_groups_padded * kGroup;
   if (c.dtype == B200MS_F8) {  // the A operand of the f16 MMA: the e4m3 query rows widened to f16
@@ -558,8 +549,7 @@ int launch_score_wgmma(b200ms_t* h, const UnitPlan* plan, const void* q_packed, 
 // expanding producer.
 int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
                           void* group_scores, int64_t ld, cudaStream_t s) {
-  const Corpus& c = h->corpus;
-  const int n_groups_padded = (n_groups_real + 3) & ~3;
+  const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_rows = n_groups_padded * kGroup;
   if (int e = reserve(h, h->b1_q_i8, size_t(n_rows) * 128 + 1024)) return e;
   if (int e = reserve(h, h->b1_tok_const, size_t(n_rows) * 4)) return e;
@@ -570,12 +560,8 @@ int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
   if (int e = query_tmap(h, q_i8, B200MS_I8, n_rows)) return e;
-  UnitPlan up;
-  up.start = static_cast<const int32_t*>(h->unit_start.p);
-  up.end = up.start + 1;
-  up.n_units = c.n_units;
-  up.slot_mode = 0;
-  return launch_tiles<1, true>(h, up, h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
+  return launch_tiles<1, true>(h, full_scan_plan(h), h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4,
+                               group_scores, ld, s);
 }
 
 }  // namespace bms

@@ -439,10 +439,8 @@ int launch_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand
 int launch_merge_gathered(b200ms_t* h, const void* gathered, int world, int n_q, int k, float* top_scores, int64_t* top_ids,
                           int32_t* top_counts, cudaStream_t s) {
   if (n_q <= 0) return B200MS_OK;
-  const int64_t n = int64_t(n_q) * k;
-  const int64_t block = (n * 12 + 15) & ~int64_t(15);  // = b200ms_xchg_bytes(n_q, k): every rank's block starts aligned
   return launch_merge_impl<float>(h, nullptr, nullptr, nullptr, n_q, world * k, k, 1.0f, top_scores, top_ids, top_counts, s,
-                                  static_cast<const uint8_t*>(gathered), k, block, n * 8);
+                                  static_cast<const uint8_t*>(gathered), k, int64_t(xchg_bytes(n_q, k)), int64_t(n_q) * k * 8);
 }
 
 }  // namespace bms
