@@ -23,8 +23,10 @@
 //                   two 64-row wgmma A blocks: block h holds tokens 16h .. 16h+15 of each of the four groups, so warp w of the
 //                   warpgroup ends up holding all 32 tokens of group w (rows l/4 and l/4+8 of both blocks) and sums its
 //                   group with warp shuffles only.  Per patch tile and query tile: two m64n128 wgmma chains (8 x k16 for
-//                   bf16 / f16, 4 x k32 for int8), per-thread max over the 8 columns of every chunk it holds, a quad
-//                   shuffle for the other 24, a running max per (token, page), and at a page end the group's sum.
+//                   bf16 / f16, 4 x k32 for int8), each issued before the previous one is reduced (two accumulator sets,
+//                   also across query-tile and patch-tile boundaries), per-lane running maxima over the 8 columns of every
+//                   chunk a lane holds, and at a page end a quad shuffle for the other 24 columns and the group's sum.
+// Registers: setmaxnreg moves the producer warpgroup's share to the consumers (RegPlan).
 // 1-bit:  128 - ham(q, d) = (128 - popc(q)) + <q', d'>  with q' = +1 / -1 per query bit and d' = 1 / 0 per document bit, so
 //         max_r (128 - ham) = c_t + max_r <q'_t, d'_r> runs as the int8 kernel plus a per-token constant c_t (0 for padding).
 #include "common.cuh"
@@ -35,6 +37,20 @@ namespace bms {
 
 constexpr int kThreads = 384;
 constexpr uint32_t kQBlockBytes = 64 * 128;  // one 64-row A block of one 128-byte panel
+
+// Registers per thread of each warpgroup role.  __launch_bounds__(kThreads, 1) gives every thread kLaunchRegs registers;
+// setmaxnreg moves them from the producer warpgroup to the two consumer warpgroups, which hold two 64-register accumulator
+// sets each.  setmaxnreg.inc blocks until the CTA's pool has the registers, so budgets that overdraw the pool would hang
+// the kernel: the static_assert rules that out.  One TMA thread needs 40; the fp8 widener (16 uint4 of loads per thread)
+// and the 1-bit expander (a ring of 8 uint4) spill below about 90.  The budgets are the splits ptxas compiled with the
+// fewest spills (none, except the consumers of the 1-bit kernel with NM = 8).
+constexpr int kLaunchRegs = (65536 / kThreads) & ~7;  // 168
+template <int KIND, bool BITS>
+struct RegPlan {
+  static constexpr int kProducer = BITS ? 104 : KIND == 2 ? 120 : 40;
+  static constexpr int kConsumer = BITS ? 200 : KIND == 2 ? 192 : 232;
+  static_assert(kProducer + 2 * kConsumer <= 3 * kLaunchRegs, "register budgets overdraw the CTA's pool");
+};
 
 // ------------------------------------------------------------------ 1-bit query side: bits -> +-1 int8 rows + token constants
 __global__ void __launch_bounds__(256)
@@ -172,8 +188,10 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
   }
   __syncthreads();
 
+  using Regs = RegPlan<KIND, BITS>;
   if (warp < 4) {
     // ================================================================ producer warpgroup
+    if constexpr (Regs::kProducer > 0) setmaxnreg_dec<Regs::kProducer>();
     if (threadIdx.x == 0) {
       // query tile m, block h, group g: rows 32g + 16h .. +16 of the tile -> rows 16g .. 16g+15 of A block h
       const uint64_t pol_q = policy_evict_last();
@@ -330,122 +348,142 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
   const int wg = (warp >> 2) - 1;
   const int w = warp & 3;  // group w of every query tile this warpgroup owns
   if (wg >= NWG) return;
+  if constexpr (Regs::kConsumer > 0) setmaxnreg_inc<Regs::kConsumer>();
   mbar_wait(qfull, 0);
   const uint32_t q_addr = smem_u32(smem_q);
   const uint32_t st_addr = smem_u32(smem_st);
+  // A block of query tile i of this warpgroup (tile m = wg + 2i < NM for every i < MPW)
+  auto a_block = [&](int i) { return q_addr + uint32_t(wg + 2 * i) * K::kTileBytes; };
 
+  // runmax: this lane's running max of its 8 columns per chunk, per (query tile, token); the quad's four lanes together
+  // hold the token's max, combined at flush.
   Acc runmax[MPW][4];
-  Acc cnst[MPW][4];
-  int cur_page[MPW];
 #pragma unroll
-  for (int i = 0; i < MPW; ++i) {
-    const int mt = m_tile_base + wg + 2 * i;
-    const bool active = (wg + 2 * i) < NM && mt * 4 + w < n_groups_real;
+  for (int i = 0; i < MPW; ++i)
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      runmax[i][k] = Acc(0);
-      cnst[i][k] = Acc(0);
-      if constexpr (BITS) {  // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w
-        if (active) cnst[i][k] = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2));
-      }
-    }
-    cur_page[i] = -1;
-  }
+    for (int k = 0; k < 4; ++k) runmax[i][k] = Acc(0);
 
-  auto flush = [&](int i, int u) {
+  // score of page `page` (unit u in slot_mode) for the group of query tile i; page < 0: nothing accumulated yet
+  auto flush = [&](int i, int u, int page) {
     const int mt = m_tile_base + wg + 2 * i;
     const int group = mt * 4 + w;
-    if (group < n_groups_real && cur_page[i] >= 0) {
-      const int o = slot_mode ? u : cur_page[i];
+    if (group < n_groups_real && page >= 0) {
+      const int o = slot_mode ? u : page;
       Acc v[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) v[k] = clamp_token_max(clamp_bits, o, runmax[i][k]) + cnst[i][k];
+      for (int k = 0; k < 4; ++k) {
+        Acc cnst = Acc(0);
+        // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w; read here, not held in registers
+        if constexpr (BITS)
+          cnst = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2));
+        v[k] = clamp_token_max(clamp_bits, o, quad_max(runmax[i][k])) + cnst;
+      }
       const Acc s = group_sum(v);
       if (lane == 0) group_scores[int64_t(group) * ld + o] = s;
     }
   };
 
+  // The warpgroup's wgmma blocks form one stream: per patch tile, per query tile i, the A blocks h = 0 and h = 1.  Every
+  // tile holds an even number of blocks, so block h always accumulates in acc0 (h = 0) or acc1 (h = 1).  The next block's
+  // chain is issued before the current block is reduced, also across query-tile and patch-tile boundaries, so the
+  // warpgroup keeps a chain on the tensor pipe while it runs its epilogue.  The next tile's first chain is retired at the end of the iteration, after the
+  // last block's epilogue and the next tile's bookkeeping: ptxas serialises every wgmma of a loop that carries a pending
+  // wgmma group across its back-edge.
+  Acc acc0[64], acc1[64];
   int stage = 0;
   uint32_t phase = 0;
   int last_u = -1;
+  int cur_page = -1;  // page of the running maxima (the same for every query tile: all walk the same chunks)
+  int pg[4];          // page of each chunk of the tile; -1: past the end of the unit
+  bool same = false;  // all four chunks continue cur_page (the common case)
   TileIter it;
   it.u = blockIdx.x;
   it.load(unit_start, unit_end, n_units);
-  for (; it.valid(n_units); it.next(unit_start, unit_end, n_units)) {
+  auto begin_tile = [&]() {
     if (it.u != last_u) {  // new unit: units end on page boundaries
-      if (last_u >= 0) {
 #pragma unroll
-        for (int i = 0; i < MPW; ++i) flush(i, last_u);
-      }
-#pragma unroll
-      for (int i = 0; i < MPW; ++i) cur_page[i] = -1;
+      for (int i = 0; i < MPW; ++i) flush(i, last_u, cur_page);
+      cur_page = -1;
       last_u = it.u;
     }
     const int cb = it.c0 + 4 * it.t;
-    int pg[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) pg[j] = (cb + j < it.c1) ? __ldg(chunk_page + cb + j) : -1;
-    mbar_wait(&full[stage], phase);
+    same = pg[0] == cur_page && pg[1] == cur_page && pg[2] == cur_page && pg[3] == cur_page;
+  };
+  // Every chain is issued unconditionally, the ones past the last tile included (their results are dropped and no producer
+  // writes a stage any more by then): a chain on a data-dependent path also makes ptxas serialise the wgmmas.
+  if (it.valid(n_units)) {
+    begin_tile();
+    mbar_wait(&full[0], 0);
+  }
+  wgmma_fence();
+  mma_chain<KIND>(acc0, a_block(0), st_addr);
+  wgmma_wait<0>();
+  while (it.valid(n_units)) {
+    TileIter nx = it;
+    nx.next(unit_start, unit_end, n_units);
+    int nstage = stage + 1;
+    uint32_t nphase = phase;
+    if (nstage == num_stages) {
+      nstage = 0;
+      nphase ^= 1;
+    }
     const uint32_t b_addr = st_addr + uint32_t(stage) * K::kTileBytes;
 #pragma unroll
     for (int i = 0; i < MPW; ++i) {
-      const int m = wg + 2 * i;
-      if (m >= NM) break;
-      const uint32_t a_addr = q_addr + uint32_t(m) * K::kTileBytes;
-      Acc d0[64], d1[64];
+      Acc cm[4][4];  // [token k][chunk]: this lane's partial maxima
       wgmma_fence();
-      mma_chain<KIND>(d0, a_addr, b_addr);
-      mma_chain<KIND>(d1, a_addr + kQBlockBytes, b_addr);
-      Acc cm[4][4];  // [token k][chunk]
-      {
-        wgmma_wait<1>();
-        reg_fence_all(d0);
-        Acc c2[2][4];
-        chunk_maxima(d0, c2);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          cm[0][c] = c2[0][c];
-          cm[1][c] = c2[1][c];
-        }
+      mma_chain<KIND>(acc1, a_block(i) + kQBlockBytes, b_addr);
+      wgmma_wait<1>();
+      reg_fence_all(acc0);
+      chunk_maxima(acc0, cm[0], cm[1]);
+      if (i + 1 < MPW) {
+        wgmma_fence();
+        mma_chain<KIND>(acc0, a_block(i + 1), b_addr);
+      } else {  // the next tile's first block
+        if (nx.valid(n_units)) mbar_wait(&full[nstage], nphase);
+        wgmma_fence();
+        mma_chain<KIND>(acc0, a_block(0), st_addr + uint32_t(nstage) * K::kTileBytes);
       }
-      {
-        wgmma_wait<0>();
-        reg_fence_all(d1);
-        if (i == MPW - 1 || m + 2 >= NM) {  // every read of this stage has completed
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[stage]);
-        }
-        Acc c2[2][4];
-        chunk_maxima(d1, c2);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          cm[2][c] = c2[0][c];
-          cm[3][c] = c2[1][c];
-        }
+      wgmma_wait<1>();
+      reg_fence_all(acc1);
+      if (i == MPW - 1) {  // every read of this stage has completed
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[stage]);
       }
+      chunk_maxima(acc1, cm[2], cm[3]);
+      if (same) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (pg[j] < 0) continue;  // chunk belongs to the next unit
-        if (pg[j] != cur_page[i]) {
-          flush(i, it.u);
-          cur_page[i] = pg[j];
+        for (int k = 0; k < 4; ++k)
+          runmax[i][k] = acc_max(acc_max(runmax[i][k], acc_max(cm[k][0], cm[k][1])), acc_max(cm[k][2], cm[k][3]));
+      } else {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) runmax[i][k] = cm[k][j];
-        } else {
+        for (int j = 0; j < 4; ++j) {
+          if (pg[j] < 0) continue;  // chunk belongs to the next unit
+          const int prev = j == 0 ? cur_page : pg[j - 1];
+          if (pg[j] != prev) {
+            flush(i, it.u, prev);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) runmax[i][k] = acc_max(runmax[i][k], cm[k][j]);
+            for (int k = 0; k < 4; ++k) runmax[i][k] = cm[k][j];
+          } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) runmax[i][k] = acc_max(runmax[i][k], cm[k][j]);
+          }
         }
       }
     }
-    if (++stage == num_stages) {
-      stage = 0;
-      phase ^= 1;
-    }
-  }
-  if (last_u >= 0) {
 #pragma unroll
-    for (int i = 0; i < MPW; ++i) flush(i, last_u);
+    for (int j = 0; j < 4; ++j)
+      if (pg[j] >= 0) cur_page = pg[j];
+    it = nx;
+    stage = nstage;
+    phase = nphase;
+    if (it.valid(n_units)) begin_tile();
+    wgmma_wait<0>();
   }
+#pragma unroll
+  for (int i = 0; i < MPW; ++i) flush(i, last_u, cur_page);
 }
 
 // ---------------------------------------------------------------------------------------------- host side

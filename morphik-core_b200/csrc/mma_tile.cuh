@@ -37,10 +37,11 @@ __device__ __forceinline__ int acc_max(int a, int b) { return max(a, b); }
 __device__ __forceinline__ float acc_max3(float a, float b, float c) { return fmax3(a, b, c); }
 __device__ __forceinline__ int acc_max3(int a, int b, int c) { return imax3(a, b, c); }
 
-// m64n128 accumulator fragment (ptx.cuh) -> cm[i][c] = max over the 32 columns of chunk c (columns 32c .. 32c+31) of this
-// thread's token row i (0: row l/4, 1: row l/4 + 8), reduced over the four lanes of the quad that share the row.
+// m64n128 accumulator fragment (ptx.cuh) -> r0[c] / r1[c] = max over this thread's 8 of the 32 columns of chunk c (columns
+// 32c .. 32c+31) of its token row l/4 (r0) and l/4 + 8 (r1).  The other 24 columns live in the other lanes of the quad: max
+// is exact and order-free, so callers keep per-lane partial maxima and combine the quad once, with quad_max.
 template <typename Acc>
-__device__ __forceinline__ void chunk_maxima(const Acc (&d)[64], Acc (&cm)[2][4]) {
+__device__ __forceinline__ void chunk_maxima(const Acc (&d)[64], Acc (&r0)[4], Acc (&r1)[4]) {
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
     Acc a = acc_max(d[16 * c + 0], d[16 * c + 1]);
@@ -50,16 +51,16 @@ __device__ __forceinline__ void chunk_maxima(const Acc (&d)[64], Acc (&cm)[2][4]
       a = acc_max3(a, d[4 * j + 0], d[4 * j + 1]);
       b = acc_max3(b, d[4 * j + 2], d[4 * j + 3]);
     }
-    cm[0][c] = a;
-    cm[1][c] = b;
+    r0[c] = a;
+    r1[c] = b;
   }
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      cm[i][c] = acc_max(cm[i][c], __shfl_xor_sync(0xffffffffu, cm[i][c], 1));
-      cm[i][c] = acc_max(cm[i][c], __shfl_xor_sync(0xffffffffu, cm[i][c], 2));
-    }
+}
+
+// max over the four lanes of a quad (the lanes that share an accumulator row)
+template <typename Acc>
+__device__ __forceinline__ Acc quad_max(Acc v) {
+  v = acc_max(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return acc_max(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
 // zero_pad_compat (option "zero_pad_compat"): colpali_engine's score_multi_vector pads every batch of pages with zero rows

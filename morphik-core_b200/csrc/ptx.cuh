@@ -75,6 +75,20 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
+// ---------------------------------------------------------------- per-warpgroup register budgets
+// Every warp of the warpgroup executes these.  dec returns registers to the CTA's pool; inc blocks until the pool holds
+// the requested registers, so the budgets of all warpgroups must fit in what the launch allocated (see RegPlan).
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  static_assert(N >= 24 && N <= 256 && N % 8 == 0, "setmaxnreg: 24..256, multiple of 8");
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  static_assert(N >= 24 && N <= 256 && N % 8 == 0, "setmaxnreg: 24..256, multiple of 8");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---------------------------------------------------------------- L2 policies + TMA
 __device__ __forceinline__ uint64_t policy_evict_first() {
   uint64_t p;
