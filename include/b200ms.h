@@ -103,6 +103,25 @@ int b200ms_pack_pages(b200ms_t* h, const void* src, int src_dtype, const int32_t
  * rows: [b200ms_padded_rows(page_lens), 128] of dtype BF16|I8|F8|B1, 1024-byte aligned.  page_lens (HOST) are the
  * TRUE lengths.  Builds the chunk->page table, the work-unit plan and the TMA descriptor. */
 int b200ms_set_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages);
+/* ---- host-resident corpus: patch rows in pinned host memory, only the rerank candidates cross PCIe ----------------------
+ * Replaces the reference's multivector storage outside the ANN index (load_multivector_from_storage,
+ * fast_multivector_store.py:545-548, :713-774): the FDE matrix stays in HBM, the packed rows stay in host RAM.
+ * set_corpus_host: same layout and arguments as b200ms_set_corpus, but rows_host is pinned, device-mapped host memory
+ *   (b200ms_host_alloc; anything else -> B200MS_EINVAL), 16-byte aligned.  Only b200ms_rerank_device /
+ *   b200ms_rerank_batch_device score it: every rerank call dedups the valid candidate pages of the whole call, gathers them
+ *   over PCIe into a library-owned HBM staging block (rounds of at most option "host_stage_bytes") and runs the same scorers
+ *   on it -- scores, ids, counts and tie order are bit-identical to an HBM corpus of the same rows.  Such a call
+ *   synchronises the caller's stream once (one small D2H of the plan) and is never graph-captured.  Full scans
+ *   (b200ms_score, b200ms_search_*, b200ms_sharded_search_*) return B200MS_ESTATE.  b200ms_fde_encode_corpus reads a bf16
+ *   host corpus through the mapping.
+ * host_alloc / host_free: cudaHostAlloc(Mapped | Portable) of exactly `bytes` (the caller owns and frees the block; host_free
+ *   also accepts a NULL handle, for a block that outlives its handle).
+ * last_gather_stats: of the last host-tier rerank call: unique pages gathered, bytes copied (padded rows x row bytes),
+ *   gather rounds, and the device time (ms, CUDA events) of the gather kernels; synchronises. */
+int b200ms_set_corpus_host(b200ms_t* h, const void* rows_host, int dtype, const int32_t* page_lens, int64_t n_pages);
+int b200ms_host_alloc(b200ms_t* h, int64_t bytes, void** out);
+int b200ms_host_free(b200ms_t* h, void* p);
+int b200ms_last_gather_stats(b200ms_t* h, int64_t* unique_pages, int64_t* bytes, int* rounds, float* ms);
 int64_t b200ms_corpus_pages(const b200ms_t* h);
 int64_t b200ms_corpus_rows(const b200ms_t* h);
 
@@ -283,7 +302,9 @@ int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas);
  *   "host_graph"      1 (default): small unmasked host searches (pack -> score -> top-k) are captured into a CUDA graph on their
  *                     second use and replayed as one launch; 0 = three plain launches (same results)
  *   "fde_gemm"        1 (default): FDE scan on wgmma when fde_dim % 64 == 0, 0 = SIMT scan
- *   "unit_rows", "max_ctas"   work-unit size (needs a new b200ms_set_corpus) and launch width. */
+ *   "unit_rows", "max_ctas"   work-unit size (needs a new b200ms_set_corpus) and launch width.
+ *   "host_stage_bytes" host-resident corpora: HBM staging budget of one gather round (default 2 GiB, raised to the largest
+ *                     page); a rerank call whose unique candidate pages need more runs in rounds (same results). */
 int b200ms_set_option(b200ms_t* h, const char* name, int64_t value);
 
 #ifdef __cplusplus

@@ -14,6 +14,10 @@ namespace bms {
 static std::mutex g_err_mu;
 static std::string g_err;
 
+static const char* const kHostFullScan =
+    "host-resident corpus (b200ms_set_corpus_host): only candidate scoring (b200ms_rerank_device / b200ms_rerank_batch_device) "
+    "is supported; full scans would stream the whole corpus over PCIe";
+
 int set_error(b200ms_t* h, int code, const std::string& msg) {
   if (h) h->err = msg;
   std::lock_guard<std::mutex> lk(g_err_mu);
@@ -268,9 +272,11 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->meta, &h->meta_b, &h->q_raw, &h->q_packed, &h->scores, &h->mask, &h->mask_index, &h->out_all,
                        &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->b1_q_i8, &h->b1_tok_const, &h->f8_q_f16,
                        &h->fde_simhash, &h->fde_ams_index, &h->fde_ams_sign, &h->fde_tmp, &h->fde_q_bf16, &h->fde_final_index,
-                       &h->fde_final_sign};
+                       &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
+                       &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
+  for (cudaEvent_t e : h->ht_ev) cudaEventDestroy(e);
   if (h->stage.p) cudaFreeHost(h->stage.p);
   for (int i = 0; i < b200ms_t::kEvRing; ++i) {
     if (h->ev0[i]) cudaEventDestroy(h->ev0[i]);
@@ -325,6 +331,8 @@ B200MS_API int b200ms_set_option(b200ms_t* h, const char* name, int64_t value) {
     h->unit_rows = value;
   } else if (n == "max_ctas" && value >= 0) {
     h->max_ctas = int(value);
+  } else if (n == "host_stage_bytes" && value > 0) {
+    h->host_stage_bytes = value;
   } else {
     return set_error(h, B200MS_EINVAL, "set_option: unknown option or bad value: " + n);
   }
@@ -404,27 +412,35 @@ B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, co
 }
 
 // ------------------------------------------------------------------------------------------------ corpus
-B200MS_API int b200ms_set_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages) {
-  if (!h) return B200MS_EINVAL;
-  if (!corpus_dtype_ok(dtype) || n_pages < 0 || (n_pages > 0 && (!rows || !page_lens)))
-    return set_error(h, B200MS_EINVAL, "set_corpus: bad arguments");
-  if (n_pages > 0 && (reinterpret_cast<uintptr_t>(rows) & 1023))
-    return set_error(h, B200MS_EINVAL, "set_corpus: rows must be 1024-byte aligned");
+// Page tables of a corpus; an HBM corpus also gets its work-unit plan, chunk table and TMA descriptor.  A host-resident one
+// (rows = the device address of mapped pinned memory) is only ever read by the candidate gather, which needs page_start.
+static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages, bool host) {
   DeviceGuard g(h->device);
   cudaStream_t s = h->stream;
   Corpus c;
   c.rows = rows;
   c.dtype = dtype;
   c.n_pages = n_pages;
+  c.host = host;
   std::vector<int64_t> ps(size_t(n_pages) + 1);
   ps[0] = 0;
   for (int64_t i = 0; i < n_pages; ++i) {
     ps[i + 1] = ps[i] + b200ms_padded_len(page_lens[i]);
     if (page_lens[i] <= 0) c.has_empty = true;
+    if (ps[i + 1] - ps[i] > c.max_page_rows) c.max_page_rows = ps[i + 1] - ps[i];
   }
   c.n_rows = ps[n_pages];
   c.n_chunks = c.n_rows / kGroup;
   if (c.n_chunks >= (int64_t(1) << 31)) return set_error(h, B200MS_EINVAL, "set_corpus: more than 2^31 chunks");
+  if (host) {
+    if (int e = upload(h, h->page_start, ps.data(), ps.size() * 8, s)) return e;
+    if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
+    h->page_len_host.assign(page_lens, page_lens + n_pages);
+    if (int e = check_cuda(h, cudaStreamSynchronize(s), "set_corpus_host: stream sync")) return e;
+    h->corpus = c;
+    h->generation++;
+    return B200MS_OK;
+  }
   // work units: runs of whole pages of about unit_rows rows; unit_start in chunks
   // (small corpora: shrink the units so that every SM still gets about four of them -- a 100-page corpus as 25 units
   // of 4096 rows would leave 123 SMs idle)
@@ -461,6 +477,79 @@ B200MS_API int b200ms_set_corpus(b200ms_t* h, const void* rows, int dtype, const
   return B200MS_OK;
 }
 
+B200MS_API int b200ms_set_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages) {
+  if (!h) return B200MS_EINVAL;
+  if (!corpus_dtype_ok(dtype) || n_pages < 0 || (n_pages > 0 && (!rows || !page_lens)))
+    return set_error(h, B200MS_EINVAL, "set_corpus: bad arguments");
+  if (n_pages > 0 && (reinterpret_cast<uintptr_t>(rows) & 1023))
+    return set_error(h, B200MS_EINVAL, "set_corpus: rows must be 1024-byte aligned");
+  return attach_corpus(h, rows, dtype, page_lens, n_pages, false);
+}
+
+B200MS_API int b200ms_set_corpus_host(b200ms_t* h, const void* rows_host, int dtype, const int32_t* page_lens, int64_t n_pages) {
+  if (!h) return B200MS_EINVAL;
+  if (!corpus_dtype_ok(dtype) || n_pages < 0 || (n_pages > 0 && (!rows_host || !page_lens)))
+    return set_error(h, B200MS_EINVAL, "set_corpus_host: bad arguments");
+  if (reinterpret_cast<uintptr_t>(rows_host) & 15)
+    return set_error(h, B200MS_EINVAL, "set_corpus_host: rows must be 16-byte aligned");
+  DeviceGuard g(h->device);
+  const void* dev = nullptr;
+  if (rows_host) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, rows_host) != cudaSuccess) {
+      cudaGetLastError();
+      return set_error(h, B200MS_EINVAL, "set_corpus_host: cudaPointerGetAttributes failed on rows");
+    }
+    if (a.type != cudaMemoryTypeHost || !a.devicePointer)
+      return set_error(h, B200MS_EINVAL, "set_corpus_host: rows must be pinned, device-mapped host memory (b200ms_host_alloc)");
+    dev = a.devicePointer;
+  }
+  return attach_corpus(h, dev, dtype, page_lens, n_pages, true);
+}
+
+B200MS_API int b200ms_host_alloc(b200ms_t* h, int64_t bytes, void** out) {
+  if (!h) return B200MS_EINVAL;
+  if (!out || bytes < 0) return set_error(h, B200MS_EINVAL, "host_alloc: bad arguments");
+  *out = nullptr;
+  DeviceGuard g(h->device);
+  // exact size: the caller's corpus may be most of host RAM
+  if (cudaError_t e = cudaHostAlloc(out, size_t(bytes > 0 ? bytes : 16), cudaHostAllocMapped | cudaHostAllocPortable);
+      e != cudaSuccess) {
+    *out = nullptr;
+    cudaGetLastError();
+    return set_error(h, B200MS_ENOMEM, "cudaHostAlloc of " + std::to_string(bytes) + " pinned bytes failed");
+  }
+  return B200MS_OK;
+}
+
+B200MS_API int b200ms_host_free(b200ms_t* h, void* p) {
+  if (!p) return B200MS_OK;
+  if (!h) {  // the handle is already gone: pinned blocks are portable, any context frees them
+    if (cudaFreeHost(p) == cudaSuccess) return B200MS_OK;
+    return check_cuda(nullptr, cudaGetLastError(), "cudaFreeHost");
+  }
+  DeviceGuard g(h->device);
+  return check_cuda(h, cudaFreeHost(p), "cudaFreeHost");
+}
+
+B200MS_API int b200ms_last_gather_stats(b200ms_t* h, int64_t* unique_pages, int64_t* bytes, int* rounds, float* ms) {
+  if (!h) return B200MS_EINVAL;
+  DeviceGuard g(h->device);
+  float total = 0.f;
+  for (int r = 0; r < h->ht_rounds; ++r) {
+    float t = 0.f;
+    if (cudaEventSynchronize(h->ht_ev[2 * r + 1]) != cudaSuccess ||
+        cudaEventElapsedTime(&t, h->ht_ev[2 * r], h->ht_ev[2 * r + 1]) != cudaSuccess)
+      return check_cuda(h, cudaGetLastError(), "last_gather_stats: gather events");
+    total += t;
+  }
+  if (unique_pages) *unique_pages = h->ht_unique;
+  if (bytes) *bytes = h->ht_bytes;
+  if (rounds) *rounds = h->ht_rounds;
+  if (ms) *ms = total;
+  return B200MS_OK;
+}
+
 // zero_pad_compat, full scan: pages are "batched" in page-id order, zero_pad_batch at a time (score_multi_vector's
 // batch_size, 128 upstream); a page shorter than the longest of its batch gets its per-token maxima clamped at 0.
 // Built on the host once per (corpus, batch size) and cached on the device.
@@ -487,12 +576,15 @@ static int ensure_clamp_pages(b200ms_t* h, cudaStream_t s, const uint32_t** out)
 }
 
 // ------------------------------------------------------------------------------------------------ hot path
-// Candidate mode of the wgmma scorers: unit j = the chunk range of candidate slot j, scores indexed by j.
-static int candidate_plan(b200ms_t* h, const CandSpec& cs, int n_q, cudaStream_t s, UnitPlan* plan) {
+// Candidate mode of the wgmma scorers: unit j = the chunk range of candidate slot j, scores indexed by j.  The units come
+// from unit_ids, page ids of v (cs.ids, or their staging-block remap for a host-resident corpus); the zero_pad_compat
+// clamp bits always come from cs.ids, the corpus page ids.
+static int candidate_plan(b200ms_t* h, const CorpusView& v, const int64_t* unit_ids, const CandSpec& cs, int n_q,
+                          cudaStream_t s, UnitPlan* plan) {
   const int n_slots = int(cs.n_slots(n_q));
   if (int e = reserve(h, h->cand_start, size_t(n_slots) * 4)) return e;
   if (int e = reserve(h, h->cand_end, size_t(n_slots) * 4)) return e;
-  if (int e = launch_cand_units(h, cs.ids, n_slots, static_cast<int32_t*>(h->cand_start.p),
+  if (int e = launch_cand_units(h, v, unit_ids, n_slots, static_cast<int32_t*>(h->cand_start.p),
                                 static_cast<int32_t*>(h->cand_end.p), nullptr, s))
     return e;
   plan->start = static_cast<const int32_t*>(h->cand_start.p);
@@ -511,8 +603,9 @@ static int candidate_plan(b200ms_t* h, const CandSpec& cs, int n_q, cudaStream_t
 
 // Per-query candidate lists on wgmma: one launch per 128-token query tile, the tile's queries against THEIR candidate
 // lists only (a contiguous slot range).
-static int score_wgmma_per_query(b200ms_t* h, const UnitPlan& plan, const CandSpec& cs, const void* q_packed, int n_groups,
-                                 const int32_t* goff, int n_q, void* group_scores, int64_t ld, cudaStream_t s) {
+static int score_wgmma_per_query(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const CandSpec& cs,
+                                 const void* q_packed, int n_groups, const int32_t* goff, int n_q, void* group_scores,
+                                 int64_t ld, cudaStream_t s) {
   const int n_mtiles = int(groups_padded(n_groups)) / 4;
   int q_lo = 0;
   for (int m = 0; m < n_mtiles; ++m) {
@@ -528,13 +621,16 @@ static int score_wgmma_per_query(b200ms_t* h, const UnitPlan& plan, const CandSp
     sub.n_units = int(int64_t(q_hi - q_lo) * cs.stride());
     if (sub.clamp_bits) sub.clamp_bits += s0 / 32;
     void* sc = static_cast<uint8_t*>(group_scores) + size_t(s0) * 4;
-    if (int e = launch_score_wgmma(h, sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
+    if (int e = launch_score_wgmma(h, v, sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
   }
   return B200MS_OK;
 }
 
+// Scores the rows of v.  unit_ids: the candidate slots as page ids of v (cs.ids unless v is a staging block); fill = false
+// skips the zero-fill (a later gather round of a host-resident corpus adds its slots to the same matrix).
 static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* goff, int n_q, const int32_t* ntok_dev,
-                      void* group_scores, int64_t ld, const CandSpec& cs, cudaStream_t s) {
+                      void* group_scores, int64_t ld, const CandSpec& cs, cudaStream_t s, const CorpusView& v,
+                      const int64_t* unit_ids, bool fill = true) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "score: no corpus attached (call b200ms_set_corpus first)");
   const int64_t n_items = cs.ids ? cs.n_slots(n_q) : c.n_pages;
@@ -552,12 +648,12 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   // zero-fill what no launch writes: the tile kernels skip pages with zero rows and unused candidate slots; the per-query
   // POPC launches write only their own query's groups and slots
   const bool zero_fill = b1 ? (b1_wgmma && c.has_empty) || cs.per_query : c.has_empty || cs.ids;
-  if (zero_fill)
+  if (zero_fill && fill)
     if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(groups_padded(n_groups)) * size_t(ld) * 4, s), "score: memset"))
       return e;
   UnitPlan plan = full_scan_plan(h);
   if (!b1) {
-    if (int e = cs.ids ? candidate_plan(h, cs, n_q, s, &plan) : ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
+    if (int e = cs.ids ? candidate_plan(h, v, unit_ids, cs, n_q, s, &plan) : ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
   }
   // ev0 / ev1 bracket the scoring launches only (b200ms_score_times_ms): bench.py derives the roofline's achieved figure
   // from this time
@@ -570,14 +666,14 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   } else if (b1 && cs.per_query) {
     for (int q = 0; q < n_q && !e; ++q)
       if (goff[q + 1] > goff[q])
-        e = launch_score_b1(h, cs.ids + int64_t(q) * cs.stride(), cs.n_cand, q_packed, n_groups, ntok_dev,
+        e = launch_score_b1(h, v, unit_ids + int64_t(q) * cs.stride(), cs.n_cand, q_packed, n_groups, ntok_dev,
                             static_cast<int32_t*>(group_scores) + int64_t(q) * cs.stride(), ld, s, goff[q], goff[q + 1]);
   } else if (b1) {
-    e = launch_score_b1(h, cs.ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups);
+    e = launch_score_b1(h, v, unit_ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups);
   } else if (cs.per_query) {
-    e = score_wgmma_per_query(h, plan, cs, q_packed, n_groups, goff, n_q, group_scores, ld, s);
+    e = score_wgmma_per_query(h, v, plan, cs, q_packed, n_groups, goff, n_q, group_scores, ld, s);
   } else {
-    e = launch_score_wgmma(h, plan, q_packed, n_groups, group_scores, ld, s);
+    e = launch_score_wgmma(h, v, plan, q_packed, n_groups, group_scores, ld, s);
   }
   if (e) return e;
   if (!h->capturing) {
@@ -590,6 +686,7 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
 B200MS_API int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* q_lens,
                             const int32_t* group_offsets, int n_q, void* group_scores, int64_t ld, void* stream) {
   if (!h) return B200MS_EINVAL;
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kHostFullScan);
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int32_t* ntok_dev = nullptr;
@@ -601,7 +698,8 @@ B200MS_API int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, con
     if (int e = upload(h, h->meta, ntok.data(), ntok.size() * 4, s)) return e;
     ntok_dev = static_cast<const int32_t*>(h->meta.p);
   }
-  return score_impl(h, q_packed, n_groups, group_offsets, n_q, ntok_dev, group_scores, ld, CandSpec{}, s);
+  return score_impl(h, q_packed, n_groups, group_offsets, n_q, ntok_dev, group_scores, ld, CandSpec{}, s, corpus_view(h),
+                    nullptr);
 }
 
 static int score_time_of(b200ms_t* h, int64_t idx, float* ms) {
@@ -663,6 +761,8 @@ namespace bms {
 int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "search: no corpus attached (call b200ms_set_corpus first)");
+  if (c.host && !r.cand.ids) return set_error(h, B200MS_ESTATE, kHostFullScan);
+  if (c.host && h->capturing) return set_error(h, B200MS_ESTATE, "search: a host-resident corpus cannot be graph-captured");
   const int n_q = r.n_q;
   if (n_q < 1 || !r.q_lens || !r.q || r.k < 1 || r.k > B200MS_MAX_K || !r.top_scores || !r.top_ids || !r.top_counts)
     return set_error(h, B200MS_EINVAL, "search: bad arguments (n_q >= 1, 1 <= k <= 4096)");
@@ -691,7 +791,25 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
                                  r.i8_q_scale, s))
       return e;
   const int ng = int(m.groups);
-  if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s)) return e;
+  if (!c.host) {
+    if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s, corpus_view(h), cs.ids)) return e;
+  } else if (ng > 0 && n_items > 0) {
+    struct Ctx {
+      const void* q;
+      int ng;
+      const int32_t* goff;
+      int n_q;
+      const int32_t* ntok;
+      int64_t ld;
+      const CandSpec* cs;
+      cudaStream_t s;
+    } ctx{h->q_packed.p, ng, m.goff(), n_q, ntok_dev, ld, &cs, s};
+    auto round = [](b200ms_t* hh, const CorpusView& v, const int64_t* unit_ids, void* scores, bool fill, void* p) {
+      const Ctx& x = *static_cast<const Ctx*>(p);
+      return score_impl(hh, x.q, x.ng, x.goff, x.n_q, x.ntok, scores, x.ld, *x.cs, x.s, v, unit_ids, fill);
+    };
+    if (int e = score_host_tier(h, cs, n_q, gp, ld, h->scores.p, s, round, &ctx)) return e;
+  }
   if (ng == 0 || n_items == 0) {
     // nothing scored: every page (if any) has score 0 -- still a defined ranking
     if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "search: memset")) return e;
@@ -704,7 +822,8 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   // candidate mode: rank the slots (ties -> lower slot = better first-stage rank), report the page ids; unused slots masked
   const int n_slots = int(cs.n_slots(n_q));
   if (int e = reserve(h, h->cand_mask, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
-  if (int e = launch_cand_units(h, cs.ids, n_slots, nullptr, nullptr, static_cast<uint32_t*>(h->cand_mask.p), s)) return e;
+  if (int e = launch_cand_units(h, corpus_view(h), cs.ids, n_slots, nullptr, nullptr, static_cast<uint32_t*>(h->cand_mask.p), s))
+    return e;
   return launch_topk(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, static_cast<const uint32_t*>(h->cand_mask.p), r.k,
                      r.score_scale, 0, cs.ids, r.top_scores, r.top_ids, r.top_counts, s, nullptr, 0, cs.stride());
 }
@@ -849,6 +968,7 @@ static int search_host_impl(b200ms_t* h, const float* q_host, const int32_t* q_l
                             const uint32_t* masks_host, int n_masks, const int32_t* mask_index_host, float i8_q_scale,
                             float score_scale, int64_t id_base, float* top_scores_host, int64_t* top_ids_host,
                             int32_t* top_counts_host) {
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kHostFullScan);
   if (n_q < 1 || !q_lens || !q_host || k < 1 || k > B200MS_MAX_K || !top_scores_host || !top_ids_host || !top_counts_host)
     return set_error(h, B200MS_EINVAL, "search_host: bad arguments (n_q >= 1, 1 <= k <= 4096)");
   DeviceGuard g(h->device);

@@ -323,11 +323,15 @@ static int sharded_begin(b200ms_t* h, const SearchRequest& r, const SearchMeta& 
   return B200MS_OK;
 }
 
+static const char* const kShardedHostCorpus =
+    "sharded search: the attached corpus is host-resident (b200ms_set_corpus_host); only candidate scoring is supported";
+
 B200MS_API int64_t b200ms_sharded_search_begin(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
                                                int k, const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
                                                float i8_q_scale, float score_scale, int64_t id_base, float* top_scores_dev,
                                                int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream) {
   if (!h) return B200MS_EINVAL;
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kShardedHostCorpus);
   if ((src_dtype != B200MS_F32 && src_dtype != B200MS_BF16) || !top_scores_dev || !top_ids_dev || !top_counts_dev ||
       n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
     return set_error(h, B200MS_EINVAL, "sharded_search_begin: bad arguments");
@@ -358,6 +362,7 @@ B200MS_API int64_t b200ms_sharded_search_host_begin(b200ms_t* h, const float* q_
                                                     const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
                                                     float i8_q_scale, float score_scale, int64_t id_base) {
   if (!h) return B200MS_EINVAL;
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kShardedHostCorpus);
   if (!q_host || !q_lens || n_q < 1 || n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
     return set_error(h, B200MS_EINVAL, "sharded_search_host_begin: bad arguments");
   DeviceGuard g(h->device);

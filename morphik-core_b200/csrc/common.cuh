@@ -129,6 +129,20 @@ struct Corpus {
   bool has_tmap = false;
   bool has_empty = false;  // some page has zero rows (its score is the memset 0)
   int64_t clamp_batch = 0;  // zero_pad_compat batch size the full-scan clamp bitmask (b200ms::clamp_pages) was built for
+  bool host = false;        // rows live in mapped pinned host memory (b200ms_set_corpus_host): candidate scoring only
+  int64_t max_page_rows = 0;  // largest padded page
+};
+
+// The packed rows a scoring launch reads: the attached corpus, or -- for a host-resident corpus -- the HBM staging block
+// one gather round filled (a packed corpus of its own: pages 0..n, chunk_page and page_start local to the block).
+struct CorpusView {
+  const void* rows = nullptr;
+  int dtype = -1;
+  int64_t n_pages = 0;  // candidate ids outside [0, n_pages) are unused slots
+  int64_t n_rows = 0;
+  const CUtensorMap* tmap = nullptr;  // NULL: no TMA descriptor (1-bit rows)
+  const int32_t* chunk_page = nullptr;
+  const int64_t* page_start = nullptr;
 };
 
 }  // namespace bms
@@ -193,7 +207,17 @@ struct b200ms {
   uint64_t graph_clock = 0;
   int host_graph = 1;        // option "host_graph": replay small unmasked host searches as one CUDA graph
   bool capturing = false;    // inside stream capture: no event timing, no allocation
-
+  // host-resident corpus (host_tier.cu): per-call dedup / plan scratch and the HBM staging block of the gathered pages
+  int64_t host_stage_bytes = int64_t(2) << 30;  // option "host_stage_bytes": staging budget per gather round
+  bms::DeviceBuf ht_bitmap, ht_wpre, ht_uniq, ht_stage_off, ht_hdr, ht_remap, ht_ps, ht_chunk_page, ht_scores;
+  bms::DeviceBuf ht_stage;           // staging rows (1024-byte aligned inside the allocation)
+  CUtensorMap ht_tmap;               // TMA descriptor of the staging block, re-encoded when the block moves
+  const void* ht_tmap_base = nullptr;
+  int ht_tmap_dtype = -1;
+  int64_t ht_tmap_rows = 0;
+  std::vector<cudaEvent_t> ht_ev;    // event pairs around each round's gather (last call)
+  int64_t ht_unique = 0, ht_bytes = 0;
+  int ht_rounds = 0;
 };
 
 namespace bms {
@@ -222,18 +246,40 @@ inline UnitPlan full_scan_plan(const b200ms_t* h) {
   return p;
 }
 
+// The attached corpus as the scorers see it
+inline CorpusView corpus_view(const b200ms_t* h) {
+  const Corpus& c = h->corpus;
+  CorpusView v;
+  v.rows = c.rows;
+  v.dtype = c.dtype;
+  v.n_pages = c.n_pages;
+  v.n_rows = c.n_rows;
+  v.tmap = c.has_tmap ? &c.tmap : nullptr;
+  v.chunk_page = static_cast<const int32_t*>(h->chunk_page.p);
+  v.page_start = static_cast<const int64_t*>(h->page_start.p);
+  return v;
+}
+
+// Candidate scoring of a host-resident corpus (host_tier.cu): dedup the candidate pages of the call, gather them into the
+// staging block in rounds of at most host_stage_bytes, score every round through score_round.  Synchronises s once.
+int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_t ld, void* group_scores, cudaStream_t s,
+                    int (*score_round)(b200ms_t*, const CorpusView&, const int64_t* unit_ids, void* scores, bool fill,
+                                       void* ctx),
+                    void* ctx);
+
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
-int launch_score_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_packed, int n_groups_real, void* group_scores,
-                       int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
-int launch_score_b1(b200ms_t* h, const int64_t* cand_ids, int64_t n_cand, const void* q_packed, int n_groups,
-                    const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo, int g_hi);
+int launch_score_wgmma(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const void* q_packed, int n_groups_real,
+                       void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
+int launch_score_b1(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
+                    int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,
+                    int g_hi);
 int launch_pad_cands(b200ms_t* h, const int64_t* src, int n_cand, int n_lists, int64_t stride, int64_t* dst, cudaStream_t s);
 int launch_clamp_slots(b200ms_t* h, const int64_t* cand_ids, int n_cand, int n_lists, int64_t list_stride, int batch,
                        uint32_t* clamp_bits, cudaStream_t s);
 int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
                           void* group_scores, int64_t ld, cudaStream_t s);
-int launch_cand_units(b200ms_t* h, const int64_t* cand_ids, int n_cand, int32_t* unit_start, int32_t* unit_end,
-                      uint32_t* slot_mask, cudaStream_t s);
+int launch_cand_units(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int n_cand, int32_t* unit_start,
+                      int32_t* unit_end, uint32_t* slot_mask, cudaStream_t s);
 int launch_hamming_batch(b200ms_t* h, const void* q, const void* cand, int64_t n, uint32_t* out, cudaStream_t s);
 int launch_chunk_page(b200ms_t* h, const int64_t* page_start_dev, int64_t n_pages, int32_t* chunk_page, cudaStream_t s);
 int launch_pack_rows(b200ms_t* h, const void* src, int src_dtype, const int64_t* src_start_dev,

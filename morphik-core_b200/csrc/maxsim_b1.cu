@@ -82,16 +82,16 @@ maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ pag
   }
 }
 
-int launch_score_b1(b200ms_t* h, const int64_t* cand_ids, int64_t n_cand, const void* q_packed, int n_groups,
-                    const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo, int g_hi) {
-  const Corpus& c = h->corpus;
+int launch_score_b1(b200ms_t* h, const CorpusView& c, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
+                    int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,
+                    int g_hi) {
   const int64_t n_items = cand_ids ? n_cand : c.n_pages;
   if (n_items == 0 || n_groups == 0) return B200MS_OK;
   int64_t want = (n_items + kB1Warps - 1) / kB1Warps;
   const int64_t cap = int64_t(h->num_sms) * 8;
   const int grid = int(want < cap ? want : cap);
   const uint4* rows = static_cast<const uint4*>(c.rows);
-  const int64_t* ps = static_cast<const int64_t*>(h->page_start.p);
+  const int64_t* ps = c.page_start;
   const uint4* qb = static_cast<const uint4*>(q_packed);
   int32_t* out = static_cast<int32_t*>(group_scores);
   // groups [g_lo, g_hi) only (the batched rerank scores each query against its own candidate list)

@@ -488,10 +488,9 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
 
 // ---------------------------------------------------------------------------------------------- host side
 template <int KIND, int NM, bool BITS>
-static int launch_one(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const, int m_tile_base,
-                      int n_groups_real, void* scores, int64_t ld, cudaStream_t s) {
+static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
+                      int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s) {
   using K = Kind<KIND>;
-  const Corpus& c = h->corpus;
   const uint32_t avail = kSmemLimit - 1024 /*align*/ - kBarrierBytes - NM * K::kTileBytes;
   int stages = int(avail / K::kTileBytes);
   if (stages > 8) stages = 8;
@@ -503,8 +502,9 @@ static int launch_one(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, co
   int grid = h->max_ctas > 0 ? h->max_ctas : h->num_sms;
   if (grid > up.n_units) grid = up.n_units;
   if (grid < 1) return B200MS_OK;
-  kern<<<grid, kThreads, smem, s>>>(c.tmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
-                                   static_cast<const int32_t*>(h->chunk_page.p), up.start, up.end, up.slot_mode, up.n_units,
+  static const CUtensorMap kNoTmap{};  // 1-bit rows: the producer expands bits and never issues TMA loads for them
+  kern<<<grid, kThreads, smem, s>>>(c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
+                                   c.chunk_page, up.start, up.end, up.slot_mode, up.n_units,
                                    m_tile_base, n_groups_real, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
                                    stages);
   h->launches++;
@@ -514,8 +514,8 @@ static int launch_one(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, co
 // Query tiles [base, base + nm) in one pass over the corpus.  nm is rounded up to a power of two: a phantom (all-zero) tile
 // costs less than a second pass over the corpus.
 template <int KIND, bool BITS>
-static int launch_tiles(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const, int n_groups_real,
-                        int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
+static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
+                        int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
   constexpr int kMaxNM = Kind<KIND>::kMaxNM;
   for (int base = m_lo; base < m_hi;) {
     const int rem = m_hi - base;
@@ -523,12 +523,12 @@ static int launch_tiles(b200ms_t* h, const UnitPlan& up, const CUtensorMap& tq, 
     while (nm < rem && nm < kMaxNM) nm <<= 1;
     int e;
     switch (nm) {
-      case 1: e = launch_one<KIND, 1, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
-      case 2: e = launch_one<KIND, 2, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
-      case 4: e = launch_one<KIND, 4, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 1: e = launch_one<KIND, 1, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 2: e = launch_one<KIND, 2, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 4: e = launch_one<KIND, 4, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
       default:
         if constexpr (kMaxNM >= 8) {
-          e = launch_one<KIND, 8, BITS>(h, up, tq, tok_const, base, n_groups_real, scores, ld, s);
+          e = launch_one<KIND, 8, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s);
         } else {
           e = set_error(h, B200MS_EINVAL, "maxsim_wgmma: bad NM");
         }
@@ -551,10 +551,9 @@ static int query_tmap(b200ms_t* h, const void* q, int dtype, int n_q_rows) {
 
 // m_tile_lo / m_tile_hi: score only query tiles [m_tile_lo, m_tile_hi) (hi < 0: all) -- the batched rerank walks the query
 // tiles one launch at a time, each against its own candidate units.
-int launch_score_wgmma(b200ms_t* h, const UnitPlan& up, const void* q_packed, int n_groups_real, void* group_scores,
-                       int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
-  const Corpus& c = h->corpus;
-  if (!c.has_tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
+int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const void* q_packed, int n_groups_real,
+                       void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
+  if (!c.tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
   const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_mtiles = n_groups_padded / 4;
   const int n_q_rows = n_groups_padded * kGroup;
@@ -576,9 +575,9 @@ int launch_score_wgmma(b200ms_t* h, const UnitPlan& up, const void* q_packed, in
     hi = m_tile_hi < n_mtiles ? m_tile_hi : n_mtiles;
   }
   switch (kind_of_dtype(c.dtype)) {
-    case 0: return launch_tiles<0, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
-    case 1: return launch_tiles<1, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
-    case 2: return launch_tiles<2, false>(h, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 0: return launch_tiles<0, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 1: return launch_tiles<1, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 2: return launch_tiles<2, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
     default: return set_error(h, B200MS_ESTATE, "score: corpus dtype has no wgmma scorer");
   }
 }
@@ -598,8 +597,8 @@ int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
   if (int e = query_tmap(h, q_i8, B200MS_I8, n_rows)) return e;
-  return launch_tiles<1, true>(h, full_scan_plan(h), h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4,
-                               group_scores, ld, s);
+  return launch_tiles<1, true>(h, corpus_view(h), full_scan_plan(h), h->tmap_q, tok_const, n_groups_real, 0,
+                               n_groups_padded / 4, group_scores, ld, s);
 }
 
 }  // namespace bms

@@ -185,11 +185,11 @@ int launch_pad_cands(b200ms_t* h, const int64_t* src, int n_cand, int n_lists, i
   return check_cuda(h, cudaGetLastError(), "launch pad_cands");
 }
 
-int launch_cand_units(b200ms_t* h, const int64_t* cand_ids, int n_cand, int32_t* unit_start, int32_t* unit_end,
-                      uint32_t* slot_mask, cudaStream_t s) {
+int launch_cand_units(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int n_cand, int32_t* unit_start,
+                      int32_t* unit_end, uint32_t* slot_mask, cudaStream_t s) {
   if (n_cand <= 0) return B200MS_OK;
-  cand_units_kernel<<<(n_cand + 255) / 256, 256, 0, s>>>(cand_ids, n_cand, static_cast<const int64_t*>(h->page_start.p),
-                                                        h->corpus.n_pages, unit_start, unit_end, slot_mask);
+  cand_units_kernel<<<(n_cand + 255) / 256, 256, 0, s>>>(cand_ids, n_cand, v.page_start, v.n_pages, unit_start, unit_end,
+                                                        slot_mask);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch cand_units");
 }

@@ -34,18 +34,56 @@ def _aligned_bytes(nbytes: int, device: torch.device, align: int = 1024) -> torc
     return raw[off:off + max(int(nbytes), 1)]
 
 
+class HostBlock:
+    """Pinned, device-mapped host memory of exactly ``nbytes`` (b200ms_host_alloc), freed by ``free`` or garbage collection.
+
+    torch's pinned allocator rounds requests up to a power of two, which would turn a 262 GB corpus into a 512 GB
+    reservation; this block is sized exactly.  ``tensor`` is a CPU uint8 view of it: views taken from it must not outlive
+    the block."""
+
+    def __init__(self, handle: "nat.Handle", nbytes: int):
+        p = ctypes.c_void_p()
+        handle.check(nat.lib.b200ms_host_alloc(handle.ptr, int(nbytes), ctypes.byref(p)), "b200ms_host_alloc")
+        self.handle, self.ptr, self.nbytes = handle, int(p.value), int(nbytes)
+        arr = np.ctypeslib.as_array((ctypes.c_uint8 * max(self.nbytes, 1)).from_address(self.ptr))
+        self.tensor = torch.from_numpy(arr)
+
+    def free(self):
+        if self.ptr:
+            self.tensor = None
+            nat.lib.b200ms_host_free(self.handle.ptr, ctypes.c_void_p(self.ptr))
+            self.ptr = 0
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 class MaxSimIndex:
     """Packed corpus of pages (each a [P_i, 128] matrix of patch embeddings) on one GPU.
 
     Layout in HBM: rows of ``row_bytes`` (bf16 256 B / int8 128 B / sign bits 16 B), every page padded to a
     multiple of 32 rows by repeating its last row, pages back to back in insertion order.  ``page id`` = insertion index.
+
+    ``tier="host"`` keeps the same packed rows in pinned host memory (``HostBlock``) instead of HBM, so the corpus is bounded
+    by host RAM rather than by the card: only ``rerank`` / ``rerank_batch`` work on it (each call copies just its candidate
+    pages over PCIe into an HBM staging block, with scores bit-identical to the HBM tier); the ``search_*`` full scans
+    raise ``NativeError``.  Growing the block allocates a new one and copies, so it briefly needs twice the corpus in
+    pinned memory; ``capacity_rows`` sizes the block once up front and avoids that.
     """
 
-    def __init__(self, device: int = 0, dtype: str = "bf16", i8_scale: float = 127.0, capacity_rows: int = 0):
+    def __init__(self, device: int = 0, dtype: str = "bf16", i8_scale: float = 127.0, capacity_rows: int = 0,
+                 tier: str = "hbm"):
         if dtype not in nat.DTYPE_NAMES or nat.DTYPE_NAMES[dtype] == nat.F32:
             raise ValueError(f"dtype must be one of bf16/int8/fp8/binary, got {dtype!r}")
+        if tier not in ("hbm", "host"):
+            raise ValueError(f"tier must be 'hbm' or 'host', got {tier!r}")
         if not torch.cuda.is_available():
             raise nat.NativeError("MaxSimIndex needs a CUDA device (H100); there is no CPU fallback")
+        self.tier = tier
+        self._block: Optional[HostBlock] = None  # host tier: owner of the memory self._buf views
         self.device = torch.device("cuda", int(device))
         self.dtype = nat.DTYPE_NAMES[dtype]
         self.dtype_name = dtype
@@ -119,16 +157,59 @@ class MaxSimIndex:
         return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     # ------------------------------------------------------------------ building the corpus
-    def _grow(self, need_rows: int):
+    def _grow(self, need_rows: int, exact: bool = False):
         if need_rows <= self._cap_rows:
             return
-        new_cap = max(need_rows, int(self._cap_rows * 1.5), 4096)
-        new_buf = _aligned_bytes(new_cap * self.row_bytes, self.device)
+        new_cap = need_rows if exact else max(need_rows, int(self._cap_rows * 1.5), 4096)
+        if self.tier == "host":
+            self._host_barrier()
+            block = HostBlock(self.h, new_cap * self.row_bytes)
+            new_buf = block.tensor
+        else:
+            new_buf = _aligned_bytes(new_cap * self.row_bytes, self.device)
         if self._buf is not None and self._rows:
             new_buf[: self._rows * self.row_bytes].copy_(self._buf[: self._rows * self.row_bytes])
+        if self.tier == "host":
+            if self._block is not None:
+                self._buf = None
+                self._block.free()
+            self._block = block
         self._buf = new_buf
         self._cap_rows = new_cap
         self._attached = False
+
+    def reserve_rows(self, rows: int):
+        """Make room for `rows` padded rows in total with one allocation of exactly that size (host tier: avoids the
+        transient second copy that growth needs)."""
+        self._grow(int(rows), exact=True)
+
+    def _host_barrier(self):
+        """A rerank of the host tier still queued on some stream may read the block: wait for the device before any host
+        write to it."""
+        if self.tier == "host" and self._block is not None:
+            torch.cuda.synchronize(self.device)
+
+    def host_tail(self, nbytes: int) -> np.ndarray:
+        """Host tier: writable uint8 view of the `nbytes` past the used rows (grown to fit) -- a shard file is read straight
+        into it; ``commit_rows`` then appends the pages it holds."""
+        if self.tier != "host":
+            raise ValueError("host_tail needs a host-tier index")
+        self._grow(self._rows + (int(nbytes) + self.row_bytes - 1) // self.row_bytes)
+        self._host_barrier()
+        o = self._rows * self.row_bytes
+        return self._buf[o:o + int(nbytes)].numpy()
+
+    def commit_rows(self, page_lens: Sequence[int]) -> Tuple[int, int]:
+        """Append pages whose packed rows were already written past the used rows (``host_tail``)."""
+        lens = [int(x) for x in page_lens]
+        need = int(nat.lib.b200ms_padded_rows(nat.i32_array(lens), len(lens)))
+        if self._rows + need > self._cap_rows:
+            raise ValueError("commit_rows: the rows were not written inside the block")
+        first = self.n_pages
+        self._rows += need
+        self._page_lens.extend(lens)
+        self._attached = False
+        return first, len(lens)
 
     def add_pages(self, pages: Sequence[ArrayLike]) -> Tuple[int, int]:
         """Append pages ([P_i,128] float32/bfloat16; numpy on host or torch on either side).  Returns (first id, count).
@@ -147,13 +228,19 @@ class MaxSimIndex:
         lens_c = nat.i32_array(lens)
         add_rows = int(nat.lib.b200ms_padded_rows(lens_c, len(lens)))
         self._grow(self._rows + add_rows)
-        dst = self._buf[self._rows * self.row_bytes:]
+        o = self._rows * self.row_bytes
+        # host tier: pack on the GPU into a device temporary, then one D2H copy into the block
+        dst = self._buf[o:] if self.tier == "hbm" else torch.empty(max(add_rows * self.row_bytes, 1), dtype=torch.uint8,
+                                                                     device=self.device)
         with torch.cuda.device(self.device):
             self.h.check(
                 nat.lib.b200ms_pack_pages(self.h.ptr, _vp(src), src_dtype, lens_c, len(lens), _vp(dst), self.dtype,
                                           ctypes.c_float(self.i8_scale), self._stream()),
                 "b200ms_pack_pages",
             )
+            if self.tier == "host" and add_rows:
+                self._host_barrier()
+                self._buf[o:o + add_rows * self.row_bytes].copy_(dst[: add_rows * self.row_bytes])
         self._rows += add_rows
         self._page_lens.extend(lens)
         self._attached = False
@@ -193,6 +280,11 @@ class MaxSimIndex:
     def adopt_packed(self, rows: torch.Tensor, page_lens: Sequence[int]):
         """Use an already packed device buffer (uint8 view or typed tensor, 1024-byte aligned, layout as described in the
         class docstring) as the corpus without copying -- bench.py builds its synthetic shard this way."""
+        if self.tier == "host":  # the rows move into a host block of exactly their size
+            self.clear()
+            self.reserve_rows(int(nat.lib.b200ms_padded_rows(nat.i32_array([int(x) for x in page_lens]), len(page_lens))))
+            self.append_packed(rows, page_lens)
+            return
         buf = rows.view(torch.uint8).reshape(-1)
         if buf.data_ptr() % 1024:
             raise ValueError("packed corpus must be 1024-byte aligned")
@@ -215,6 +307,7 @@ class MaxSimIndex:
             raise ValueError("packed buffer smaller than the page lengths imply")
         first = self.n_pages
         self._grow(self._rows + need)
+        self._host_barrier()
         self._buf[self._rows * self.row_bytes:(self._rows + need) * self.row_bytes].copy_(flat[: need * self.row_bytes])
         self._rows += need
         self._page_lens.extend(lens)
@@ -233,8 +326,12 @@ class MaxSimIndex:
         lens_c = nat.i32_array(self._page_lens)
         with torch.cuda.device(self.device):
             torch.cuda.current_stream(self.device).synchronize()  # pack kernels ran on torch's stream
-            self.h.check(nat.lib.b200ms_set_corpus(self.h.ptr, _vp(self._buf), self.dtype, lens_c, self.n_pages),
-                         "b200ms_set_corpus")
+            if self.tier == "host":
+                self.h.check(nat.lib.b200ms_set_corpus_host(self.h.ptr, _vp(self._buf) if self.n_pages else None, self.dtype,
+                                                            lens_c, self.n_pages), "b200ms_set_corpus_host")
+            else:
+                self.h.check(nat.lib.b200ms_set_corpus(self.h.ptr, _vp(self._buf), self.dtype, lens_c, self.n_pages),
+                             "b200ms_set_corpus")
         self._attached = True
 
     def clear(self):
@@ -251,6 +348,22 @@ class MaxSimIndex:
         pad = [(n + 31) // 32 * 32 for n in lens]
         starts = np.concatenate([[0], np.cumsum(pad)]).astype(np.int64)
         new_rows = int(sum(pad[p] for p in keep))
+        if self.tier == "host":  # in place: surviving runs move down with forward (overlap-safe) host copies
+            self._host_barrier()
+            base, dst, i = self._buf.data_ptr(), 0, 0
+            while i < len(keep):
+                j = i
+                while j + 1 < len(keep) and keep[j + 1] == keep[j] + 1:
+                    j += 1
+                a, b = int(starts[keep[i]]) * self.row_bytes, int(starts[keep[j] + 1]) * self.row_bytes
+                if dst != a:
+                    ctypes.memmove(base + dst, base + a, b - a)
+                dst += b - a
+                i = j + 1
+            self._rows = new_rows
+            self._page_lens = [lens[p] for p in keep]
+            self._attached = False
+            return
         new_buf = _aligned_bytes(max(new_rows, 4096) * self.row_bytes, self.device)
         dst = 0
         i = 0
@@ -267,10 +380,18 @@ class MaxSimIndex:
         self._attached = False
 
     def packed_rows(self) -> torch.Tensor:
-        """The packed corpus as a uint8 tensor [rows_padded, row_bytes] (a view)."""
+        """The packed corpus as a uint8 tensor [rows_padded, row_bytes] (a view; of host memory for the host tier)."""
         if self._buf is None:
-            return torch.empty((0, self.row_bytes), dtype=torch.uint8, device=self.device)
+            return torch.empty((0, self.row_bytes), dtype=torch.uint8, device=self.device if self.tier == "hbm" else "cpu")
         return self._buf[: self._rows * self.row_bytes].view(self._rows, self.row_bytes)
+
+    def gather_stats(self) -> dict:
+        """Of the last host-tier rerank call: unique pages gathered, bytes copied over PCIe (padded rows x row bytes),
+        staging rounds, and the device time of the gather kernels (ms); synchronises."""
+        u, b, r, ms = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int(), ctypes.c_float()
+        self.h.check(nat.lib.b200ms_last_gather_stats(self.h.ptr, ctypes.byref(u), ctypes.byref(b), ctypes.byref(r),
+                                                      ctypes.byref(ms)), "b200ms_last_gather_stats")
+        return {"unique_pages": int(u.value), "bytes": int(b.value), "rounds": int(r.value), "ms": float(ms.value)}
 
     # ------------------------------------------------------------------ queries
     @staticmethod
@@ -520,6 +641,27 @@ class MaxSimIndex:
         return ts, ti, tc
 
     # ------------------------------------------------------------------ candidate rerank (two-stage search)
+    def rerank(self, q_dev: torch.Tensor, q_lens: Sequence[int], cand_ids: torch.Tensor, k: int):
+        """Exact MaxSim of every query over ONE shared candidate list: cand_ids int64 [n_cand] on the device (-1 = unused
+        slot) -> (scores [n_q,k], page ids [n_q,k], counts [n_q]) on the device (b200ms_rerank_device)."""
+        self._attach()
+        n_q = len(q_lens)
+        if cand_ids.dtype != torch.int64 or not cand_ids.is_contiguous():
+            raise ValueError("cand_ids must be a contiguous int64 device tensor")
+        n_cand = int(cand_ids.numel())
+        kk = int(min(k, n_cand))
+        ts = torch.empty((n_q, kk), dtype=torch.float32, device=self.device)
+        ti = torch.empty((n_q, kk), dtype=torch.int64, device=self.device)
+        tc = torch.empty((n_q,), dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_rerank_device(self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32,
+                                             nat.i32_array(q_lens), n_q, _vp(cand_ids), n_cand, kk,
+                                             ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), _vp(ts), _vp(ti),
+                                             _vp(tc), self._stream()),
+                "b200ms_rerank_device")
+        return ts, ti, tc
+
     def rerank_batch(self, q_dev: torch.Tensor, q_lens: Sequence[int], cand_ids: torch.Tensor, k: int,
                      out: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
         """Exact MaxSim of every query over ITS OWN candidate list: cand_ids int64 [n_q, n_cand] on the device (-1 = unused
@@ -636,5 +778,9 @@ class MaxSimIndex:
                      "b200ms_sharded_search_host_end")
 
     def close(self):
-        self.h.close()
         self._buf = None
+        if self._block is not None:
+            torch.cuda.synchronize(self.device)
+            self._block.free()
+            self._block = None
+        self.h.close()

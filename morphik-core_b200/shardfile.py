@@ -70,18 +70,31 @@ def read_header(path: str) -> Tuple[dict, np.ndarray, int]:
     return header, lens, payload_off
 
 
-def load_index(path: str, device: int = 0, into: Optional[MaxSimIndex] = None) -> MaxSimIndex:
+def load_index(path: str, device: int = 0, into: Optional[MaxSimIndex] = None, tier: str = "hbm") -> MaxSimIndex:
     """Read a shard file straight into a 1024-byte-aligned device buffer and adopt it (no repacking); with ``into`` the
-    pages are APPENDED to an existing index of the same dtype (journal segments)."""
+    pages are APPENDED to an existing index of the same dtype (journal segments).  A host-tier index (``tier="host"``, or
+    ``into`` of that tier) reads the rows straight into its pinned host block, sized from the header, with no device copy."""
     header, lens, payload_off = read_header(path)
     if into is not None and (into.dtype_name != header["dtype"] or float(into.i8_scale) != float(header["i8_scale"])):
         raise ValueError(f"{path}: segment dtype/scale differs from the index it is appended to")
-    index = into if into is not None else MaxSimIndex(device=device, dtype=header["dtype"], i8_scale=header["i8_scale"])
+    index = into if into is not None else MaxSimIndex(device=device, dtype=header["dtype"], i8_scale=header["i8_scale"],
+                                                      tier=tier)
     total = header["n_rows_padded"] * header["row_bytes"]
     if int(nat.lib.b200ms_padded_rows(nat.i32_array(lens.tolist()), len(lens))) != header["n_rows_padded"]:
         raise ValueError(f"{path}: page lengths do not match the row count")
     if os.path.getsize(path) < payload_off + total:
         raise ValueError(f"{path}: truncated payload")
+    if index.tier == "host":
+        index.reserve_rows(index.n_rows_padded + header["n_rows_padded"])
+        dst = memoryview(index.host_tail(total))
+        with open(path, "rb") as f:
+            f.seek(payload_off)
+            for o in range(0, total, CHUNK_BYTES):
+                n = min(CHUNK_BYTES, total - o)
+                if f.readinto(dst[o:o + n]) != n:
+                    raise ValueError(f"{path}: short read")
+        index.commit_rows(lens.tolist())
+        return index
     buf = _aligned_bytes(total, index.device)
     stages = [torch.empty(min(CHUNK_BYTES, max(total, 1)), dtype=torch.uint8).pin_memory() for _ in range(2)]
     events = [torch.cuda.Event(), torch.cuda.Event()]

@@ -180,7 +180,15 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
     def __init__(self, uri: str = "b200://0", device: int = 0, mode: str = "bf16", storage: Any = None,
                  auto_initialize: bool = True, compact_dead_fraction: float = 0.3, index: Any = None,
                  fde_candidates: Optional[int] = None, coalesce_queries: bool = True, max_coalesced_tokens: int = 1024,
-                 max_coalesced_queries: int = 64, zero_pad_compat: int = 0):
+                 max_coalesced_queries: int = 64, zero_pad_compat: int = 0, corpus_tier: str = "hbm"):
+        # corpus_tier "host": patch rows in pinned host memory, bounded by host RAM instead of HBM; only the FDE candidates of
+        # a query cross PCIe (the reference's load_multivector_from_storage, fast_multivector_store.py:545-548), so it needs
+        # the two-stage search
+        if corpus_tier not in ("hbm", "host"):
+            raise ValueError(f"corpus_tier must be 'hbm' or 'host', got {corpus_tier!r}")
+        if corpus_tier == "host" and not fde_candidates:
+            raise ValueError("corpus_tier='host' needs fde_candidates: a host-resident corpus is only scored on candidate lists")
+        self.corpus_tier = corpus_tier
         self.uri = uri
         self.device = int(device)
         self.mode = mode
@@ -212,7 +220,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             if self.fde_candidates:
                 from .fde import TwoStageIndex
 
-                self._two_stage = TwoStageIndex(device=self.device, dtype=self.mode)
+                self._two_stage = TwoStageIndex(device=self.device, dtype=self.mode, tier=self.corpus_tier)
                 self._index = self._two_stage.index
             else:
                 self._index = MaxSimIndex(device=self.device, dtype=self.mode)
@@ -451,7 +459,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
         from . import shardfile
 
-        index = shardfile.load_index(os.path.join(directory, "corpus.b2ms"), device=device)
+        index = shardfile.load_index(os.path.join(directory, "corpus.b2ms"), device=device, tier=kw.get("corpus_tier", "hbm"))
         store = cls(device=device, mode=index.dtype_name, auto_initialize=False, index=index, **kw)
         with open(os.path.join(directory, "catalog.jsonl")) as f:
             for line in f:
@@ -475,7 +483,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
         journal = shardfile.StoreJournal(directory)
         store = cls(device=device, mode=mode, **kw)
-        for op in journal.read_ops():
+        ops = journal.read_ops()
+        if getattr(store._index, "tier", "hbm") == "host":  # size the host block once from the segment headers
+            segs = [shardfile.read_header(journal.segment_files(op["seq"])[0])[0] for op in ops if op["op"] == "segment"]
+            store._index.reserve_rows(sum(int(h["n_rows_padded"]) for h in segs))
+        for op in ops:
             if op["op"] == "segment":
                 seg, cat, fde = journal.segment_files(op["seq"])
                 first = store._index.n_pages
