@@ -250,6 +250,9 @@ int b200ms_sharded_search_host_end(b200ms_t* h, int64_t ticket, float* top_score
  * Turbopuffer ANN over its output (:526-532) with an exact encoder and an exhaustive cosine scan.
  * configure: reps repetitions x 2^ksim SimHash partitions x proj_dim AMS-sketch dims = fde_dim floats per item.
  *   simhash [reps,128,ksim] Gaussian, ams_index [reps,128] in [0,proj_dim), ams_sign [reps,128] = +-1 (HOST arrays).
+ *   Needs 1 <= reps <= 65535, 1 <= ksim <= 8, 1 <= proj_dim <= 64, proj_dim * 2^ksim <= 512 and a multiple of 8.  Every
+ *   argument is checked before anything is uploaded: a call that returns B200MS_EINVAL leaves the previous configuration
+ *   in force.
  * encode: items stored back to back at rows (device F32|BF16, [sum len,128]); is_document 0: SUM per partition (query),
  *   1: AVERAGE per partition, empty partition -> 0 (document); out device float32 [n_items, fde_dim].
  * finalize: fp32 FDEs -> bf16 rows of the FDE corpus + 1/||row||.

@@ -27,6 +27,9 @@ int set_error(b200ms_t* h, int code, const std::string& msg) {
 
 int check_cuda(b200ms_t* h, cudaError_t e, const char* what) {
   if (e == cudaSuccess) return B200MS_OK;
+  // a failed runtime call (e.g. cudaFuncSetAttribute) also leaves its error as the thread's last error: clear it, or the
+  // next launch check on this thread -- in any later call -- would report it as its own failure
+  cudaGetLastError();
   return set_error(h, B200MS_ECUDA, std::string(what) + ": " + cudaGetErrorName(e) + " (" + cudaGetErrorString(e) + ")");
 }
 
@@ -243,6 +246,7 @@ B200MS_API int b200ms_create(int device, b200ms_t** out) {
   b200ms_t* h = new b200ms_t();
   h->device = device;
   h->num_sms = prop.multiProcessorCount;
+  h->smem_optin = int(prop.sharedMemPerBlockOptin);
   if (const char* e = getenv("B200MS_B1_TENSOR")) h->b1_tensor = atoi(e);
   if (const char* e = getenv("B200MS_ZERO_COPY")) h->zero_copy = atoi(e);
   if (const char* e = getenv("B200MS_UNIT_ROWS")) { if (atoll(e) > 0) h->unit_rows = atoll(e); }

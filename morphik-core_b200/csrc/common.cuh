@@ -150,6 +150,7 @@ struct CorpusView {
 struct b200ms {
   int device = 0;
   int num_sms = 0;
+  int smem_optin = 0;  // largest dynamic shared memory one block may opt in to (cudaDevAttrMaxSharedMemoryPerBlockOptin)
   std::string err;
   bms::Corpus corpus;
   // device metadata of the attached corpus

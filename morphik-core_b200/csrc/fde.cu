@@ -179,15 +179,20 @@ fde_finalize_kernel(const float* __restrict__ fde, int64_t n, int fde_dim, __nv_
 }
 
 // ------------------------------------------------------------------------------------------------ SIMT scan (fallback)
-// One warp per page row, 16-byte loads, up to kFdeQ queries resident in shared memory.
+// One warp per page row, 16-byte loads, up to q_per_launch (<= kFdeQ) queries per launch.  kSmemQ: the queries are staged
+// in shared memory; otherwise (one query of fde_dim floats exceeds the block's shared memory) they are read through L2.
 constexpr int kFdeQ = 4;
+template <bool kSmemQ>
 __global__ void __launch_bounds__(256)
 fde_scan_kernel(const uint4* __restrict__ F, const float* __restrict__ inv_norm, int64_t n_pages, int fde_dim,
-                const float* __restrict__ q_fde, int n_q, int q_base, float* __restrict__ scores, int64_t ld) {
-  extern __shared__ float s_q[];  // [nq_here][fde_dim]
-  const int nq_here = min(kFdeQ, n_q - q_base);
-  for (int i = threadIdx.x; i < nq_here * fde_dim; i += blockDim.x) s_q[i] = q_fde[int64_t(q_base) * fde_dim + i];
-  __syncthreads();
+                const float* __restrict__ q_fde, int n_q, int q_base, int q_per_launch, float* __restrict__ scores, int64_t ld) {
+  extern __shared__ float s_q[];  // [nq_here][fde_dim] when kSmemQ
+  const int nq_here = min(q_per_launch, n_q - q_base);
+  const float* q_src = q_fde + int64_t(q_base) * fde_dim;
+  if (kSmemQ) {
+    for (int64_t i = threadIdx.x; i < int64_t(nq_here) * fde_dim; i += blockDim.x) s_q[i] = q_src[i];
+    __syncthreads();
+  }
   const int lane = threadIdx.x & 31;
   const int64_t warp_global = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int64_t warp_stride = (int64_t(gridDim.x) * blockDim.x) >> 5;
@@ -217,8 +222,16 @@ fde_scan_kernel(const uint4* __restrict__ F, const float* __restrict__ inv_norm,
 #pragma unroll
         for (int q = 0; q < kFdeQ; ++q) {
           if (q < nq_here) {
-            const float4* qq = reinterpret_cast<const float4*>(s_q + q * fde_dim + v * 8);
-            const float4 q0 = qq[0], q1 = qq[1];
+            float4 q0, q1;
+            if (kSmemQ) {
+              const float4* qq = reinterpret_cast<const float4*>(s_q + q * fde_dim + v * 8);
+              q0 = qq[0];
+              q1 = qq[1];
+            } else {  // q_fde carries no alignment promise beyond 4 bytes
+              const float* qq = q_src + int64_t(q) * fde_dim + v * 8;
+              q0 = make_float4(__ldg(qq + 0), __ldg(qq + 1), __ldg(qq + 2), __ldg(qq + 3));
+              q1 = make_float4(__ldg(qq + 4), __ldg(qq + 5), __ldg(qq + 6), __ldg(qq + 7));
+            }
             acc[q] = fmaf(f[0], q0.x, acc[q]); acc[q] = fmaf(f[1], q0.y, acc[q]);
             acc[q] = fmaf(f[2], q0.z, acc[q]); acc[q] = fmaf(f[3], q0.w, acc[q]);
             acc[q] = fmaf(f[4], q1.x, acc[q]); acc[q] = fmaf(f[5], q1.y, acc[q]);
@@ -394,18 +407,29 @@ int launch_fde_finalize(b200ms_t* h, const float* fde, int64_t n, void* out_rows
 
 static int launch_fde_scan_simt(b200ms_t* h, const void* F, const float* inv_norm, int64_t n_pages, const float* q_fde, int n_q,
                                 float* scores, int64_t ld, cudaStream_t s) {
-  const int nq_res = n_q < kFdeQ ? n_q : kFdeQ;  // queries resident per launch
-  const size_t smem = size_t(nq_res) * h->fde_dim * sizeof(float);
-  if (int e = ensure_smem(h, reinterpret_cast<const void*>(fde_scan_kernel), int(smem), "cudaFuncSetAttribute(fde_scan)"))
-    return e;
+  // queries resident in shared memory per launch: up to kFdeQ, as many as the block's opt-in limit holds (4 at the default
+  // 10240 dims).  When not even one fits, kFdeQ queries per launch are read through L2 instead.
+  const size_t q_bytes = size_t(h->fde_dim) * sizeof(float);
+  int nq_res = int(size_t(h->smem_optin) / q_bytes);
+  if (nq_res > kFdeQ) nq_res = kFdeQ;
+  if (nq_res > n_q) nq_res = n_q;
+  const int q_per_launch = nq_res > 0 ? nq_res : (n_q < kFdeQ ? n_q : kFdeQ);
+  const size_t smem = size_t(nq_res) * q_bytes;
+  const void* kern = nq_res > 0 ? reinterpret_cast<const void*>(fde_scan_kernel<true>)
+                                : reinterpret_cast<const void*>(fde_scan_kernel<false>);
+  if (int e = ensure_smem(h, kern, int(smem), "cudaFuncSetAttribute(fde_scan)")) return e;
   int per_sm = int((220 * 1024) / (smem + 1024));  // CTAs per SM by shared memory (40 KB per resident query)
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 8) per_sm = 8;
   int64_t blocks = (n_pages + 7) / 8;
   if (blocks > int64_t(h->num_sms) * per_sm) blocks = int64_t(h->num_sms) * per_sm;
-  for (int qb = 0; qb < n_q; qb += kFdeQ) {
-    fde_scan_kernel<<<int(blocks), 256, smem, s>>>(static_cast<const uint4*>(F), inv_norm, n_pages, h->fde_dim, q_fde, n_q, qb,
-                                                   scores, ld);
+  for (int qb = 0; qb < n_q; qb += q_per_launch) {
+    if (nq_res > 0)
+      fde_scan_kernel<true><<<int(blocks), 256, smem, s>>>(static_cast<const uint4*>(F), inv_norm, n_pages, h->fde_dim, q_fde,
+                                                           n_q, qb, q_per_launch, scores, ld);
+    else
+      fde_scan_kernel<false><<<int(blocks), 256, 0, s>>>(static_cast<const uint4*>(F), inv_norm, n_pages, h->fde_dim, q_fde,
+                                                         n_q, qb, q_per_launch, scores, ld);
     h->launches++;
     if (int e = check_cuda(h, cudaGetLastError(), "launch fde_scan")) return e;
   }
@@ -473,23 +497,22 @@ B200MS_API int b200ms_fde_configure_ex(b200ms_t* h, int reps, int ksim, int proj
                                        const int32_t* ams_index, const float* ams_sign, int fill_empty_partitions,
                                        int final_dim, const int32_t* final_index, const float* final_sign) {
   if (!h) return B200MS_EINVAL;
-  if (reps < 1 || ksim < 1 || ksim > 8 || proj_dim < 1 || proj_dim > 64 || (proj_dim << ksim) > 512 || ((proj_dim << ksim) % 8) ||
-      !simhash || !ams_index || !ams_sign)
-    return set_error(h, B200MS_EINVAL, "fde_configure: need 1<=ksim<=8, proj_dim<=64, proj_dim*2^ksim <= 512 and a multiple of 8");
+  // every argument is checked before the first upload: a refused call leaves the device matrices and h->fde_* as they were
+  if (reps < 1 || reps > 65535 || ksim < 1 || ksim > 8 || proj_dim < 1 || proj_dim > 64 || (proj_dim << ksim) > 512 ||
+      ((proj_dim << ksim) % 8) || !simhash || !ams_index || !ams_sign)
+    return set_error(h, B200MS_EINVAL,
+                     "fde_configure: need 1<=reps<=65535, 1<=ksim<=8, proj_dim<=64, proj_dim*2^ksim <= 512 and a multiple of 8");
   for (int i = 0; i < reps * kDim; ++i)
     if (ams_index[i] < 0 || ams_index[i] >= proj_dim) return set_error(h, B200MS_EINVAL, "fde_configure: ams_index out of range");
   const int inner = reps * (1 << ksim) * proj_dim;
   if (final_dim < 0 || (final_dim > 0 && (!final_index || !final_sign || final_dim % 8)))
     return set_error(h, B200MS_EINVAL, "fde_configure: final projection needs index/sign arrays and a dimension that is a multiple of 8");
-  DeviceGuard g(h->device);
-  cudaStream_t s = h->stream;
-  if (int e = upload(h, h->fde_simhash, simhash, size_t(reps) * kDim * ksim * 4, s)) return e;
-  if (int e = upload(h, h->fde_ams_index, ams_index, size_t(reps) * kDim * 4, s)) return e;
-  if (int e = upload(h, h->fde_ams_sign, ams_sign, size_t(reps) * kDim * 4, s)) return e;
+  // CSR of the final projection by output bucket, ascending input index inside a bucket (the order the oracle adds in)
+  std::vector<int32_t> csr;
+  std::vector<float> sg;
   if (final_dim > 0) {
-    // CSR by output bucket, ascending input index inside a bucket (the order the oracle adds in)
-    std::vector<int32_t> csr(size_t(final_dim) + 1 + size_t(inner), 0);
-    std::vector<float> sg(static_cast<size_t>(inner), 0.f);
+    csr.assign(size_t(final_dim) + 1 + size_t(inner), 0);
+    sg.assign(static_cast<size_t>(inner), 0.f);
     for (int i = 0; i < inner; ++i) {
       if (final_index[i] < 0 || final_index[i] >= final_dim) return set_error(h, B200MS_EINVAL, "fde_configure: final_index out of range");
       csr[size_t(final_index[i]) + 1]++;
@@ -502,6 +525,15 @@ B200MS_API int b200ms_fde_configure_ex(b200ms_t* h, int reps, int ksim, int proj
       csr[size_t(final_dim) + 1 + pos] = i;
       sg[pos] = final_sign[i];
     }
+  }
+  DeviceGuard g(h->device);
+  cudaStream_t s = h->stream;
+  // a failure from here on may leave the device matrices half replaced: the handle is unconfigured until a call succeeds
+  h->fde_dim = 0;
+  if (int e = upload(h, h->fde_simhash, simhash, size_t(reps) * kDim * ksim * 4, s)) return e;
+  if (int e = upload(h, h->fde_ams_index, ams_index, size_t(reps) * kDim * 4, s)) return e;
+  if (int e = upload(h, h->fde_ams_sign, ams_sign, size_t(reps) * kDim * 4, s)) return e;
+  if (final_dim > 0) {
     if (int e = upload(h, h->fde_final_index, csr.data(), csr.size() * 4, s)) return e;
     if (int e = upload(h, h->fde_final_sign, sg.data(), sg.size() * 4, s)) return e;
   }

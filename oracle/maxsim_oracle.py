@@ -352,17 +352,23 @@ def dequantize_e4m3_np(codes: np.ndarray) -> np.ndarray:
 
 
 def fde_encode_np(x: np.ndarray, simhash: np.ndarray, ams_index: np.ndarray, ams_sign: np.ndarray, scale: float,
-                  is_document: bool, proj: int) -> np.ndarray:
-    """Independent numpy restatement (float64 arithmetic) used to cross-check the C loops within rounding."""
+                  is_document: bool, proj: int, fill_empty: bool = False, final_index: Optional[np.ndarray] = None,
+                  final_sign: Optional[np.ndarray] = None, final_dim: int = 0) -> np.ndarray:
+    """Independent numpy restatement (float64 arithmetic) used to cross-check the C loops within rounding.
+
+    A row whose SimHash dot lies near zero may fall into another partition here than in the fp32 loops; callers draw rows
+    with a margin so that the partitions agree."""
     x = np.asarray(x, dtype=np.float64)
     reps, dim, ksim = simhash.shape
     n_part = 1 << ksim
     out = np.zeros((reps, n_part, proj))
     for r in range(reps):
-        bits = (np.asarray(x, dtype=np.float32) @ simhash[r].astype(np.float32)) > 0  # [n, ksim]
+        bits = (x @ simhash[r].astype(np.float64)) > 0  # [n, ksim]
         code = np.zeros(x.shape[0], dtype=np.int64)
+        sign_bits = np.zeros(x.shape[0], dtype=np.int64)  # first projection in the most significant bit
         for k in range(ksim):
             code = (code << 1) + (bits[:, k].astype(np.int64) ^ (code & 1))
+            sign_bits = (sign_bits << 1) | bits[:, k].astype(np.int64)
         A = np.zeros((dim, proj))
         A[np.arange(dim), ams_index[r]] = ams_sign[r]
         y = x @ A
@@ -370,4 +376,13 @@ def fde_encode_np(x: np.ndarray, simhash: np.ndarray, ams_index: np.ndarray, ams
             sel = code == p
             if sel.any():
                 out[r, p] = y[sel].sum(axis=0) * scale / (sel.sum() if is_document else 1.0)
-    return out.reshape(-1).astype(np.float32)
+            elif is_document and fill_empty and x.shape[0]:
+                # partition p holds the rows whose sign bits are p's Gray code; nearest by Hamming distance, first wins
+                dist = np.bitwise_count(sign_bits ^ (p ^ (p >> 1)))
+                out[r, p] = y[int(np.argmin(dist))] * scale
+    v = out.reshape(-1)
+    if final_dim > 0:
+        f = np.zeros(final_dim)
+        np.add.at(f, np.asarray(final_index, dtype=np.int64), np.asarray(final_sign, dtype=np.float64) * v)
+        v = f
+    return v.astype(np.float32)
