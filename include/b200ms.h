@@ -93,9 +93,18 @@ int b200ms_hamming_batch(b200ms_t* h, const uint8_t* q_bits, const uint8_t* cand
 
 /* Convert n_pages pages stored back to back at src (device, [sum len,128] F32|BF16) into the padded
  * corpus layout at dst (device): page i occupies padded_len(len_i) rows, the padding rows repeat the
- * page's last true row (max-/min-invariant, so scores are unchanged).  dst_dtype BF16: round-to-nearest-even;
- * I8: rint(x * i8_scale) clamped to [-127,127]; F8: e4m3(x * i8_scale), round-to-nearest-even, saturating (use a power-of-two
- * scale, 64 for unit-norm rows); B1: sign bits.  page_lens is a HOST array. */
+ * page's last true row byte for byte (max-/min-invariant, so scores are unchanged); a page of length 0 occupies no rows.
+ * Per element, for every float32 input (a BF16 source is widened exactly first):
+ *   BF16: round-to-nearest-even; subnormals are kept; finite values past the largest bf16 round to +-inf; +-inf stay;
+ *         every NaN -> 0x7fff (the canonical bf16 NaN, sign dropped).
+ *   I8:   rint(fp32 product x * i8_scale) (ties to even) clamped to [-127,127]; +-inf -> +-127; NaN -> 0 (it has no sign
+ *         and no magnitude).
+ *   F8:   e4m3 of the fp32 product x * i8_scale (so the product is rounded first, then rounded again to e4m3: use a
+ *         power-of-two scale, 64 for unit-norm rows, to make the first rounding exact), round-to-nearest-even, saturating:
+ *         |x * i8_scale| > 448 and +-inf -> +-448 (0x7e / 0xfe); -0 and negative values that round to 0 -> 0x80;
+ *         every NaN -> 0x7f (sign dropped).
+ *   B1:   bit = x > 0, so +-0 and every NaN -> 0, +inf -> 1.
+ * page_lens is a HOST array. */
 int b200ms_pack_pages(b200ms_t* h, const void* src, int src_dtype, const int32_t* page_lens, int64_t n_pages,
                       void* dst, int dst_dtype, float i8_scale, void* stream);
 
@@ -142,16 +151,21 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
 int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* q_lens, const int32_t* group_offsets,
                  int n_q, void* group_scores, int64_t ld, void* stream);
 
-/* Per query: score[p] = scale * sum_{g in [group_offsets[q], group_offsets[q+1])} group_scores[g, p]; keep the k
- * best pages whose bit is set in allow_mask (device, bit p&31 of word p>>5; NULL = all), ordered by score DESC
- * then page id ASC (the reference leaves ties unspecified).  Outputs are device arrays: top_scores/top_ids
+/* Per query: sum[p] = the group scores group_scores[g, p], g in [group_offsets[q], group_offsets[q+1]), added in order to
+ * +0 (float32, or int32 for score_dtype I32: the caller keeps the sums in range); keep the k best pages whose bit is set
+ * in allow_mask (device, bit p&31 of word p>>5; NULL = all; bits at p >= n_pages are ignored), ordered by sum DESC then
+ * page id ASC (the reference leaves ties unspecified).  The order is total: -0 ties with +0, every NaN ranks above every
+ * number (+inf included) and NaNs tie with each other -- as torch.topk and Postgres ORDER BY ... DESC order them.  I32
+ * sums are ranked exactly, also where float32 would merge them.  Columns p >= n_pages (ld > n_pages) are never read.
+ * Reported score = float32(sum) * scale in fp32 (a NaN as 0x7fffffff).  Outputs are device arrays: top_scores/top_ids
  * [n_q, k] (unused slots: -inf / -1), top_counts [n_q].  id_base is added to every page id (global ids of a shard). */
 int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
                 const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, int k, float scale, int64_t id_base,
                 float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream);
 
 /* Merge candidate lists (e.g. the all-gathered per-shard top-k): cand_scores/cand_ids device [n_q, m]
- * (entries with id < 0 are ignored) -> best k by (score DESC, id ASC).  m <= 2*B200MS_MAX_K. */
+ * (entries with id < 0 are ignored) -> best k by (score DESC, id ASC) in the total order of b200ms_topk (-0 == +0, NaN
+ * above every number, NaNs tied); a -0 is reported as +0 and a NaN as 0x7fffffff.  m <= 2*B200MS_MAX_K. */
 int b200ms_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand_ids, int n_q, int m, int k,
                       float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream);
 

@@ -28,9 +28,10 @@ __device__ __forceinline__ float4 load_row4(const void* src, int src_dtype, int6
   return v;
 }
 
+// NaN -> 0: it has neither sign nor magnitude (fmaxf(NaN, -127) alone would make it -127, the strongest negative value)
 __device__ __forceinline__ int quant_i8(float x, float scale) {
   const float r = rintf(x * scale);  // round-half-even, like numpy.rint in the oracle
-  return int(fminf(fmaxf(r, -127.f), 127.f));
+  return isnan(r) ? 0 : int(fminf(fmaxf(r, -127.f), 127.f));
 }
 
 __device__ __forceinline__ void store_row4(void* dst, int dst_dtype, int64_t row, int lane, float4 v, float i8_scale) {

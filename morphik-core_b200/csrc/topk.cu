@@ -24,6 +24,11 @@ __device__ __forceinline__ uint32_t key_of(float s) {
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ uint32_t key_of(int s) { return uint32_t(s) ^ 0x80000000u; }
+// key_of of a caller's float: -0 -> +0 and every NaN -> the canonical NaN 0x7fffffff (the device's fadd returns it), so
+// that -0 ties with +0 and every NaN ranks above +inf, tied with the other NaNs.  The sums page_key forms from T(0) are
+// canonical already; raw floats handed to the merge are not (a NaN with its sign bit set would key below -inf, and
+// 0xffffffff would get key 0, the key of an invalid entry).
+__device__ __forceinline__ uint32_t key_of_canonical(float s) { return key_of(s + 0.0f); }
 __device__ __forceinline__ float score_of_key(uint32_t k, float) {
   const uint32_t u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
   return __uint_as_float(u);
@@ -313,10 +318,10 @@ merge_topk_kernel(const float* __restrict__ cand_scores, const uint32_t* __restr
         const uint8_t* blk = gathered + int64_t(i / kx) * rank_stride;
         const int64_t e = int64_t(q) * kx + (i % kx);
         id = reinterpret_cast<const int64_t*>(blk)[e];
-        kraw = key_of(reinterpret_cast<const float*>(blk + scores_off)[e]);
+        kraw = key_of_canonical(reinterpret_cast<const float*>(blk + scores_off)[e]);
       } else {
         id = cand_ids[int64_t(q) * m + i];
-        kraw = cand_keys ? cand_keys[int64_t(q) * m + i] : key_of(cand_scores[int64_t(q) * m + i]);
+        kraw = cand_keys ? cand_keys[int64_t(q) * m + i] : key_of_canonical(cand_scores[int64_t(q) * m + i]);
       }
     }
     const bool ok = id >= 0;

@@ -154,29 +154,40 @@ def int8_maxsim_np(q: np.ndarray, rows: np.ndarray, off: np.ndarray, zero_pad_co
     return out
 
 
+def rank_desc_np(scores: np.ndarray, ids: np.ndarray) -> np.ndarray:
+    """Positions of `scores` in the build's order: score DESC, then id ASC.  Every NaN ranks above every number and NaNs
+    tie with each other (torch.topk, Postgres ORDER BY ... DESC); -0.0 ties with +0.0."""
+    with np.errstate(invalid="ignore"):
+        s = np.asarray(scores).astype(np.float64) + 0.0  # -0.0 + 0.0 = +0.0
+    nan = np.isnan(s)
+    return np.lexsort((np.asarray(ids), -np.where(nan, 0.0, s), ~nan))
+
+
 def topk_np(scores: np.ndarray, k: int, allow: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
-    """ORDER BY score DESC, page index ASC (the build's tie rule) LIMIT k; allow = bool mask per page."""
+    """ORDER BY score DESC, page index ASC (the build's tie rule, rank_desc_np) LIMIT k; allow = bool mask per page."""
     ids = np.arange(len(scores), dtype=np.int64)
     if allow is not None:
         ids = ids[np.asarray(allow, dtype=bool)]
     s = np.asarray(scores)[ids]
-    order = np.lexsort((ids, -s.astype(np.float64)))[:k]
+    order = rank_desc_np(s, ids)[:k]
     return s[order], ids[order]
 
 
 def quantize_int8_np(x: np.ndarray, scale: float) -> np.ndarray:
-    """The build's int8 rule (no reference, SURVEY F5): round-half-even(x * scale) clamped to [-127, 127]."""
-    return np.clip(np.rint(np.asarray(x, dtype=np.float32) * np.float32(scale)), -127, 127).astype(np.int8)
+    """The build's int8 rule (no reference, SURVEY F5): round-half-even of the float32 product x * scale, clamped to
+    [-127, 127] (so +-inf -> +-127); NaN -> 0 (it has neither sign nor magnitude)."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        r = np.rint(np.asarray(x, dtype=np.float32) * np.float32(scale))
+    return np.where(np.isnan(r), 0, np.clip(r, -127, 127)).astype(np.int8)
 
 
 def bf16_round_np(x: np.ndarray) -> np.ndarray:
-    """fp32 -> bf16 (round-to-nearest-even) -> fp32, bit-exact with torch/CUDA __float2bfloat16_rn."""
+    """fp32 -> bf16 (round-to-nearest-even; overflow -> +-inf; subnormals kept) -> fp32, bit-exact with the device's
+    cvt.rn.bf16x2.f32: every NaN becomes the canonical bf16 NaN 0x7fff (sign dropped; torch's own cast writes 0x7fc0)."""
     u = np.asarray(x, dtype=np.float32).view(np.uint32).astype(np.uint64)
     rounded = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
-    nan = np.isnan(np.asarray(x, dtype=np.float32))
-    out = rounded.astype(np.uint32).view(np.float32).copy()
-    out[nan] = np.nan
-    return out
+    nan = (u & 0x7FFFFFFF) > 0x7F800000
+    return np.where(nan, np.uint64(0x7FFF0000), rounded).astype(np.uint32).view(np.float32)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -334,15 +345,19 @@ _E4M3 = _e4m3_table()
 
 
 def quantize_e4m3_np(x: np.ndarray, scale: float = 64.0) -> np.ndarray:
-    """float -> e4m3 CODES (uint8) of x*scale, round-to-nearest-even (ties -> even code), |x*scale| > 448 saturates."""
-    y = np.asarray(x, dtype=np.float32).astype(np.float64) * float(scale)
-    a = np.minimum(np.abs(y), 448.0)
+    """float -> e4m3 CODES (uint8) of the float32 product x*scale (the library multiplies in fp32, then rounds once more):
+    round-to-nearest-even (ties -> even code), |x*scale| > 448 and +-inf saturate to +-448, NaN -> 0x7f (sign dropped)."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        y32 = np.asarray(x, dtype=np.float32) * np.float32(scale)
+    y = y32.astype(np.float64)
+    nan = np.isnan(y)
+    a = np.minimum(np.abs(np.where(nan, 0.0, y)), 448.0)
     hi = np.clip(np.searchsorted(_E4M3, a, side="left"), 0, len(_E4M3) - 1)
     lo = np.maximum(hi - 1, 0)
     d_lo, d_hi = a - _E4M3[lo], _E4M3[hi] - a
     pick_hi = (d_hi < d_lo) | ((d_hi == d_lo) & (hi % 2 == 0))
-    code = np.where(pick_hi, hi, lo).astype(np.uint8)
-    return code | (np.signbit(y).astype(np.uint8) << 7)
+    code = np.where(pick_hi, hi, lo).astype(np.uint8) | (np.signbit(y32).astype(np.uint8) << 7)
+    return np.where(nan, np.uint8(0x7F), code).astype(np.uint8)
 
 
 def dequantize_e4m3_np(codes: np.ndarray) -> np.ndarray:
