@@ -213,6 +213,32 @@ int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, co
                                const int64_t* cand_ids_dev, int n_cand, int k, float i8_q_scale, float score_scale,
                                float* top_scores_dev, int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream);
 
+/* ---- explaining a match (new; no reference counterpart) ---------------------------------------------------------------
+ * Per-token MaxSim breakdown of chosen pages: for query q, page slot j, token t
+ *   token_scores[q, j, t] = max over the TRUE rows r of page page_ids[q, j] of sim(q_t, d_r)
+ *   best_rows[q, j, t]    = the lowest r attaining that max  (0 <= r < page length)
+ *   sim_map[q, j, t, r]   = sim(q_t, d_r) for r < min(page length, map_rows)      (sim_map may be NULL)
+ * sim() is the search's own per-token value, in the units of the reported score:
+ *   BF16 / F8 fp32 dot (times score_scale), I8 int32 dot (times score_scale), B1 (128 - hamming) (times score_scale).
+ * The dense dtypes compute it on the scan's tensor-core instructions in the scan's order, so the map holds the very values the
+ * scan took its max over: sum_t token_scores[q, j, t] is the score b200ms_rerank_batch_device reports for that page (exactly
+ * for I8 / B1; for BF16 / F8 up to the order of the float32 sum over tokens), and token_scores == sim_map at best_rows.
+ * q_dev: F32 | BF16 rows [sum q_lens, 128]; q_lens HOST; page_ids_dev device int64 [n_q, n_cand] (-1 or outside
+ * [0, n_pages) = unused slot; a page may appear in several slots); t_max = max(q_lens).  Outputs are device arrays:
+ *   token_scores / best_rows [n_q, n_cand, t_max], sim_map [n_q, n_cand, t_max, map_rows].
+ * Every output entry is written.  For an unused slot, a page with no rows, or a token t >= q_lens[q]: score 0,
+ * best row -1, map entries -inf.  Map entries at r >= page length are -inf.
+ * Queries are packed exactly as b200ms_search_device packs them (same i8_q_scale, same sign rule).
+ * A max over rows is fmaxf's (a NaN only when every row is NaN); a tie, +0 and -0 included, reports the lowest row.
+ * Host-resident corpora: the named pages are gathered like a rerank's candidates (b200ms_last_gather_stats reports the call)
+ * and the outputs are bit-identical to an HBM corpus of the same rows.
+ * Option "zero_pad_compat" is ignored: maps are over true rows only.
+ * B200MS_EINVAL: NULL or inconsistent arguments, a negative query length, map_rows < 0, n_q * n_cand >= 2^30;
+ * B200MS_ESTATE: no corpus attached. */
+int b200ms_explain_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
+                          const int64_t* page_ids_dev, int n_cand, float i8_q_scale, float score_scale,
+                          float* token_scores, int32_t* best_rows, float* sim_map, int64_t map_rows, void* stream);
+
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the
  * path in B200MS_NCCL_LIB); b200ms_comm_available() says whether that worked.

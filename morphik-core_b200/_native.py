@@ -108,6 +108,7 @@ def _declare(lib: ctypes.CDLL) -> ctypes.CDLL:
         "b200ms_host_alloc": (c_int, [vp, c_int64, POINTER(c_void_p)]),
         "b200ms_host_free": (c_int, [vp, vp]),
         "b200ms_last_gather_stats": (c_int, [vp, i64p, i64p, POINTER(c_int), f32p]),
+        "b200ms_explain_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, c_float, vp, vp, vp, c_int64, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)
@@ -130,7 +131,7 @@ EXPORTED = [
     "b200ms_sharded_search_begin", "b200ms_sharded_search_end", "b200ms_sharded_search_host_begin",
     "b200ms_sharded_search_host_end", "b200ms_fde_configure_ex", "b200ms_fde_encode_corpus",
     "b200ms_send_device", "b200ms_recv_device", "b200ms_set_corpus_host", "b200ms_host_alloc", "b200ms_host_free",
-    "b200ms_last_gather_stats",
+    "b200ms_last_gather_stats", "b200ms_explain_device",
 ]
 
 

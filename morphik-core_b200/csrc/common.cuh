@@ -261,8 +261,15 @@ inline CorpusView corpus_view(const b200ms_t* h) {
   return v;
 }
 
-// Candidate scoring of a host-resident corpus (host_tier.cu): dedup the candidate pages of the call, gather them into the
-// staging block in rounds of at most host_stage_bytes, score every round through score_round.  Synchronises s once.
+// Pages of a host-resident corpus named by ids[0..n_slots) (host_tier.cu): dedup them, gather them into the staging block in
+// rounds of at most host_stage_bytes and call round_fn after each round's gather with the block as a corpus view and remap
+// (slot -> page of the view; -1 = invalid id or a page of another round).  Sets the gather stats; h->ht_rounds stays 0 when
+// no named page has a row.  Synchronises s once.
+int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStream_t s,
+                     int (*round_fn)(b200ms_t*, const CorpusView&, const int64_t* remap, int r, int rounds, void* ctx),
+                     void* ctx);
+// Candidate scoring of a host-resident corpus: gather_host_tier over the candidate slots, every round scored through
+// score_round.
 int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_t ld, void* group_scores, cudaStream_t s,
                     int (*score_round)(b200ms_t*, const CorpusView&, const int64_t* unit_ids, void* scores, bool fill,
                                        void* ctx),

@@ -164,8 +164,7 @@ ht_gather_kernel(const uint4* __restrict__ src, int piece_shift, const int64_t* 
   }
 }
 
-// 1-bit rounds: the POPC rerank kernel writes 0 for every slot outside its round, so each round scores into scratch and
-// only its own slots are copied over
+// 1-bit rounds of a rerank: merge one round's own slots (score_host_tier)
 __global__ void ht_merge_round_kernel(int32_t* __restrict__ dst, const int32_t* __restrict__ src, const int64_t* __restrict__ remap,
                                       int64_t n_slots, int64_t rows, int64_t ld) {
   for (int64_t idx = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; idx < rows * n_slots; idx += int64_t(gridDim.x) * blockDim.x) {
@@ -181,12 +180,10 @@ static int grid_of(const b200ms_t* h, int64_t n) {
   return b < 1 ? 1 : int(b);
 }
 
-int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_t ld, void* group_scores, cudaStream_t s,
-                    int (*score_round)(b200ms_t*, const CorpusView&, const int64_t* unit_ids, void* scores, bool fill,
-                                       void* ctx),
-                    void* ctx) {
+int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStream_t s,
+                     int (*round_fn)(b200ms_t*, const CorpusView&, const int64_t* remap, int r, int rounds, void* ctx),
+                     void* ctx) {
   const Corpus& c = h->corpus;
-  const int64_t n_slots = cs.n_slots(n_q);
   const int64_t rb = b200ms_row_bytes(c.dtype);
   const int64_t n_words = (c.n_pages + 31) / 32;
   h->ht_unique = h->ht_bytes = 0;
@@ -205,7 +202,7 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
   const int64_t* ps = static_cast<const int64_t*>(h->page_start.p);
   // 1-2: dedup + plan
   if (int e = check_cuda(h, cudaMemsetAsync(bitmap, 0, size_t(n_words > 0 ? n_words : 1) * 4, s), "host tier: memset")) return e;
-  ht_mark_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(cs.ids, n_slots, c.n_pages, bitmap);
+  ht_mark_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(ids, n_slots, c.n_pages, bitmap);
   ht_scan_words_kernel<<<1, kScanThreads, 0, s>>>(bitmap, n_words, wpre);
   ht_compact_kernel<<<grid_of(h, n_words), 256, 0, s>>>(bitmap, n_words, wpre, uniq);
   ht_scan_rows_kernel<<<1, kScanThreads, 0, s>>>(uniq, wpre + n_words, ps, stage_off, static_cast<int64_t*>(h->ht_hdr.p));
@@ -217,8 +214,7 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
   const int64_t n_uniq = hdr[0], rows = hdr[1];
   h->ht_unique = n_uniq;
   h->ht_bytes = rows * rb;
-  if (rows == 0)  // no valid candidate, or only empty pages: every score is 0, what the scorers leave for them
-    return check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(gp) * size_t(ld) * 4, s), "host tier: memset scores");
+  if (rows == 0) return B200MS_OK;  // no valid candidate, or only empty pages: nothing to gather
   // round geometry: capacity cap rows (the budget, at least the largest page), pages starting in each W-row window
   int64_t cap = (h->host_stage_bytes / rb) & ~int64_t(kGroup - 1);
   if (cap < c.max_page_rows) cap = c.max_page_rows;
@@ -238,11 +234,6 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
   }
   if (int e = reserve(h, h->ht_ps, size_t(n_uniq + 1) * 8)) return e;
   if (int e = reserve(h, h->ht_chunk_page, size_t(stage_rows / kGroup > 0 ? stage_rows / kGroup : 1) * 4)) return e;
-  const bool split_b1 = b1 && rounds > 1;
-  if (split_b1) {
-    if (int e = reserve(h, h->ht_scores, size_t(gp) * size_t(ld) * 4)) return e;
-    if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(gp) * size_t(ld) * 4, s), "host tier: memset scores")) return e;
-  }
   while (h->ht_ev.size() < size_t(2 * rounds)) {
     cudaEvent_t ev = nullptr;
     if (int e = check_cuda(h, cudaEventCreate(&ev), "host tier: cudaEventCreate")) return e;
@@ -260,7 +251,7 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
   for (int r = 0; r < rounds; ++r) {
     ht_round_plan_kernel<<<grid_of(h, n_uniq), 256, 0, s>>>(stage_off, n_uniq, W, r, static_cast<int64_t*>(h->ht_ps.p),
                                                           static_cast<int32_t*>(h->ht_chunk_page.p));
-    ht_remap_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(cs.ids, n_slots, c.n_pages, bitmap, wpre, stage_off, n_uniq, W, r, remap);
+    ht_remap_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(ids, n_slots, c.n_pages, bitmap, wpre, stage_off, n_uniq, W, r, remap);
     if (int e = check_cuda(h, cudaEventRecord(h->ht_ev[2 * r], s), "host tier: event record")) return e;
     ht_gather_kernel<<<h->num_sms * 8, 256, 0, s>>>(static_cast<const uint4*>(c.rows), piece_shift, ps, uniq, stage_off, n_uniq,
                                                    W, r, v.page_start, v.chunk_page, static_cast<uint4*>(stage));
@@ -268,17 +259,43 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
     h->launches += 3;
     if (int e = check_cuda(h, cudaGetLastError(), "launch host-tier gather")) return e;
     h->ht_rounds = r + 1;
-    if (split_b1) {
-      if (int e = score_round(h, v, remap, h->ht_scores.p, true, ctx)) return e;
-      ht_merge_round_kernel<<<grid_of(h, gp * n_slots), 256, 0, s>>>(static_cast<int32_t*>(group_scores),
-                                                                    static_cast<const int32_t*>(h->ht_scores.p), remap, n_slots,
-                                                                    gp, ld);
-      h->launches++;
-      if (int e = check_cuda(h, cudaGetLastError(), "launch host-tier merge")) return e;
-    } else if (int e = score_round(h, v, remap, group_scores, r == 0, ctx)) {
-      return e;
-    }
+    if (int e = round_fn(h, v, remap, r, rounds, ctx)) return e;
   }
+  return B200MS_OK;
+}
+
+int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_t ld, void* group_scores, cudaStream_t s,
+                    int (*score_round)(b200ms_t*, const CorpusView&, const int64_t* unit_ids, void* scores, bool fill,
+                                       void* ctx),
+                    void* ctx) {
+  const int64_t n_slots = cs.n_slots(n_q);
+  struct Ctx {
+    int64_t n_slots, gp, ld;
+    void* group_scores;
+    cudaStream_t s;
+    int (*score_round)(b200ms_t*, const CorpusView&, const int64_t*, void*, bool, void*);
+    void* ctx;
+  } x{n_slots, gp, ld, group_scores, s, score_round, ctx};
+  auto round = [](b200ms_t* hh, const CorpusView& v, const int64_t* remap, int r, int rounds, void* p) {
+    const Ctx& x = *static_cast<const Ctx*>(p);
+    if (v.dtype != B200MS_B1 || rounds == 1) return x.score_round(hh, v, remap, x.group_scores, r == 0, x.ctx);
+    // 1-bit rounds: the POPC rerank kernel writes 0 for every slot outside its round, so each round scores into scratch and
+    // only its own slots are copied over
+    if (r == 0) {
+      if (int e = reserve(hh, hh->ht_scores, size_t(x.gp) * size_t(x.ld) * 4)) return e;
+      if (int e = check_cuda(hh, cudaMemsetAsync(x.group_scores, 0, size_t(x.gp) * size_t(x.ld) * 4, x.s), "host tier: memset scores"))
+        return e;
+    }
+    if (int e = x.score_round(hh, v, remap, hh->ht_scores.p, true, x.ctx)) return e;
+    ht_merge_round_kernel<<<grid_of(hh, x.gp * x.n_slots), 256, 0, x.s>>>(static_cast<int32_t*>(x.group_scores),
+                                                                        static_cast<const int32_t*>(hh->ht_scores.p), remap,
+                                                                        x.n_slots, x.gp, x.ld);
+    hh->launches++;
+    return check_cuda(hh, cudaGetLastError(), "launch host-tier merge");
+  };
+  if (int e = gather_host_tier(h, cs.ids, n_slots, s, round, &x)) return e;
+  if (h->ht_rounds == 0)  // no valid candidate, or only empty pages: every score is 0, what the scorers leave for them
+    return check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(gp) * size_t(ld) * 4, s), "host tier: memset scores");
   return B200MS_OK;
 }
 

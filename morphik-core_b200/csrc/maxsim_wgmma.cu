@@ -126,18 +126,6 @@ __device__ __forceinline__ Acc group_sum(const Acc (&v)[4]) {
   return s;
 }
 
-// e4m3 x 8 (one 8-byte word) -> 8 f16 (exact)
-__device__ __forceinline__ uint4 e4m3x8_to_f16x8(uint32_t lo, uint32_t hi) {
-  uint4 o;
-  asm("{\n\t.reg .b16 a, b, c, d;\n\t"
-      "mov.b32 {a, b}, %4;\n\tmov.b32 {c, d}, %5;\n\t"
-      "cvt.rn.f16x2.e4m3x2 %0, a;\n\tcvt.rn.f16x2.e4m3x2 %1, b;\n\t"
-      "cvt.rn.f16x2.e4m3x2 %2, c;\n\tcvt.rn.f16x2.e4m3x2 %3, d;\n\t}"
-      : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-      : "r"(lo), "r"(hi));
-  return o;
-}
-
 // e4m3 query rows -> f16 rows (the A operand of the KIND 2 kernel)
 __global__ void __launch_bounds__(256)
 f8_query_widen_kernel(const uint2* __restrict__ q, int64_t n_words, uint4* __restrict__ out) {

@@ -32,6 +32,18 @@ __host__ __device__ constexpr int kind_of_dtype(int dtype) {
   return dtype == B200MS_BF16 ? 0 : dtype == B200MS_I8 ? 1 : dtype == B200MS_F8 ? 2 : -1;
 }
 
+// e4m3 x 8 (one 8-byte word) -> 8 f16 (exact)
+__device__ __forceinline__ uint4 e4m3x8_to_f16x8(uint32_t lo, uint32_t hi) {
+  uint4 o;
+  asm("{\n\t.reg .b16 a, b, c, d;\n\t"
+      "mov.b32 {a, b}, %4;\n\tmov.b32 {c, d}, %5;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, a;\n\tcvt.rn.f16x2.e4m3x2 %1, b;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %2, c;\n\tcvt.rn.f16x2.e4m3x2 %3, d;\n\t}"
+      : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+      : "r"(lo), "r"(hi));
+  return o;
+}
+
 __device__ __forceinline__ float acc_max(float a, float b) { return fmaxf(a, b); }
 __device__ __forceinline__ int acc_max(int a, int b) { return max(a, b); }
 __device__ __forceinline__ float acc_max3(float a, float b, float c) { return fmax3(a, b, c); }

@@ -388,6 +388,11 @@ class TwoStageIndex:
         ev[3].record()
         return ts, ti, tc, ev
 
+    def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
+        """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
+        the same exact scorer that ranked them."""
+        return self.index.explain(queries, page_ids, map_rows)
+
     def search(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
         """Two-stage search; returns host arrays (scores [n_q,k], page ids [n_q,k], counts [n_q]) and fills last_timing_ms
         with the reference's stage names (fast_multivector_store.py:523,534,550,574): encode_query / ns.query (here: FDE scan

@@ -687,6 +687,44 @@ class MaxSimIndex:
                 "b200ms_rerank_batch_device")
         return ts, ti, tc
 
+    # ------------------------------------------------------------------ explaining a match
+    def explain(self, queries: Sequence[ArrayLike], page_ids, map_rows: int = 0):
+        """Why pages matched: per query token, the best patch row of each named page and its similarity, computed with the
+        search's own arithmetic on the packed rows (b200ms_explain_device), so the token scores add up to the page's score.
+
+        queries: [T_i,128] float32/bfloat16 matrices (numpy or torch, either side).  page_ids: int64 [n_q, n_cand] (one list
+        per query) or [n_cand] (shared by every query); -1 or an id outside [0, n_pages) is an unused slot.
+        Returns device tensors (token_scores float32 [n_q, n_cand, T_max], best_rows int32 [n_q, n_cand, T_max],
+        sim_map float32 [n_q, n_cand, T_max, map_rows] or None when map_rows == 0), in the units of the reported scores.
+        best_rows index the page's rows in the order they were added; unused slots, empty pages and tokens past a query's
+        length hold 0 / -1 / -inf, as do map rows past a page's length.  Works on both tiers."""
+        self._attach()
+        lens = self._q_lens(queries)
+        n_q = len(lens)
+        ids = page_ids if isinstance(page_ids, torch.Tensor) else torch.from_numpy(np.asarray(page_ids, dtype=np.int64))
+        ids = ids.to(device=self.device, dtype=torch.int64)
+        if ids.ndim == 1:
+            ids = ids.unsqueeze(0).expand(n_q, -1)
+        if ids.ndim != 2 or ids.shape[0] != n_q:
+            raise ValueError(f"page_ids must be [n_cand] or [n_q={n_q}, n_cand], got {tuple(ids.shape)}")
+        ids = ids.contiguous()
+        n_cand, t_max, map_rows = int(ids.shape[1]), max(lens, default=0), int(map_rows)
+        if map_rows < 0:
+            raise ValueError("map_rows must be >= 0")
+        ts = torch.empty((n_q, n_cand, t_max), dtype=torch.float32, device=self.device)
+        br = torch.empty((n_q, n_cand, t_max), dtype=torch.int32, device=self.device)
+        sm = torch.empty((n_q, n_cand, t_max, map_rows), dtype=torch.float32, device=self.device) if map_rows else None
+        if n_q == 0 or n_cand == 0:
+            return ts, br, sm
+        src, src_dtype = self._stage_rows(list(queries))
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_explain_device(self.h.ptr, _vp(src), src_dtype, nat.i32_array(lens), n_q, _vp(ids), n_cand,
+                                              ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), _vp(ts),
+                                              _vp(br), _vp(sm), map_rows, self._stream()),
+                "b200ms_explain_device")
+        return ts, br, sm
+
     # ------------------------------------------------------------------ multi-GPU (document shards, NCCL inside libb200ms)
     @staticmethod
     def comm_unique_id() -> bytes:

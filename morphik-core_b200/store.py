@@ -406,6 +406,45 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                                      embedding=[], metadata=dict(rec.metadata), score=0.0))
         return out
 
+    async def explain_chunks(self, query_embedding, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
+                             with_map: bool = False) -> List[Dict[str, Any]]:
+        """Why chunks matched a query (extension): one record per visible chunk, under the rules of ``get_chunks_by_id``
+        (unknown or deleted chunks and chunks of another ``app_id`` are skipped, duplicates collapsed), holding
+        ``document_id``, ``chunk_number``, ``score`` (the sum of its token scores: the chunk's query_similar score),
+        ``token_scores`` float32 [T], ``best_patch`` int32 [T] (per query token, the row of the chunk's embedding -- in the order
+        the embedding model emitted it -- that answered it) and, with ``with_map``, ``sim_map`` float32 [T, n_rows].  Placing
+        rows on the page image (patch grid, special tokens) is the embedding processor's business."""
+        q = as_query_matrix(query_embedding)
+        if not chunk_identifiers:
+            return []
+        return await asyncio.to_thread(self._explain_locked, q, list(chunk_identifiers), app_id, bool(with_map))
+
+    def _explain_locked(self, q, chunk_identifiers, app_id, with_map):
+        with self._lock:
+            recs = []
+            for doc_id, chunk_num in dict.fromkeys((d, int(n)) for d, n in chunk_identifiers):
+                pid = self.catalog.lookup(doc_id, chunk_num)
+                if pid is None:
+                    continue
+                rec = self.catalog.records[pid]
+                if app_id is not None and rec.app_id is not None and rec.app_id != app_id:
+                    continue
+                recs.append((pid, rec))
+            if not recs:
+                return []
+            map_rows = max(rec.n_rows for _, rec in recs) if with_map else 0
+            ts, br, sm = self._index.explain([q], [pid for pid, _ in recs], map_rows)
+            ts, br = ts[0].cpu().numpy(), br[0].cpu().numpy()
+            sm = sm[0].cpu().numpy() if sm is not None else None
+        out = []
+        for j, (_, rec) in enumerate(recs):
+            r = {"document_id": rec.document_id, "chunk_number": rec.chunk_number, "score": float(ts[j].sum(dtype=np.float64)),
+                 "token_scores": ts[j], "best_patch": br[j]}
+            if with_map:
+                r["sim_map"] = sm[j][:, :rec.n_rows]
+            out.append(r)
+        return out
+
     async def delete_chunks_by_document_id(self, document_id: str, app_id: Optional[str] = None) -> bool:
         try:  # off the event loop: the lock may be held by a GPU pass, and a compaction copies device memory
             await asyncio.to_thread(self._delete_locked, document_id)
