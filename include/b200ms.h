@@ -63,6 +63,7 @@ extern "C" {
 #define B200MS_DIM 128        /* embedding dimension of ColPali / ColQwen patch vectors */
 #define B200MS_ROW_GROUP 32   /* pages and queries are padded to multiples of 32 rows   */
 #define B200MS_MAX_K 4096     /* largest k accepted by b200ms_topk / b200ms_merge_topk  */
+#define B200MS_MAX_PER_DOC 64 /* most pages per document the b200ms_*_docs calls return   */
 
 typedef struct b200ms b200ms_t;
 
@@ -238,6 +239,42 @@ int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, co
 int b200ms_explain_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
                           const int64_t* page_ids_dev, int n_cand, float i8_q_scale, float score_scale,
                           float* token_scores, int32_t* best_rows, float* sim_map, int64_t map_rows, void* stream);
+
+/* ---- grouping results by document (new; no reference counterpart) -------------------------------------------------------
+ * The top k DOCUMENTS instead of the top k pages, for callers that want documents: DocumentService.retrieve_docs
+ * (core/services/document_service.py:819-851) asks for k chunks and keeps the best chunk per document
+ * (_create_document_results, :1759-1763), so a long document whose pages all match fills every slot by itself.
+ * page_doc: device int32 [n_pages] (indexed by page id, candidate mode too), the document ordinal of every page; a page
+ * whose value is outside [0, n_docs) is never returned (the table is not validated: holes are safe).
+ * For query q let L be the flat ranking of the eligible pages in b200ms_topk's order (a page is eligible when its allow bit
+ * is set, if a mask is given, and its page_doc is in range).  The result is
+ *   - documents in the order of their first page in L, at most k of them;
+ *   - for each, its first per_doc pages in L (a document with fewer eligible pages returns fewer);
+ *   - every score bit for bit the score the flat call reports for that page; a document's score is its first page's.
+ * Candidate mode: L ranks q's valid slots (id in [0, n_pages)) by score DESC then slot ASC; a page that occupies several
+ * slots counts once, at its earliest slot.  With n_docs == n_pages, page_doc[p] == p and per_doc == 1 the result equals
+ * the flat call's.  Outputs are device arrays:
+ *   doc_page_scores float32 [n_q, k, per_doc] (unused: -inf), doc_page_ids int64 [n_q, k, per_doc] (page id + id_base;
+ *   unused: -1), doc_page_counts int32 [n_q, k] (unused documents: 0), doc_counts int32 [n_q].
+ * B200MS_EINVAL: NULL outputs or page_doc, k outside [1, 4096], per_doc outside [1, B200MS_MAX_PER_DOC], n_docs < 1 while
+ * pages exist, n_docs > n_pages, and the per-call bounds of the flat call;  B200MS_ESTATE: as the flat call (no corpus; a
+ * full scan of a host-resident corpus).  Nothing is launched when a call is refused. */
+/* over a score matrix, like b200ms_topk (group_offsets HOST, one allow mask or NULL) */
+int b200ms_topk_docs(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                     const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, const int32_t* page_doc, int64_t n_docs,
+                     int k, int per_doc, float scale, int64_t id_base, float* doc_page_scores, int64_t* doc_page_ids,
+                     int32_t* doc_page_counts, int32_t* doc_counts, void* stream);
+/* full scan, masks as b200ms_search_device_masked (n_masks = 0: unfiltered) */
+int b200ms_search_docs_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k, int per_doc,
+                              const int32_t* page_doc, int64_t n_docs, const uint32_t* allow_masks_dev, int n_masks,
+                              const int32_t* mask_index_dev, float i8_q_scale, float score_scale, int64_t id_base,
+                              float* doc_page_scores, int64_t* doc_page_ids, int32_t* doc_page_counts, int32_t* doc_counts,
+                              void* stream);
+/* per-query candidate lists, as b200ms_rerank_batch_device */
+int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
+                                    const int64_t* cand_ids_dev, int n_cand, int k, int per_doc, const int32_t* page_doc,
+                                    int64_t n_docs, float i8_q_scale, float score_scale, float* doc_page_scores,
+                                    int64_t* doc_page_ids, int32_t* doc_page_counts, int32_t* doc_counts, void* stream);
 
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the

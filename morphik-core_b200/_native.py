@@ -109,6 +109,12 @@ def _declare(lib: ctypes.CDLL) -> ctypes.CDLL:
         "b200ms_host_free": (c_int, [vp, vp]),
         "b200ms_last_gather_stats": (c_int, [vp, i64p, i64p, POINTER(c_int), f32p]),
         "b200ms_explain_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, c_float, vp, vp, vp, c_int64, vp]),
+        "b200ms_topk_docs": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, vp, c_int64, c_int, c_int, c_float, c_int64,
+                                     vp, vp, vp, vp, vp]),
+        "b200ms_search_docs_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, c_int, vp, c_int64, vp, c_int, vp, c_float, c_float,
+                                              c_int64, vp, vp, vp, vp, vp]),
+        "b200ms_rerank_docs_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, c_float,
+                                                    c_float, vp, vp, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)
@@ -131,8 +137,10 @@ EXPORTED = [
     "b200ms_sharded_search_begin", "b200ms_sharded_search_end", "b200ms_sharded_search_host_begin",
     "b200ms_sharded_search_host_end", "b200ms_fde_configure_ex", "b200ms_fde_encode_corpus",
     "b200ms_send_device", "b200ms_recv_device", "b200ms_set_corpus_host", "b200ms_host_alloc", "b200ms_host_free",
-    "b200ms_last_gather_stats", "b200ms_explain_device",
+    "b200ms_last_gather_stats", "b200ms_explain_device", "b200ms_topk_docs", "b200ms_search_docs_device",
+    "b200ms_rerank_docs_batch_device",
 ]
+MAX_PER_DOC = 64
 
 
 def i32_array(values):

@@ -88,6 +88,16 @@ class PageCatalog:
         pid = self._by_key.get((document_id, int(chunk_number)))
         return pid if pid is not None and self.alive[pid] else None
 
+    @property
+    def n_documents(self) -> int:
+        """Number of document ordinals handed out (page_documents() values lie in [0, n_documents))."""
+        return len(self._doc_index)
+
+    def page_documents(self) -> np.ndarray:
+        """int32 [n_pages]: the document ordinal of every page, -1 for a deleted page (the table the grouped search reads)."""
+        n = self._n
+        return np.where(self.alive[:n], self._page_doc[:n], -1).astype(np.int32)
+
     def pages_of(self, document_id: str) -> List[int]:
         return [p for p in self._by_doc.get(document_id, []) if self.alive[p]]
 

@@ -274,7 +274,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
     if (g2.exec) cudaGraphExecDestroy(g2.exec);
   DeviceBuf* bufs[] = {&h->chunk_page, &h->unit_start, &h->page_start, &h->page_len, &h->clamp_pages, &h->clamp_slots,
                        &h->meta, &h->meta_b, &h->q_raw, &h->q_packed, &h->scores, &h->mask, &h->mask_index, &h->out_all,
-                       &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->b1_q_i8, &h->b1_tok_const, &h->f8_q_f16,
+                       &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->docs_best, &h->docs_mask, &h->docs_top, &h->docs_pick, &h->b1_q_i8, &h->b1_tok_const, &h->f8_q_f16,
                        &h->fde_simhash, &h->fde_ams_index, &h->fde_ams_sign, &h->fde_tmp, &h->fde_q_bf16, &h->fde_final_index,
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage};
@@ -770,6 +770,12 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   const int n_q = r.n_q;
   if (n_q < 1 || !r.q_lens || !r.q || r.k < 1 || r.k > B200MS_MAX_K || !r.top_scores || !r.top_ids || !r.top_counts)
     return set_error(h, B200MS_EINVAL, "search: bad arguments (n_q >= 1, 1 <= k <= 4096)");
+  if (r.docs) {
+    const DocSpec& d = *r.docs;
+    if (!d.page_doc || !d.page_counts || d.per_doc < 1 || d.per_doc > B200MS_MAX_PER_DOC || d.n_docs < 0 ||
+        (c.n_pages > 0 && d.n_docs < 1) || d.n_docs > c.n_pages || (r.cand.ids && !r.cand.per_query))
+      return set_error(h, B200MS_EINVAL, "search_docs: bad arguments (page_doc and outputs, 1 <= per_doc <= 64, 1 <= n_docs <= n_pages)");
+  }
   CandSpec cs = r.cand;
   if (cs.per_query && cs.stride() != cs.n_cand) {  // caller's lists are [n_q, n_cand]: give every list a 32-slot-aligned stride
     if (int e = reserve(h, h->cand_pad, size_t(cs.stride()) * size_t(n_q) * 8)) return e;
@@ -819,6 +825,11 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
     if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "search: memset")) return e;
   }
   const int sdt = (c.dtype == B200MS_BF16 || c.dtype == B200MS_F8) ? B200MS_F32 : B200MS_I32;
+  if (r.docs)
+    return cs.ids ? launch_topk_docs(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, nullptr, nullptr, cs.ids, cs.stride(),
+                                     c.n_pages, *r.docs, r.k, r.score_scale, 0, s)
+                  : launch_topk_docs(h, h->scores.p, sdt, c.n_pages, ld, goff_dev, n_q, r.allow, r.mask_index, nullptr, 0,
+                                     c.n_pages, *r.docs, r.k, r.score_scale, r.id_base, s);
   if (!cs.ids) {
     return launch_topk(h, h->scores.p, sdt, c.n_pages, ld, goff_dev, n_q, r.allow, r.k, r.score_scale, r.id_base, nullptr,
                        r.top_scores, r.top_ids, r.top_counts, s, r.mask_index, (c.n_pages + 31) / 32);
@@ -885,6 +896,68 @@ B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int s
     r.allow = allow_masks_dev;
     r.mask_index = mask_index_dev;
   }
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+}
+
+// ---- grouping results by document
+static bool docs_dims_ok(int k, int per_doc, int64_t n_docs, int64_t n_pages) {
+  return k >= 1 && k <= B200MS_MAX_K && per_doc >= 1 && per_doc <= B200MS_MAX_PER_DOC && n_docs >= 0 &&
+         (n_pages == 0 || n_docs >= 1) && n_docs <= n_pages;
+}
+
+B200MS_API int b200ms_topk_docs(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                                const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, const int32_t* page_doc,
+                                int64_t n_docs, int k, int per_doc, float scale, int64_t id_base, float* doc_page_scores,
+                                int64_t* doc_page_ids, int32_t* doc_page_counts, int32_t* doc_counts, void* stream) {
+  if (!h) return B200MS_EINVAL;
+  if ((score_dtype != B200MS_F32 && score_dtype != B200MS_I32) || n_pages < 0 || ld < n_pages || n_q < 0 ||
+      !docs_dims_ok(k, per_doc, n_docs, n_pages) || !page_doc || !doc_page_scores || !doc_page_ids || !doc_page_counts ||
+      !doc_counts || (n_q > 0 && !group_offsets) || (n_q > 0 && n_pages > 0 && !group_scores))
+    return set_error(h, B200MS_EINVAL, "topk_docs: bad arguments (1 <= k <= 4096, 1 <= per_doc <= 64, 1 <= n_docs <= n_pages)");
+  if (n_q == 0) return B200MS_OK;
+  DeviceGuard g(h->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (int e = upload(h, h->meta, group_offsets, size_t(n_q + 1) * 4, s)) return e;
+  const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
+  return launch_topk_docs(h, group_scores, score_dtype, n_pages, ld, static_cast<const int32_t*>(h->meta.p), n_q, allow_mask,
+                          nullptr, nullptr, 0, n_pages, d, k, scale, id_base, s);
+}
+
+B200MS_API int b200ms_search_docs_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
+                                         int per_doc, const int32_t* page_doc, int64_t n_docs, const uint32_t* allow_masks_dev,
+                                         int n_masks, const int32_t* mask_index_dev, float i8_q_scale, float score_scale,
+                                         int64_t id_base, float* doc_page_scores, int64_t* doc_page_ids,
+                                         int32_t* doc_page_counts, int32_t* doc_counts, void* stream) {
+  if (!h) return B200MS_EINVAL;
+  if (!src_dtype_ok(src_dtype)) return set_error(h, B200MS_EINVAL, "search_docs_device: src dtype must be F32 or BF16");
+  if (n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
+    return set_error(h, B200MS_EINVAL, "search_docs_device: n_masks > 0 needs the mask matrix and one index per query");
+  DeviceGuard g(h->device);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, doc_page_scores, doc_page_ids, doc_counts, id_base};
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
+  const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
+  r.docs = &d;
+  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+}
+
+B200MS_API int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
+                                               const int64_t* cand_ids_dev, int n_cand, int k, int per_doc,
+                                               const int32_t* page_doc, int64_t n_docs, float i8_q_scale, float score_scale,
+                                               float* doc_page_scores, int64_t* doc_page_ids, int32_t* doc_page_counts,
+                                               int32_t* doc_counts, void* stream) {
+  if (!h) return B200MS_EINVAL;
+  const CandSpec cand{cand_ids_dev, n_cand, 1};
+  if (!src_dtype_ok(src_dtype) || !cand_ids_dev || n_cand < 1 || n_q < 1 || cand.n_slots(n_q) >= (int64_t(1) << 30))
+    return set_error(h, B200MS_EINVAL,
+                     "rerank_docs_batch_device: bad arguments (F32/BF16 queries, n_cand >= 1, n_q*n_cand < 2^30)");
+  DeviceGuard g(h->device);
+  SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, doc_page_scores, doc_page_ids, doc_counts};
+  r.cand = cand;
+  const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
+  r.docs = &d;
   return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
 }
 

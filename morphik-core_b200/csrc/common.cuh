@@ -66,6 +66,19 @@ SearchMeta build_search_meta(const int32_t* lens, int64_t n, bool with_groups = 
 // n_groups are skipped
 void group_tokens(const int32_t* lens, int64_t n, const int32_t* goff, int64_t n_groups, int32_t* ntok);
 
+// Grouping a search's results by document (topk_docs.cu): page_doc int32 [n_pages] (device) maps a page to its document
+// ordinal; pages with a value outside [0, n_docs) are never returned.  Outputs (device): scores / ids [n_q, k, per_doc],
+// page_counts [n_q, k], doc_counts [n_q].
+struct DocSpec {
+  const int32_t* page_doc = nullptr;
+  int64_t n_docs = 0;
+  int per_doc = 1;
+  float* scores = nullptr;
+  int64_t* ids = nullptr;
+  int32_t* page_counts = nullptr;
+  int32_t* doc_counts = nullptr;
+};
+
 // One search: pack queries -> score -> top-k.  Device pointers, except that q and the outputs may be mapped pinned memory.
 struct SearchRequest {
   const void* q = nullptr;  // rows [sum q_lens,128] of q_dtype (F32 | BF16)
@@ -82,6 +95,7 @@ struct SearchRequest {
   const uint32_t* allow = nullptr;       // allow-mask bits over the pages (NULL = all); with mask_index: [n_masks, words]
   const int32_t* mask_index = nullptr;   // per query: row of `allow` (-1 = no mask); NULL = the one mask for every query
   CandSpec cand;                         // ids == NULL: full scan
+  const DocSpec* docs = nullptr;         // != NULL: the top k documents (per-query candidate lists only) instead of pages
 };
 
 // Results of a search as one block: [n_q*k int64 ids | n_q*k f32 scores | n_q int32 counts], padded to 16 bytes, so that
@@ -166,6 +180,8 @@ struct b200ms {
   bms::DeviceBuf q_raw, q_packed, scores, mask, mask_index, out_all;
   bms::PinnedBuf stage;         // host entry points: [metadata | query rows | results], mapped into the device address space
   bms::DeviceBuf topk_keys, topk_ids;  // first-level (per-slice) top-k candidates
+  bms::DeviceBuf docs_best, docs_mask, docs_top, docs_pick;  // grouping by document: per-(query, document) best key / rank,
+                                                             // best-page mask, document order, picked pages' keys
   bms::DeviceBuf b1_q_i8, b1_tok_const;  // tensor-core 1-bit scorer: +-1 int8 query tiles and per-token constants
   bms::DeviceBuf f8_q_f16;  // e4m3 corpora: the query rows widened to f16 (A operand of the f16 MMA)
   bms::DeviceBuf cand_pad;  // batched rerank: per-query candidate lists re-laid out with a 32-slot-aligned stride
@@ -297,6 +313,13 @@ int launch_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t 
                 const int32_t* group_offsets_dev, int n_q, const uint32_t* allow_mask, int k, float scale,
                 int64_t id_base, const int64_t* id_map, float* top_scores, int64_t* top_ids, int32_t* top_counts,
                 cudaStream_t s, const int32_t* mask_index = nullptr, int64_t mask_stride = 0, int64_t q_stride = 0);
+// the top k documents (DocSpec) over a group-score matrix, in the total order of launch_topk.  Full scan (cand == NULL):
+// items are pages [0, n_items), filtered as launch_topk filters them (allow, mask_index); candidate mode: per-query lists
+// cand [n_q, q_stride] of n_items slots (q_stride a multiple of 32), page ids valid in [0, n_pages).
+int launch_topk_docs(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_items, int64_t ld,
+                     const int32_t* group_offsets_dev, int n_q, const uint32_t* allow, const int32_t* mask_index,
+                     const int64_t* cand, int64_t q_stride, int64_t n_pages, const DocSpec& d, int k, float scale,
+                     int64_t id_base, cudaStream_t s);
 // merge straight from the all-gathered exchange layout: gathered = world blocks of [n_q*k int64 ids | n_q*k f32 scores]
 int launch_merge_gathered(b200ms_t* h, const void* gathered, int world, int n_q, int k, float* top_scores, int64_t* top_ids,
                           int32_t* top_counts, cudaStream_t s);

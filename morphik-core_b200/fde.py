@@ -388,6 +388,29 @@ class TwoStageIndex:
         ev[3].record()
         return ts, ti, tc, ev
 
+    def search_docs_device(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                           n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None):
+        """Two-stage search grouped by document: max(n_candidates, k * per_doc) FDE candidates per query (at most MAX_K),
+        then MaxSimIndex.rerank_docs_batch over them.  Returns its four device tensors."""
+        kc = int(min(max(n_candidates, k * per_doc), nat.MAX_K, max(self._n, 1)))
+        ci, _, _ = self.candidates(queries, kc, allow_mask_dev)
+        src, _ = self.index._stage_rows(list(queries))
+        return self.index.rerank_docs_batch(src, [int(q.shape[0]) for q in queries], ci, k, per_doc, page_doc_dev, n_docs)
+
+    def search_docs(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                    n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
+        """search_docs_device with a host allow mask (uint32 words, restricting both stages); synchronous, returns host
+        arrays (scores [n_q,k,per_doc], page ids [n_q,k,per_doc], pages per document [n_q,k], documents [n_q])."""
+        mask_dev = None if allow_mask is None else torch.from_numpy(
+            self.index._check_mask(allow_mask).view(np.int32)).to(self.device)
+        ts, ti, pc, dc = self.search_docs_device(queries, k, per_doc, page_doc_dev, n_docs, n_candidates, mask_dev)
+        n_q, kk = len(queries), ts.shape[1]
+        out_s = np.full((n_q, k, per_doc), -np.inf, dtype=np.float32)
+        out_i = np.full((n_q, k, per_doc), -1, dtype=np.int64)
+        out_pc = np.zeros((n_q, k), dtype=np.int32)
+        out_s[:, :kk], out_i[:, :kk], out_pc[:, :kk] = ts.cpu().numpy(), ti.cpu().numpy(), pc.cpu().numpy()
+        return out_s, out_i, out_pc, dc.cpu().numpy()
+
     def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
         """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
         the same exact scorer that ranked them."""

@@ -687,6 +687,92 @@ class MaxSimIndex:
                 "b200ms_rerank_batch_device")
         return ts, ti, tc
 
+    # ------------------------------------------------------------------ grouping results by document
+    def _check_docs_args(self, q_dev: torch.Tensor, per_doc: int, page_doc_dev: torch.Tensor):
+        if q_dev.dtype not in (torch.float32, torch.bfloat16) or not q_dev.is_contiguous():
+            raise ValueError("q_dev must be a contiguous float32/bfloat16 tensor")
+        if not 1 <= int(per_doc) <= nat.MAX_PER_DOC:
+            raise ValueError(f"per_doc must be in [1, {nat.MAX_PER_DOC}]")
+        if (page_doc_dev.dtype != torch.int32 or page_doc_dev.shape != (self.n_pages,) or not page_doc_dev.is_contiguous()
+                or page_doc_dev.device != self.device):
+            raise ValueError(f"page_doc_dev must be a contiguous int32 [{self.n_pages}] tensor on {self.device}")
+
+    def _docs_outputs(self, n_q: int, k: int, per_doc: int):
+        return (torch.empty((n_q, k, per_doc), dtype=torch.float32, device=self.device),
+                torch.empty((n_q, k, per_doc), dtype=torch.int64, device=self.device),
+                torch.empty((n_q, k), dtype=torch.int32, device=self.device),
+                torch.empty((n_q,), dtype=torch.int32, device=self.device))
+
+    def search_docs_device(self, q_dev: torch.Tensor, q_lens: Sequence[int], k: int, per_doc: int, page_doc_dev: torch.Tensor,
+                           n_docs: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                           mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0):
+        """The top k DOCUMENTS instead of the top k pages (b200ms_search_docs_device), asynchronous on torch's current stream.
+
+        page_doc_dev: int32 [n_pages] document ordinal of every page (a value outside [0, n_docs) hides the page).  Documents
+        come in the order of their best page in search_device's ranking, each with its best ``per_doc`` pages in that
+        ranking and their search_device scores.  Masks as search_device.  Returns device tensors (scores float32
+        [n_q,k,per_doc], page ids + id_base int64 [n_q,k,per_doc], pages per document int32 [n_q,k], documents int32 [n_q]);
+        unused entries are -inf / -1 / 0."""
+        self._attach()
+        n_q = len(q_lens)
+        self._check_docs_args(q_dev, per_doc, page_doc_dev)
+        words = (self.n_pages + 31) // 32
+        n_masks = 0
+        if mask_index_dev is not None:
+            if (allow_mask_dev is None or allow_mask_dev.ndim != 2 or allow_mask_dev.shape[1] != words
+                    or not allow_mask_dev.is_contiguous()):
+                raise ValueError("per-query masks: allow_mask_dev must be a contiguous [n_masks, ceil(n_pages/32)] word matrix")
+            if mask_index_dev.dtype != torch.int32 or mask_index_dev.numel() != n_q:
+                raise ValueError("mask_index_dev must be int32 [n_q]")
+            n_masks = int(allow_mask_dev.shape[0])
+        elif allow_mask_dev is not None:  # one mask for every query: a one-row matrix
+            if allow_mask_dev.shape != (words,) or not allow_mask_dev.is_contiguous():
+                raise ValueError(f"allow_mask_dev must have {words} words for {self.n_pages} pages")
+            mask_index_dev = torch.zeros((n_q,), dtype=torch.int32, device=self.device)
+            n_masks = 1
+        ts, ti, pc, dc = self._docs_outputs(n_q, int(k), int(per_doc))
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_search_docs_device(
+                    self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens), n_q,
+                    int(k), int(per_doc), _vp(page_doc_dev), int(n_docs), _vp(allow_mask_dev) if n_masks else None, n_masks,
+                    _vp(mask_index_dev) if n_masks else None, ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale),
+                    int(id_base), _vp(ts), _vp(ti), _vp(pc), _vp(dc), self._stream()),
+                "b200ms_search_docs_device")
+        return ts, ti, pc, dc
+
+    def search_docs(self, queries: Sequence[ArrayLike], k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                    allow_mask: Optional[np.ndarray] = None):
+        """search_docs_device from host query matrices and an optional host allow mask (uint32 words); synchronous, returns
+        host arrays."""
+        lens = self._q_lens(queries)
+        src, _ = self._stage_rows(list(queries))
+        mask_dev = None if allow_mask is None else torch.from_numpy(self._check_mask(allow_mask).view(np.int32)).to(self.device)
+        out = self.search_docs_device(src, lens, k, per_doc, page_doc_dev, n_docs, allow_mask_dev=mask_dev)
+        return tuple(t.cpu().numpy() for t in out)
+
+    def rerank_docs_batch(self, q_dev: torch.Tensor, q_lens: Sequence[int], cand_ids: torch.Tensor, k: int, per_doc: int,
+                          page_doc_dev: torch.Tensor, n_docs: int):
+        """rerank_batch grouped by document (b200ms_rerank_docs_batch_device): each query's own candidate list cand_ids int64
+        [n_q, n_cand] (-1 = unused slot) is ranked as rerank_batch ranks it, and a page listed in several slots counts once,
+        at its earliest slot.  k is capped at n_cand.  Outputs as search_docs_device."""
+        self._attach()
+        n_q = len(q_lens)
+        if cand_ids.dtype != torch.int64 or cand_ids.ndim != 2 or cand_ids.shape[0] != n_q or not cand_ids.is_contiguous():
+            raise ValueError("cand_ids must be a contiguous int64 [n_q, n_cand] device tensor")
+        self._check_docs_args(q_dev, per_doc, page_doc_dev)
+        n_cand = int(cand_ids.shape[1])
+        kk = int(min(k, n_cand))
+        ts, ti, pc, dc = self._docs_outputs(n_q, kk, int(per_doc))
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_rerank_docs_batch_device(
+                    self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens), n_q,
+                    _vp(cand_ids), n_cand, kk, int(per_doc), _vp(page_doc_dev), int(n_docs), ctypes.c_float(self.i8_scale),
+                    ctypes.c_float(self.score_scale), _vp(ts), _vp(ti), _vp(pc), _vp(dc), self._stream()),
+                "b200ms_rerank_docs_batch_device")
+        return ts, ti, pc, dc
+
     # ------------------------------------------------------------------ explaining a match
     def explain(self, queries: Sequence[ArrayLike], page_ids, map_rows: int = 0):
         """Why pages matched: per query token, the best patch row of each named page and its similarity, computed with the

@@ -209,6 +209,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         self._journal = None  # shardfile.StoreJournal when the store is durable (B200MultiVectorStore.open)
         self._last_store_metrics: Dict[str, Any] = {}
         self.last_query_timing: Dict[str, float] = {}
+        self._page_doc_cache: Optional[Tuple[int, Any]] = None  # (catalog.version, device page -> document table)
         if auto_initialize:
             self.initialize()
 
@@ -389,6 +390,52 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         if self._two_stage is not None:
             return self._two_stage.search(queries, k, n_candidates=max(int(self.fde_candidates), k), allow_mask=words)
         return self._index.search_host(queries, k, allow_mask=words)
+
+    async def query_similar_documents(self, query_embedding, k: int, pages_per_document: int = 1,
+                                      doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None,
+                                      min_score: Optional[float] = None) -> List[List[DocumentChunk]]:
+        """The top k DOCUMENTS instead of the top k chunks (extension): one list per document, best document first, each
+        holding that document's best ``pages_per_document`` chunks in score order.  A document ranks by its best chunk and
+        scores are query_similar's, so this is query_similar's ranking grouped by document, computed on the GPU without
+        over-fetching chunks.  ``doc_ids`` / ``app_id`` filter as in query_similar; ``min_score`` drops chunks below it and
+        a document left without chunks.  Mask, GPU search and chunk construction are one critical section."""
+        q = as_query_matrix(query_embedding)
+        per = int(pages_per_document)
+        if not 1 <= per <= 64:
+            raise ValueError("pages_per_document must be in [1, 64]")
+        if k <= 0:
+            return []
+        return await asyncio.to_thread(self._search_docs_locked, q, int(k), per, doc_ids, app_id, min_score)
+
+    def _search_docs_locked(self, q, k, per, doc_ids, app_id, min_score):
+        import torch
+
+        with self._lock:
+            n = len(self.catalog)
+            if n == 0:
+                return []
+            visible, words = self.catalog.allow_words(doc_ids, app_id)
+            if not visible:
+                return []
+            if k > 4096:
+                logger.warning("k=%d requested; truncated to 4096 (B200MS_MAX_K)", k)
+            n_docs = self.catalog.n_documents
+            kk = min(k, n_docs, 4096)
+            if self._page_doc_cache is None or self._page_doc_cache[0] != self.catalog.version:
+                table = torch.from_numpy(self.catalog.page_documents()).to(self._index.device)
+                self._page_doc_cache = (self.catalog.version, table)
+            page_doc = self._page_doc_cache[1]
+            if self._two_stage is not None:
+                ts, ti, pc, dc = self._two_stage.search_docs([q], kk, per, page_doc, n_docs,
+                                                             n_candidates=max(int(self.fde_candidates), kk * per), allow_mask=words)
+            else:
+                ts, ti, pc, dc = self._index.search_docs([q], kk, per, page_doc, n_docs, allow_mask=words)
+            out = []
+            for i in range(int(dc[0])):
+                chunks = self._chunks(ts[0, i], ti[0, i], int(pc[0, i]), min_score)
+                if chunks:
+                    out.append(chunks)
+            return out
 
     async def get_chunks_by_id(self, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
                                skip_image_content: bool = False) -> List[DocumentChunk]:
