@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
+from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libb200ms.so")
@@ -45,78 +45,81 @@ def _load() -> ctypes.CDLL:
     return _declare(ctypes.CDLL(LIB_PATH))
 
 
+# (restype, argtypes) of every function include/b200ms.h declares
+vp, i32p, i64p, f32p = c_void_p, POINTER(c_int32), POINTER(c_int64), POINTER(c_float)
+_SIGNATURES = {
+    "b200ms_version": (c_int, []),
+    "b200ms_device_count": (c_int, []),
+    "b200ms_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "b200ms_destroy": (c_int, [vp]),
+    "b200ms_last_error": (c_char_p, [vp]),
+    "b200ms_padded_len": (c_int64, [c_int64]),
+    "b200ms_padded_rows": (c_int64, [i32p, c_int64]),
+    "b200ms_row_bytes": (c_int64, [c_int]),
+    "b200ms_query_groups": (c_int64, [i32p, c_int]),
+    "b200ms_sign_pack": (c_int, [vp, vp, c_int, c_int64, vp, vp]),
+    "b200ms_hamming_batch": (c_int, [vp, vp, vp, c_int64, vp, vp]),
+    "b200ms_pack_pages": (c_int, [vp, vp, c_int, i32p, c_int64, vp, c_int, c_float, vp]),
+    "b200ms_set_corpus": (c_int, [vp, vp, c_int, i32p, c_int64]),
+    "b200ms_corpus_pages": (c_int64, [vp]),
+    "b200ms_corpus_rows": (c_int64, [vp]),
+    "b200ms_pack_queries": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, i32p, POINTER(c_int), vp]),
+    "b200ms_score": (c_int, [vp, vp, c_int, i32p, i32p, c_int, vp, c_int64, vp]),
+    "b200ms_topk": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, c_int, c_float, c_int64, vp, vp, vp, vp]),
+    "b200ms_merge_topk": (c_int, [vp, vp, vp, c_int, c_int, c_int, vp, vp, vp, vp]),
+    "b200ms_search_host": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_float, c_float, c_int64, vp, vp, vp]),
+    "b200ms_search_host_masked": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_int, i32p, c_float, c_float, c_int64, vp, vp, vp]),
+    "b200ms_search_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_float, c_float, c_int64, vp, vp, vp, vp]),
+    "b200ms_search_device_masked": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64, vp, vp,
+                                    vp, vp]),
+    "b200ms_launch_count": (c_int64, [vp]),
+    "b200ms_last_score_ms": (c_float, [vp]),
+    "b200ms_set_tuning": (c_int, [vp, c_int64, c_int]),
+    "b200ms_set_option": (c_int, [vp, c_char_p, c_int64]),
+    "b200ms_rerank_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_float, c_float, vp, vp, vp, vp]),
+    "b200ms_rerank_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_float, c_float, vp, vp, vp, vp]),
+    "b200ms_comm_available": (c_int, []),
+    "b200ms_comm_unique_id": (c_int, [vp]),
+    "b200ms_comm_init": (c_int, [vp, vp, c_int, c_int]),
+    "b200ms_comm_adopt": (c_int, [vp, vp, c_int, c_int]),
+    "b200ms_comm_destroy": (c_int, [vp]),
+    "b200ms_comm_rank": (c_int, [vp]),
+    "b200ms_comm_world": (c_int, [vp]),
+    "b200ms_xchg_bytes": (c_int64, [c_int, c_int]),
+    "b200ms_bcast_device": (c_int, [vp, vp, c_int64, c_int, vp]),
+    "b200ms_allgather_topk": (c_int, [vp, vp, vp, c_int, c_int, vp, vp, vp, vp]),
+    "b200ms_send_device": (c_int, [vp, vp, c_int64, c_int, vp]),
+    "b200ms_recv_device": (c_int, [vp, vp, c_int64, c_int, vp]),
+    "b200ms_sharded_search_begin": (c_int64, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64, vp,
+                                    vp, vp, vp]),
+    "b200ms_sharded_search_end": (c_int, [vp, c_int64, vp]),
+    "b200ms_sharded_search_host_begin": (c_int64, [vp, vp, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64]),
+    "b200ms_sharded_search_host_end": (c_int, [vp, c_int64, vp, vp, vp]),
+    "b200ms_fde_configure_ex": (c_int, [vp, c_int, c_int, c_int, c_float, vp, vp, vp, c_int, c_int, vp, vp]),
+    "b200ms_fde_configure": (c_int, [vp, c_int, c_int, c_int, c_float, vp, vp, vp]),
+    "b200ms_fde_dim": (c_int64, [vp]),
+    "b200ms_fde_encode": (c_int, [vp, vp, c_int, i32p, c_int64, c_int, vp, vp]),
+    "b200ms_fde_finalize": (c_int, [vp, vp, c_int64, vp, vp, vp]),
+    "b200ms_fde_encode_corpus": (c_int, [vp, c_int64, c_int64, vp, vp]),
+    "b200ms_fde_scan": (c_int, [vp, vp, vp, c_int64, vp, c_int, vp, c_int64, vp]),
+    "b200ms_score_call_count": (c_int64, [vp]),
+    "b200ms_score_times_ms": (c_int, [vp, f32p, c_int]),
+    "b200ms_set_corpus_host": (c_int, [vp, vp, c_int, i32p, c_int64]),
+    "b200ms_host_alloc": (c_int, [vp, c_int64, POINTER(c_void_p)]),
+    "b200ms_host_free": (c_int, [vp, vp]),
+    "b200ms_last_gather_stats": (c_int, [vp, i64p, i64p, POINTER(c_int), f32p]),
+    "b200ms_explain_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, c_float, vp, vp, vp, c_int64, vp]),
+    "b200ms_topk_docs": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, vp, c_int64, c_int, c_int, c_float, c_int64,
+                                 vp, vp, vp, vp, vp]),
+    "b200ms_search_docs_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, c_int, vp, c_int64, vp, c_int, vp, c_float, c_float,
+                                          c_int64, vp, vp, vp, vp, vp]),
+    "b200ms_rerank_docs_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, c_float,
+                                                c_float, vp, vp, vp, vp, vp]),
+}
+
+
 def _declare(lib: ctypes.CDLL) -> ctypes.CDLL:
-    vp, i32p, i64p, u32p, f32p = c_void_p, POINTER(c_int32), POINTER(c_int64), POINTER(c_uint32), POINTER(c_float)
-    sig = {
-        "b200ms_version": (c_int, []),
-        "b200ms_device_count": (c_int, []),
-        "b200ms_create": (c_int, [c_int, POINTER(c_void_p)]),
-        "b200ms_destroy": (c_int, [vp]),
-        "b200ms_last_error": (c_char_p, [vp]),
-        "b200ms_padded_len": (c_int64, [c_int64]),
-        "b200ms_padded_rows": (c_int64, [i32p, c_int64]),
-        "b200ms_row_bytes": (c_int64, [c_int]),
-        "b200ms_query_groups": (c_int64, [i32p, c_int]),
-        "b200ms_sign_pack": (c_int, [vp, vp, c_int, c_int64, vp, vp]),
-        "b200ms_hamming_batch": (c_int, [vp, vp, vp, c_int64, vp, vp]),
-        "b200ms_pack_pages": (c_int, [vp, vp, c_int, i32p, c_int64, vp, c_int, c_float, vp]),
-        "b200ms_set_corpus": (c_int, [vp, vp, c_int, i32p, c_int64]),
-        "b200ms_corpus_pages": (c_int64, [vp]),
-        "b200ms_corpus_rows": (c_int64, [vp]),
-        "b200ms_pack_queries": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, i32p, POINTER(c_int), vp]),
-        "b200ms_score": (c_int, [vp, vp, c_int, i32p, i32p, c_int, vp, c_int64, vp]),
-        "b200ms_topk": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, c_int, c_float, c_int64, vp, vp, vp, vp]),
-        "b200ms_merge_topk": (c_int, [vp, vp, vp, c_int, c_int, c_int, vp, vp, vp, vp]),
-        "b200ms_search_host": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_float, c_float, c_int64, vp, vp, vp]),
-        "b200ms_search_host_masked": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_int, i32p, c_float, c_float, c_int64, vp, vp, vp]),
-        "b200ms_search_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_float, c_float, c_int64, vp, vp, vp, vp]),
-        "b200ms_search_device_masked": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64, vp, vp,
-                                        vp, vp]),
-        "b200ms_launch_count": (c_int64, [vp]),
-        "b200ms_last_score_ms": (c_float, [vp]),
-        "b200ms_set_tuning": (c_int, [vp, c_int64, c_int]),
-        "b200ms_set_option": (c_int, [vp, c_char_p, c_int64]),
-        "b200ms_rerank_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_float, c_float, vp, vp, vp, vp]),
-        "b200ms_rerank_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_float, c_float, vp, vp, vp, vp]),
-        "b200ms_comm_available": (c_int, []),
-        "b200ms_comm_unique_id": (c_int, [vp]),
-        "b200ms_comm_init": (c_int, [vp, vp, c_int, c_int]),
-        "b200ms_comm_adopt": (c_int, [vp, vp, c_int, c_int]),
-        "b200ms_comm_destroy": (c_int, [vp]),
-        "b200ms_comm_rank": (c_int, [vp]),
-        "b200ms_comm_world": (c_int, [vp]),
-        "b200ms_xchg_bytes": (c_int64, [c_int, c_int]),
-        "b200ms_bcast_device": (c_int, [vp, vp, c_int64, c_int, vp]),
-        "b200ms_allgather_topk": (c_int, [vp, vp, vp, c_int, c_int, vp, vp, vp, vp]),
-        "b200ms_send_device": (c_int, [vp, vp, c_int64, c_int, vp]),
-        "b200ms_recv_device": (c_int, [vp, vp, c_int64, c_int, vp]),
-        "b200ms_sharded_search_begin": (c_int64, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64, vp,
-                                        vp, vp, vp]),
-        "b200ms_sharded_search_end": (c_int, [vp, c_int64, vp]),
-        "b200ms_sharded_search_host_begin": (c_int64, [vp, vp, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, c_int64]),
-        "b200ms_sharded_search_host_end": (c_int, [vp, c_int64, vp, vp, vp]),
-        "b200ms_fde_configure_ex": (c_int, [vp, c_int, c_int, c_int, c_float, vp, vp, vp, c_int, c_int, vp, vp]),
-        "b200ms_fde_configure": (c_int, [vp, c_int, c_int, c_int, c_float, vp, vp, vp]),
-        "b200ms_fde_dim": (c_int64, [vp]),
-        "b200ms_fde_encode": (c_int, [vp, vp, c_int, i32p, c_int64, c_int, vp, vp]),
-        "b200ms_fde_finalize": (c_int, [vp, vp, c_int64, vp, vp, vp]),
-        "b200ms_fde_encode_corpus": (c_int, [vp, c_int64, c_int64, vp, vp]),
-        "b200ms_fde_scan": (c_int, [vp, vp, vp, c_int64, vp, c_int, vp, c_int64, vp]),
-        "b200ms_score_call_count": (c_int64, [vp]),
-        "b200ms_score_times_ms": (c_int, [vp, f32p, c_int]),
-        "b200ms_set_corpus_host": (c_int, [vp, vp, c_int, i32p, c_int64]),
-        "b200ms_host_alloc": (c_int, [vp, c_int64, POINTER(c_void_p)]),
-        "b200ms_host_free": (c_int, [vp, vp]),
-        "b200ms_last_gather_stats": (c_int, [vp, i64p, i64p, POINTER(c_int), f32p]),
-        "b200ms_explain_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, c_float, vp, vp, vp, c_int64, vp]),
-        "b200ms_topk_docs": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, vp, c_int64, c_int, c_int, c_float, c_int64,
-                                     vp, vp, vp, vp, vp]),
-        "b200ms_search_docs_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, c_int, vp, c_int64, vp, c_int, vp, c_float, c_float,
-                                              c_int64, vp, vp, vp, vp, vp]),
-        "b200ms_rerank_docs_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, c_float,
-                                                    c_float, vp, vp, vp, vp, vp]),
-    }
-    for name, (res, args) in sig.items():
+    for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
@@ -124,22 +127,7 @@ def _declare(lib: ctypes.CDLL) -> ctypes.CDLL:
 
 
 lib = _load()
-EXPORTED = [
-    "b200ms_version", "b200ms_device_count", "b200ms_create", "b200ms_destroy", "b200ms_last_error",
-    "b200ms_padded_len", "b200ms_padded_rows", "b200ms_row_bytes", "b200ms_query_groups", "b200ms_sign_pack",
-    "b200ms_pack_pages", "b200ms_set_corpus", "b200ms_corpus_pages", "b200ms_corpus_rows", "b200ms_pack_queries",
-    "b200ms_score", "b200ms_topk", "b200ms_merge_topk", "b200ms_search_host", "b200ms_search_host_masked", "b200ms_search_device", "b200ms_search_device_masked",
-    "b200ms_launch_count", "b200ms_last_score_ms", "b200ms_set_tuning", "b200ms_score_call_count",
-    "b200ms_score_times_ms", "b200ms_set_option", "b200ms_rerank_device", "b200ms_fde_configure", "b200ms_fde_dim",
-    "b200ms_fde_encode", "b200ms_fde_finalize", "b200ms_fde_scan", "b200ms_hamming_batch", "b200ms_rerank_batch_device",
-    "b200ms_comm_available", "b200ms_comm_unique_id", "b200ms_comm_init", "b200ms_comm_adopt", "b200ms_comm_destroy",
-    "b200ms_comm_rank", "b200ms_comm_world", "b200ms_xchg_bytes", "b200ms_bcast_device", "b200ms_allgather_topk",
-    "b200ms_sharded_search_begin", "b200ms_sharded_search_end", "b200ms_sharded_search_host_begin",
-    "b200ms_sharded_search_host_end", "b200ms_fde_configure_ex", "b200ms_fde_encode_corpus",
-    "b200ms_send_device", "b200ms_recv_device", "b200ms_set_corpus_host", "b200ms_host_alloc", "b200ms_host_free",
-    "b200ms_last_gather_stats", "b200ms_explain_device", "b200ms_topk_docs", "b200ms_search_docs_device",
-    "b200ms_rerank_docs_batch_device",
-]
+EXPORTED = list(_SIGNATURES)
 MAX_PER_DOC = 64
 
 

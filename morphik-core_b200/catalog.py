@@ -147,6 +147,23 @@ class PageCatalog:
             return np.zeros(0, dtype=np.uint32)
         return np.packbits(bits.reshape(-1, 32), axis=1, bitorder="little").view(np.uint32).reshape(-1).copy()
 
+    @staticmethod
+    def stack_masks(masks: Sequence[Optional[np.ndarray]]) -> Tuple[Optional[np.ndarray], List[int]]:
+        """One word array (or None = unfiltered) per query -> (matrix [n_distinct, words] with one row per distinct mask, or
+        None when no query is filtered; each query's row, -1 = unfiltered): the per-query filter format of the library.
+        Users sharing a filter share a row, so it is uploaded once."""
+        rows, index, seen = [], [], {}
+        for m in masks:
+            if m is None:
+                index.append(-1)
+                continue
+            key = m.tobytes()
+            if key not in seen:
+                seen[key] = len(rows)
+                rows.append(m)
+            index.append(seen[key])
+        return (np.stack(rows) if rows else None), index
+
     # ------------------------------------------------------------------ compaction
     def compaction_plan(self) -> Tuple[np.ndarray, np.ndarray]:
         """(kept old page ids in order, old->new id map with -1 for dropped pages)."""

@@ -37,7 +37,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .index import MaxSimIndex, _vp
+from .index import MaxSimIndex, _check_device_masks, _host_mask_to_device, _topk_outputs, _vp
 
 
 @dataclass(frozen=True)
@@ -319,43 +319,33 @@ class TwoStageIndex:
             self._inv = self._inv[: self._n].index_select(0, keep_t).contiguous()
         self._n = len(keep)
 
+    def _fde_topk(self, q_fde: torch.Tensor, kc: int, mask: Optional[torch.Tensor]):
+        """Scan of the FDE matrix for query FDEs [n_q, fde_dim] -> top kc pages per query among those `mask` (already
+        checked) allows: (scores, page ids, counts) on the device."""
+        n_q = q_fde.shape[0]
+        scores = self.fde_scores(q_fde)
+        ts, ti, tc = _topk_outputs(n_q, kc, self.device)
+        goff = nat.i32_array(list(range(n_q + 1)))
+        with torch.cuda.device(self.device):
+            self.index.h.check(
+                nat.lib.b200ms_topk(self.index.h.ptr, _vp(scores), nat.F32, self._n, scores.shape[1], goff, n_q, _vp(mask), kc,
+                                    ctypes.c_float(1.0), 0, _vp(ts), _vp(ti), _vp(tc), self.index._stream()),
+                "b200ms_topk(fde)")
+        return ts, ti, tc
+
     def candidates(self, queries: Sequence, n_candidates: int, allow_mask_dev: Optional[torch.Tensor] = None):
         """First stage only: (candidate page ids int64 [n_q, n_candidates] (-1 padded), FDE scores, counts) on the device.
         allow_mask_dev: optional uint32 page bitmask (the doc_ids filter, applied BEFORE candidate selection like the
         reference's Turbopuffer filter, fast_multivector_store.py:527)."""
-        n_q = len(queries)
+        mask, _, _ = _check_device_masks(allow_mask_dev, None, len(queries), self._n, self.device)
         q_fde = encode_items(self.index, list(queries), False, self.fde_dim)
-        scores = self.fde_scores(q_fde)
-        kk = int(min(n_candidates, nat.MAX_K))
-        ts = torch.empty((n_q, kk), dtype=torch.float32, device=self.device)
-        ti = torch.empty((n_q, kk), dtype=torch.int64, device=self.device)
-        tc = torch.empty((n_q,), dtype=torch.int32, device=self.device)
-        goff = nat.i32_array(list(range(n_q + 1)))
-        with torch.cuda.device(self.device):
-            self.index.h.check(
-                nat.lib.b200ms_topk(self.index.h.ptr, _vp(scores), nat.F32, self._n, scores.shape[1], goff, n_q,
-                                    _vp(allow_mask_dev), kk,
-                                    ctypes.c_float(1.0), 0, _vp(ts), _vp(ti), _vp(tc), self.index._stream()),
-                "b200ms_topk(fde)")
+        ts, ti, tc = self._fde_topk(q_fde, int(min(n_candidates, nat.MAX_K)), mask)
         return ti, ts, tc
 
     def rerank(self, query, cand_ids: torch.Tensor, k: int):
         """Exact MaxSim of ONE query over the candidate pages (device int64 [n_cand], -1 = unused) -> top-k."""
-        self.index._attach()
-        src, src_dtype = self.index._stage_rows([query])
-        n_cand = int(cand_ids.numel())
-        kk = int(min(k, n_cand))
-        ts = torch.empty((1, kk), dtype=torch.float32, device=self.device)
-        ti = torch.empty((1, kk), dtype=torch.int64, device=self.device)
-        tc = torch.empty((1,), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            self.index.h.check(
-                nat.lib.b200ms_rerank_device(self.index.h.ptr, _vp(src), src_dtype, nat.i32_array([int(query.shape[0])]), 1,
-                                             _vp(cand_ids.contiguous()), n_cand, kk, ctypes.c_float(self.index.i8_scale),
-                                             ctypes.c_float(self.index.score_scale), _vp(ts), _vp(ti), _vp(tc),
-                                             self.index._stream()),
-                "b200ms_rerank_device")
-        return ts, ti, tc
+        src, _ = self.index._stage_rows([query])
+        return self.index.rerank(src, [int(query.shape[0])], cand_ids.contiguous(), k)
 
     def search_device(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
                       id_base: int = 0):
@@ -363,23 +353,13 @@ class TwoStageIndex:
         whole batch (wgmma) -> top-n_candidates per query -> ONE batched rerank call (each query against its own list)
         -> top-k.  Returns device tensors (scores [n_q,kk], page ids + id_base [n_q,kk], counts [n_q]) and the CUDA events
         that bracket the stages (for last_timing_ms)."""
-        n_q = len(queries)
+        mask, _, _ = _check_device_masks(allow_mask_dev, None, len(queries), self._n, self.device)
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
         q_fde = encode_items(self.index, list(queries), False, self.fde_dim)
         ev[1].record()
-        scores = self.fde_scores(q_fde)
         kc = int(min(max(n_candidates, k), nat.MAX_K, max(self._n, 1)))
-        cs = torch.empty((n_q, kc), dtype=torch.float32, device=self.device)
-        ci = torch.empty((n_q, kc), dtype=torch.int64, device=self.device)
-        cc = torch.empty((n_q,), dtype=torch.int32, device=self.device)
-        goff = nat.i32_array(list(range(n_q + 1)))
-        with torch.cuda.device(self.device):
-            self.index.h.check(
-                nat.lib.b200ms_topk(self.index.h.ptr, _vp(scores), nat.F32, self._n, scores.shape[1], goff, n_q,
-                                    _vp(allow_mask_dev), kc, ctypes.c_float(1.0), 0, _vp(cs), _vp(ci), _vp(cc),
-                                    self.index._stream()),
-                "b200ms_topk(fde)")
+        _, ci, _ = self._fde_topk(q_fde, kc, mask)
         ev[2].record()
         src, _ = self.index._stage_rows(list(queries))
         ts, ti, tc = self.index.rerank_batch(src, [int(q.shape[0]) for q in queries], ci, k)
@@ -401,8 +381,7 @@ class TwoStageIndex:
                     n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
         """search_docs_device with a host allow mask (uint32 words, restricting both stages); synchronous, returns host
         arrays (scores [n_q,k,per_doc], page ids [n_q,k,per_doc], pages per document [n_q,k], documents [n_q])."""
-        mask_dev = None if allow_mask is None else torch.from_numpy(
-            self.index._check_mask(allow_mask).view(np.int32)).to(self.device)
+        mask_dev = _host_mask_to_device(allow_mask, self._n, self.device)
         ts, ti, pc, dc = self.search_docs_device(queries, k, per_doc, page_doc_dev, n_docs, n_candidates, mask_dev)
         n_q, kk = len(queries), ts.shape[1]
         out_s = np.full((n_q, k, per_doc), -np.inf, dtype=np.float32)
@@ -422,8 +401,7 @@ class TwoStageIndex:
         + candidate top-k on the GPU) / load_multivectors (0: resident in HBM) / rerank_scoring.
         allow_mask: optional uint32 words (page bitmask) restricting BOTH stages (the reference filters inside the ANN query)."""
         n_q = len(queries)
-        mask_dev = None if allow_mask is None else torch.from_numpy(
-            self.index._check_mask(allow_mask).view(np.int32)).to(self.device)
+        mask_dev = _host_mask_to_device(allow_mask, self._n, self.device)
         ts, ti, tc, ev = self.search_device(queries, k, n_candidates, mask_dev)
         torch.cuda.synchronize(self.device)
         kk = ts.shape[1]

@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
+from .catalog import PageCatalog
 
 ArrayLike = Union[np.ndarray, torch.Tensor]
 
@@ -32,6 +33,105 @@ def _aligned_bytes(nbytes: int, device: torch.device, align: int = 1024) -> torc
     raw = torch.empty(max(int(nbytes), 1) + align, dtype=torch.uint8, device=device)
     off = (-raw.data_ptr()) % align
     return raw[off:off + max(int(nbytes), 1)]
+
+
+def _padded_lens(lens: Sequence[int]) -> np.ndarray:
+    """int64 rows each page occupies in the packed layout: its length rounded up to whole 32-row groups
+    (= b200ms_padded_len, computed here for every page at once)."""
+    return -(-np.asarray(lens, dtype=np.int64) // nat.ROW_GROUP) * nat.ROW_GROUP
+
+
+def _runs(ids: Sequence[int]):
+    """(first, last) of every maximal run of consecutive ids in ascending `ids`."""
+    i = 0
+    while i < len(ids):
+        j = i
+        while j + 1 < len(ids) and ids[j + 1] == ids[j] + 1:
+            j += 1
+        yield ids[i], ids[j]
+        i = j + 1
+
+
+# ---- argument checks of the device calls: tensor metadata only (no value is read, nothing synchronises or is allocated),
+# so a tensor the library would read past its end or in the wrong format is refused with ValueError before any launch
+def _check_queries(q_dev: torch.Tensor, q_lens: Sequence[int], device: torch.device) -> int:
+    """Query rows: contiguous float32/bfloat16 [>= sum(q_lens), 128] on `device`.  Returns the library's dtype code."""
+    if q_dev.dtype not in (torch.float32, torch.bfloat16) or not q_dev.is_contiguous() or q_dev.device != device:
+        raise ValueError(f"q_dev must be a contiguous float32/bfloat16 tensor on {device}, got {q_dev.dtype} on {q_dev.device}")
+    rows = sum(int(n) for n in q_lens)
+    if q_dev.ndim != 2 or q_dev.shape[1] != nat.DIM or q_dev.shape[0] < rows:
+        raise ValueError(f"q_dev must be [>= sum(q_lens) = {rows}, {nat.DIM}], got {tuple(q_dev.shape)}")
+    return nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32
+
+
+def _check_device_masks(allow_mask_dev: Optional[torch.Tensor], mask_index_dev: Optional[torch.Tensor], n_q: int,
+                        n_pages: int, device: torch.device):
+    """Allow filter on `device`, int32/uint32 words (bit p&31 of word p>>5): one [ceil(n_pages/32)] row for every query, or a
+    [n_masks, ceil(n_pages/32)] matrix with ``mask_index_dev`` int32 [n_q] naming each query's row (-1 = unfiltered).
+    Returns (masks, n_masks, index) for the C call: (None, 0, None) unfiltered, (row, 1, None) for one row."""
+    words = (n_pages + 31) // 32
+    if allow_mask_dev is None:
+        if mask_index_dev is not None:
+            raise ValueError("mask_index_dev needs allow_mask_dev")
+        return None, 0, None
+    m = allow_mask_dev
+    if m.dtype not in (torch.int32, torch.uint32) or not m.is_contiguous() or m.device != device:
+        raise ValueError(f"allow_mask_dev must be a contiguous int32/uint32 tensor on {device}, got {m.dtype} on {m.device}")
+    if mask_index_dev is None:
+        if tuple(m.shape) != (words,):
+            raise ValueError(f"allow_mask_dev must have {words} words for {n_pages} pages, got shape {tuple(m.shape)}")
+        return m, 1, None
+    if m.ndim != 2 or m.shape[1] != words:
+        raise ValueError(f"per-query masks: allow_mask_dev must be a [n_masks, {words}] word matrix, got {tuple(m.shape)}")
+    mi = mask_index_dev
+    if mi.dtype != torch.int32 or tuple(mi.shape) != (n_q,) or not mi.is_contiguous() or mi.device != device:
+        raise ValueError(f"mask_index_dev must be a contiguous int32 [{n_q}] tensor on {device}")
+    return m, int(m.shape[0]), mi
+
+
+def _host_mask_words(allow_mask, n_pages: int) -> np.ndarray:
+    """Host allow mask -> contiguous uint32 words.  The library reads ceil(n_pages/32) words: a mask built for an older
+    (shorter) corpus must never reach it."""
+    m = np.ascontiguousarray(allow_mask, dtype=np.uint32)
+    words = (n_pages + 31) // 32
+    if m.shape != (words,):
+        raise ValueError(f"allow-mask must have {words} uint32 words for {n_pages} pages, got shape {m.shape}")
+    return m
+
+
+def _host_mask_to_device(allow_mask: Optional[np.ndarray], n_pages: int, device: torch.device) -> Optional[torch.Tensor]:
+    """Checked host allow mask (uint32 words) -> int32 words on `device`; None stays None (unfiltered)."""
+    if allow_mask is None:
+        return None
+    return torch.from_numpy(_host_mask_words(allow_mask, n_pages).view(np.int32)).to(device)
+
+
+def _check_candidates(cand_ids: torch.Tensor, n_q: int, k: int, device: torch.device, per_query: bool) -> Tuple[int, int]:
+    """Candidate page ids: contiguous int64 [n_cand] shared by every query, or with ``per_query`` [n_q, n_cand], on `device`.
+    Returns (n_cand, k capped at n_cand)."""
+    shape = "[n_q, n_cand]" if per_query else "[n_cand]"
+    ok_shape = cand_ids.ndim == 2 and cand_ids.shape[0] == n_q if per_query else cand_ids.ndim == 1
+    if cand_ids.dtype != torch.int64 or not ok_shape or not cand_ids.is_contiguous() or cand_ids.device != device:
+        raise ValueError(f"cand_ids must be a contiguous int64 {shape} tensor on {device} (n_q = {n_q}), "
+                         f"got {cand_ids.dtype} {tuple(cand_ids.shape)} on {cand_ids.device}")
+    n_cand = int(cand_ids.shape[-1])
+    return n_cand, int(min(k, n_cand))
+
+
+def _topk_outputs(n_q: int, k: int, device: torch.device, out=None, per_doc: int = 0):
+    """Result buffers of a top-k call on `device`: (scores float32 [n_q,k], page ids int64 [n_q,k], counts int32 [n_q]), or
+    with ``per_doc`` the grouped form (scores float32 [n_q,k,per_doc], page ids int64 [n_q,k,per_doc], pages per document
+    int32 [n_q,k], documents int32 [n_q]).  Allocated when `out` is None, else the caller's tuple is checked to be exactly
+    that and returned."""
+    row = (n_q, k, per_doc) if per_doc else (n_q, k)
+    specs = [(row, torch.float32), (row, torch.int64)] + ([((n_q, k), torch.int32)] if per_doc else []) + [((n_q,), torch.int32)]
+    if out is None:
+        return tuple(torch.empty(shape, dtype=dt, device=device) for shape, dt in specs)
+    if len(out) != len(specs) or any(tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous() or t.device != device
+                                     for t, (shape, dt) in zip(out, specs)):
+        want = ", ".join(f"{str(dt).replace('torch.', '')} {list(shape)}" for shape, dt in specs)
+        raise ValueError(f"out must be contiguous tensors on {device}: {want}")
+    return tuple(out)
 
 
 class HostBlock:
@@ -255,7 +355,7 @@ class MaxSimIndex:
             cat = cat.contiguous()
             if cat.shape[0] == 0:
                 cat = torch.zeros((1, nat.DIM), dtype=dt, device=self.device)
-            return cat, (nat.BF16 if dt == torch.bfloat16 else nat.F32)
+            return cat, _check_queries(cat, (), self.device)
         mats = [np.asarray(m.cpu() if isinstance(m, torch.Tensor) else m, dtype=np.float32) for m in mats]
         total = int(sum(m.shape[0] for m in mats))
         if total == 0:
@@ -316,9 +416,9 @@ class MaxSimIndex:
 
     def page_row_range(self, first: int, n: int) -> Tuple[int, int]:
         """Padded row range [r0, r1) that pages [first, first+n) occupy in the packed buffer."""
-        pad = [(x + 31) // 32 * 32 for x in self._page_lens]
-        r0 = int(sum(pad[:first]))
-        return r0, r0 + int(sum(pad[first:first + n]))
+        pad = _padded_lens(self._page_lens)
+        r0 = int(pad[:first].sum())
+        return r0, r0 + int(pad[first:first + n].sum())
 
     def _attach(self):
         if self._attached:
@@ -345,37 +445,26 @@ class MaxSimIndex:
         the surviving page runs into a fresh buffer (DELETE ... WHERE document_id, multi_vector_store.py:929-933)."""
         keep = [int(p) for p in keep]
         lens = self._page_lens
-        pad = [(n + 31) // 32 * 32 for n in lens]
+        pad = _padded_lens(lens)
         starts = np.concatenate([[0], np.cumsum(pad)]).astype(np.int64)
-        new_rows = int(sum(pad[p] for p in keep))
+        new_rows = int(pad[keep].sum())
         if self.tier == "host":  # in place: surviving runs move down with forward (overlap-safe) host copies
             self._host_barrier()
-            base, dst, i = self._buf.data_ptr(), 0, 0
-            while i < len(keep):
-                j = i
-                while j + 1 < len(keep) and keep[j + 1] == keep[j] + 1:
-                    j += 1
-                a, b = int(starts[keep[i]]) * self.row_bytes, int(starts[keep[j] + 1]) * self.row_bytes
+            base = self._buf.data_ptr()
+        else:
+            new_buf = _aligned_bytes(max(new_rows, 4096) * self.row_bytes, self.device)
+        dst = 0
+        for first, last in _runs(keep):  # one copy per maximal run of consecutive surviving pages
+            a, b = int(starts[first]) * self.row_bytes, int(starts[last + 1]) * self.row_bytes
+            if self.tier == "host":
                 if dst != a:
                     ctypes.memmove(base + dst, base + a, b - a)
-                dst += b - a
-                i = j + 1
-            self._rows = new_rows
-            self._page_lens = [lens[p] for p in keep]
-            self._attached = False
-            return
-        new_buf = _aligned_bytes(max(new_rows, 4096) * self.row_bytes, self.device)
-        dst = 0
-        i = 0
-        while i < len(keep):  # copy maximal runs of consecutive surviving pages
-            j = i
-            while j + 1 < len(keep) and keep[j + 1] == keep[j] + 1:
-                j += 1
-            a, b = int(starts[keep[i]]) * self.row_bytes, int(starts[keep[j] + 1]) * self.row_bytes
-            new_buf[dst:dst + (b - a)].copy_(self._buf[a:b])
+            else:
+                new_buf[dst:dst + (b - a)].copy_(self._buf[a:b])
             dst += b - a
-            i = j + 1
-        self._buf, self._cap_rows, self._rows = new_buf, new_buf.numel() // self.row_bytes, new_rows
+        if self.tier == "hbm":
+            self._buf, self._cap_rows = new_buf, new_buf.numel() // self.row_bytes
+        self._rows = new_rows
         self._page_lens = [lens[p] for p in keep]
         self._attached = False
 
@@ -406,17 +495,10 @@ class MaxSimIndex:
         allowed = np.asarray(allowed, dtype=bool)
         if allowed.shape[0] != self.n_pages:
             raise ValueError("mask length must equal n_pages")
-        pad = (-len(allowed)) % 32
-        bits = np.concatenate([allowed, np.zeros(pad, dtype=bool)]) if pad else allowed
-        return np.packbits(bits.reshape(-1, 32), axis=1, bitorder="little").view(np.uint32).reshape(-1).copy()
+        return PageCatalog.mask_words(allowed)
 
     def _check_mask(self, allow_mask) -> np.ndarray:
-        """The library reads ceil(n_pages/32) words: a mask built for an older (shorter) corpus must never reach it."""
-        m = np.ascontiguousarray(allow_mask, dtype=np.uint32)
-        words = (self.n_pages + 31) // 32
-        if m.shape != (words,):
-            raise ValueError(f"allow-mask must have {words} uint32 words for {self.n_pages} pages, got shape {m.shape}")
-        return m
+        return _host_mask_words(allow_mask, self.n_pages)
 
     def search_host(self, queries: Sequence[np.ndarray], k: int, allow_mask: Optional[np.ndarray] = None,
                     id_base: int = 0, out: Optional[Tuple[np.ndarray, np.ndarray, np.ndarray]] = None):
@@ -459,26 +541,13 @@ class MaxSimIndex:
         if len(allow_masks) != n_q:
             raise ValueError("one allow-mask (or None) per query")
         q_host = np.ascontiguousarray(np.concatenate([np.asarray(q, dtype=np.float32) for q in queries], axis=0))
-        words = (self.n_pages + 31) // 32
-        rows, index, seen = [], [], {}
-        for m in allow_masks:
-            if m is None:
-                index.append(-1)
-                continue
-            m = np.ascontiguousarray(m, dtype=np.uint32)
-            if m.shape != (words,):
-                raise ValueError(f"allow-mask must have {words} uint32 words, got {m.shape}")
-            key = m.tobytes()
-            if key not in seen:
-                seen[key] = len(rows)
-                rows.append(m)
-            index.append(seen[key])
+        mat, index = PageCatalog.stack_masks([None if m is None else self._check_mask(m) for m in allow_masks])
         ts, ti, tc = np.empty((n_q, k), np.float32), np.empty((n_q, k), np.int64), np.empty((n_q,), np.int32)
-        mat = np.stack(rows) if rows else None
         self.h.check(
             nat.lib.b200ms_search_host_masked(
                 self.h.ptr, q_host.ctypes.data_as(ctypes.c_void_p), nat.i32_array(lens), n_q, int(k),
-                None if mat is None else mat.ctypes.data_as(ctypes.c_void_p), len(rows), nat.i32_array(index),
+                None if mat is None else mat.ctypes.data_as(ctypes.c_void_p), 0 if mat is None else len(mat),
+                nat.i32_array(index),
                 ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base),
                 ts.ctypes.data_as(ctypes.c_void_p), ti.ctypes.data_as(ctypes.c_void_p), tc.ctypes.data_as(ctypes.c_void_p)),
             "b200ms_search_host_masked",
@@ -517,26 +586,16 @@ class MaxSimIndex:
 
         ``allow_mask_dev``: one mask (int32/uint32 words) for every query, or -- with ``mask_index_dev`` (int32 [n_q], -1 =
         unfiltered) -- a [n_masks, words] matrix with one row per distinct filter (b200ms_search_device_masked)."""
-        self._attach()
         n_q = len(q_lens)
-        if q_dev.dtype not in (torch.float32, torch.bfloat16) or not q_dev.is_contiguous():
-            raise ValueError("q_dev must be a contiguous float32/bfloat16 tensor")
-        if out is None:
-            out = (torch.empty((n_q, k), dtype=torch.float32, device=self.device),
-                   torch.empty((n_q, k), dtype=torch.int64, device=self.device),
-                   torch.empty((n_q,), dtype=torch.int32, device=self.device))
-        ts, ti, tc = out
-        if mask_index_dev is not None:
-            if (allow_mask_dev is None or allow_mask_dev.ndim != 2 or allow_mask_dev.shape[1] != (self.n_pages + 31) // 32
-                    or not allow_mask_dev.is_contiguous()):
-                raise ValueError("per-query masks: allow_mask_dev must be a contiguous [n_masks, ceil(n_pages/32)] word matrix")
-            if mask_index_dev.dtype != torch.int32 or mask_index_dev.numel() != n_q:
-                raise ValueError("mask_index_dev must be int32 [n_q]")
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, n_q, self.n_pages, self.device)
+        ts, ti, tc = _topk_outputs(n_q, int(k), self.device, out)
+        self._attach()
+        if index is not None:
             with torch.cuda.device(self.device):
                 self.h.check(
                     nat.lib.b200ms_search_device_masked(
-                        self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens),
-                        n_q, int(k), _vp(allow_mask_dev), int(allow_mask_dev.shape[0]), _vp(mask_index_dev),
+                        self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, int(k), _vp(masks), n_masks, _vp(index),
                         ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base), _vp(ts), _vp(ti),
                         _vp(tc), self._stream()),
                     "b200ms_search_device_masked",
@@ -544,8 +603,7 @@ class MaxSimIndex:
             return ts, ti, tc
         with torch.cuda.device(self.device):
             self.h.check(
-                nat.lib.b200ms_search_device(self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32,
-                                             nat.i32_array(q_lens), n_q, int(k), _vp(allow_mask_dev),
+                nat.lib.b200ms_search_device(self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, int(k), _vp(masks),
                                              ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base),
                                              _vp(ts), _vp(ti), _vp(tc), self._stream()),
                 "b200ms_search_device",
@@ -629,9 +687,7 @@ class MaxSimIndex:
     def merge_topk(self, cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int):
         """Merge candidate lists [n_q, m] (ids < 0 ignored) -> top-k by (score desc, id asc), on the device."""
         n_q, m = cand_scores.shape
-        ts = torch.empty((n_q, k), dtype=torch.float32, device=self.device)
-        ti = torch.empty((n_q, k), dtype=torch.int64, device=self.device)
-        tc = torch.empty((n_q,), dtype=torch.int32, device=self.device)
+        ts, ti, tc = _topk_outputs(n_q, int(k), self.device)
         with torch.cuda.device(self.device):
             self.h.check(
                 nat.lib.b200ms_merge_topk(self.h.ptr, _vp(cand_scores.contiguous()), _vp(cand_ids.contiguous()), n_q, m, int(k),
@@ -644,19 +700,14 @@ class MaxSimIndex:
     def rerank(self, q_dev: torch.Tensor, q_lens: Sequence[int], cand_ids: torch.Tensor, k: int):
         """Exact MaxSim of every query over ONE shared candidate list: cand_ids int64 [n_cand] on the device (-1 = unused
         slot) -> (scores [n_q,k], page ids [n_q,k], counts [n_q]) on the device (b200ms_rerank_device)."""
-        self._attach()
         n_q = len(q_lens)
-        if cand_ids.dtype != torch.int64 or not cand_ids.is_contiguous():
-            raise ValueError("cand_ids must be a contiguous int64 device tensor")
-        n_cand = int(cand_ids.numel())
-        kk = int(min(k, n_cand))
-        ts = torch.empty((n_q, kk), dtype=torch.float32, device=self.device)
-        ti = torch.empty((n_q, kk), dtype=torch.int64, device=self.device)
-        tc = torch.empty((n_q,), dtype=torch.int32, device=self.device)
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        n_cand, kk = _check_candidates(cand_ids, n_q, k, self.device, per_query=False)
+        ts, ti, tc = _topk_outputs(n_q, kk, self.device)
+        self._attach()
         with torch.cuda.device(self.device):
             self.h.check(
-                nat.lib.b200ms_rerank_device(self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32,
-                                             nat.i32_array(q_lens), n_q, _vp(cand_ids), n_cand, kk,
+                nat.lib.b200ms_rerank_device(self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, _vp(cand_ids), n_cand, kk,
                                              ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), _vp(ts), _vp(ti),
                                              _vp(tc), self._stream()),
                 "b200ms_rerank_device")
@@ -667,41 +718,27 @@ class MaxSimIndex:
         """Exact MaxSim of every query over ITS OWN candidate list: cand_ids int64 [n_q, n_cand] on the device (-1 = unused
         slot) -> (scores [n_q,k], page ids [n_q,k], counts [n_q]) on the device; one call for the whole batch
         (b200ms_rerank_batch_device; fast_multivector_store.py:545-557 does this one query at a time on <= 75 pages)."""
-        self._attach()
         n_q = len(q_lens)
-        if cand_ids.dtype != torch.int64 or cand_ids.ndim != 2 or cand_ids.shape[0] != n_q or not cand_ids.is_contiguous():
-            raise ValueError("cand_ids must be a contiguous int64 [n_q, n_cand] device tensor")
-        n_cand = int(cand_ids.shape[1])
-        kk = int(min(k, n_cand))
-        if out is None:
-            out = (torch.empty((n_q, kk), dtype=torch.float32, device=self.device),
-                   torch.empty((n_q, kk), dtype=torch.int64, device=self.device),
-                   torch.empty((n_q,), dtype=torch.int32, device=self.device))
-        ts, ti, tc = out
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        n_cand, kk = _check_candidates(cand_ids, n_q, k, self.device, per_query=True)
+        ts, ti, tc = _topk_outputs(n_q, kk, self.device, out)
+        self._attach()
         with torch.cuda.device(self.device):
             self.h.check(
-                nat.lib.b200ms_rerank_batch_device(self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32,
-                                                   nat.i32_array(q_lens), n_q, _vp(cand_ids), n_cand, kk,
+                nat.lib.b200ms_rerank_batch_device(self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, _vp(cand_ids),
+                                                   n_cand, kk,
                                                    ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), _vp(ts),
                                                    _vp(ti), _vp(tc), self._stream()),
                 "b200ms_rerank_batch_device")
         return ts, ti, tc
 
     # ------------------------------------------------------------------ grouping results by document
-    def _check_docs_args(self, q_dev: torch.Tensor, per_doc: int, page_doc_dev: torch.Tensor):
-        if q_dev.dtype not in (torch.float32, torch.bfloat16) or not q_dev.is_contiguous():
-            raise ValueError("q_dev must be a contiguous float32/bfloat16 tensor")
+    def _check_docs_args(self, per_doc: int, page_doc_dev: torch.Tensor):
         if not 1 <= int(per_doc) <= nat.MAX_PER_DOC:
             raise ValueError(f"per_doc must be in [1, {nat.MAX_PER_DOC}]")
         if (page_doc_dev.dtype != torch.int32 or page_doc_dev.shape != (self.n_pages,) or not page_doc_dev.is_contiguous()
                 or page_doc_dev.device != self.device):
             raise ValueError(f"page_doc_dev must be a contiguous int32 [{self.n_pages}] tensor on {self.device}")
-
-    def _docs_outputs(self, n_q: int, k: int, per_doc: int):
-        return (torch.empty((n_q, k, per_doc), dtype=torch.float32, device=self.device),
-                torch.empty((n_q, k, per_doc), dtype=torch.int64, device=self.device),
-                torch.empty((n_q, k), dtype=torch.int32, device=self.device),
-                torch.empty((n_q,), dtype=torch.int32, device=self.device))
 
     def search_docs_device(self, q_dev: torch.Tensor, q_lens: Sequence[int], k: int, per_doc: int, page_doc_dev: torch.Tensor,
                            n_docs: int, allow_mask_dev: Optional[torch.Tensor] = None,
@@ -713,31 +750,20 @@ class MaxSimIndex:
         ranking and their search_device scores.  Masks as search_device.  Returns device tensors (scores float32
         [n_q,k,per_doc], page ids + id_base int64 [n_q,k,per_doc], pages per document int32 [n_q,k], documents int32 [n_q]);
         unused entries are -inf / -1 / 0."""
-        self._attach()
         n_q = len(q_lens)
-        self._check_docs_args(q_dev, per_doc, page_doc_dev)
-        words = (self.n_pages + 31) // 32
-        n_masks = 0
-        if mask_index_dev is not None:
-            if (allow_mask_dev is None or allow_mask_dev.ndim != 2 or allow_mask_dev.shape[1] != words
-                    or not allow_mask_dev.is_contiguous()):
-                raise ValueError("per-query masks: allow_mask_dev must be a contiguous [n_masks, ceil(n_pages/32)] word matrix")
-            if mask_index_dev.dtype != torch.int32 or mask_index_dev.numel() != n_q:
-                raise ValueError("mask_index_dev must be int32 [n_q]")
-            n_masks = int(allow_mask_dev.shape[0])
-        elif allow_mask_dev is not None:  # one mask for every query: a one-row matrix
-            if allow_mask_dev.shape != (words,) or not allow_mask_dev.is_contiguous():
-                raise ValueError(f"allow_mask_dev must have {words} words for {self.n_pages} pages")
-            mask_index_dev = torch.zeros((n_q,), dtype=torch.int32, device=self.device)
-            n_masks = 1
-        ts, ti, pc, dc = self._docs_outputs(n_q, int(k), int(per_doc))
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        self._check_docs_args(per_doc, page_doc_dev)
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, n_q, self.n_pages, self.device)
+        ts, ti, pc, dc = _topk_outputs(n_q, int(k), self.device, per_doc=int(per_doc))
+        if masks is not None and index is None:  # one mask for every query: a one-row matrix
+            index = torch.zeros((n_q,), dtype=torch.int32, device=self.device)
+        self._attach()
         with torch.cuda.device(self.device):
             self.h.check(
                 nat.lib.b200ms_search_docs_device(
-                    self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens), n_q,
-                    int(k), int(per_doc), _vp(page_doc_dev), int(n_docs), _vp(allow_mask_dev) if n_masks else None, n_masks,
-                    _vp(mask_index_dev) if n_masks else None, ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale),
-                    int(id_base), _vp(ts), _vp(ti), _vp(pc), _vp(dc), self._stream()),
+                    self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, int(k), int(per_doc), _vp(page_doc_dev),
+                    int(n_docs), _vp(masks), n_masks, _vp(index), ctypes.c_float(self.i8_scale),
+                    ctypes.c_float(self.score_scale), int(id_base), _vp(ts), _vp(ti), _vp(pc), _vp(dc), self._stream()),
                 "b200ms_search_docs_device")
         return ts, ti, pc, dc
 
@@ -747,7 +773,7 @@ class MaxSimIndex:
         host arrays."""
         lens = self._q_lens(queries)
         src, _ = self._stage_rows(list(queries))
-        mask_dev = None if allow_mask is None else torch.from_numpy(self._check_mask(allow_mask).view(np.int32)).to(self.device)
+        mask_dev = _host_mask_to_device(allow_mask, self.n_pages, self.device)
         out = self.search_docs_device(src, lens, k, per_doc, page_doc_dev, n_docs, allow_mask_dev=mask_dev)
         return tuple(t.cpu().numpy() for t in out)
 
@@ -756,20 +782,18 @@ class MaxSimIndex:
         """rerank_batch grouped by document (b200ms_rerank_docs_batch_device): each query's own candidate list cand_ids int64
         [n_q, n_cand] (-1 = unused slot) is ranked as rerank_batch ranks it, and a page listed in several slots counts once,
         at its earliest slot.  k is capped at n_cand.  Outputs as search_docs_device."""
-        self._attach()
         n_q = len(q_lens)
-        if cand_ids.dtype != torch.int64 or cand_ids.ndim != 2 or cand_ids.shape[0] != n_q or not cand_ids.is_contiguous():
-            raise ValueError("cand_ids must be a contiguous int64 [n_q, n_cand] device tensor")
-        self._check_docs_args(q_dev, per_doc, page_doc_dev)
-        n_cand = int(cand_ids.shape[1])
-        kk = int(min(k, n_cand))
-        ts, ti, pc, dc = self._docs_outputs(n_q, kk, int(per_doc))
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        n_cand, kk = _check_candidates(cand_ids, n_q, k, self.device, per_query=True)
+        self._check_docs_args(per_doc, page_doc_dev)
+        ts, ti, pc, dc = _topk_outputs(n_q, kk, self.device, per_doc=int(per_doc))
+        self._attach()
         with torch.cuda.device(self.device):
             self.h.check(
                 nat.lib.b200ms_rerank_docs_batch_device(
-                    self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens), n_q,
-                    _vp(cand_ids), n_cand, kk, int(per_doc), _vp(page_doc_dev), int(n_docs), ctypes.c_float(self.i8_scale),
-                    ctypes.c_float(self.score_scale), _vp(ts), _vp(ti), _vp(pc), _vp(dc), self._stream()),
+                    self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, _vp(cand_ids), n_cand, kk, int(per_doc),
+                    _vp(page_doc_dev), int(n_docs), ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), _vp(ts),
+                    _vp(ti), _vp(pc), _vp(dc), self._stream()),
                 "b200ms_rerank_docs_batch_device")
         return ts, ti, pc, dc
 
@@ -852,11 +876,7 @@ class MaxSimIndex:
     def allgather_topk(self, xchg: torch.Tensor, n_q: int, k: int, out=None):
         """The one collective of the path for a caller-made local list: xchg = uint8 device buffer in the exchange layout
         ([n_q*k int64 global ids][n_q*k float32 scores]) -> merged (scores, ids, counts), identical on every rank."""
-        if out is None:
-            out = (torch.empty((n_q, k), dtype=torch.float32, device=self.device),
-                   torch.empty((n_q, k), dtype=torch.int64, device=self.device),
-                   torch.empty((n_q,), dtype=torch.int32, device=self.device))
-        ts, ti, tc = out
+        ts, ti, tc = _topk_outputs(int(n_q), int(k), self.device, out)
         with torch.cuda.device(self.device):
             self.h.check(nat.lib.b200ms_allgather_topk(self.h.ptr, None, _vp(xchg), int(n_q), int(k), _vp(ts), _vp(ti), _vp(tc),
                                                        self._stream()), "b200ms_allgather_topk")
@@ -867,14 +887,16 @@ class MaxSimIndex:
                              allow_masks_dev: Optional[torch.Tensor] = None, mask_index_dev: Optional[torch.Tensor] = None) -> int:
         """Enqueue local scan + top-k on torch's current stream and the all-gather + merge behind it on the handle's
         communication stream; returns a ticket.  The current stream does not wait for the other ranks."""
+        n_q = len(q_lens)
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        masks, n_masks, index = _check_device_masks(allow_masks_dev, mask_index_dev, n_q, self.n_pages, self.device)
+        ts, ti, tc = _topk_outputs(n_q, int(k), self.device, out)
         self._attach()
-        ts, ti, tc = out
-        n_masks = 0 if allow_masks_dev is None else int(allow_masks_dev.shape[0])
         with torch.cuda.device(self.device):
             t = int(nat.lib.b200ms_sharded_search_begin(
-                self.h.ptr, _vp(q_dev), nat.BF16 if q_dev.dtype == torch.bfloat16 else nat.F32, nat.i32_array(q_lens), len(q_lens),
-                int(k), _vp(allow_masks_dev), n_masks, _vp(mask_index_dev), ctypes.c_float(self.i8_scale),
-                ctypes.c_float(self.score_scale), int(id_base), _vp(ts), _vp(ti), _vp(tc), self._stream()))
+                self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), n_q, int(k), _vp(masks), n_masks, _vp(index),
+                ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base), _vp(ts), _vp(ti), _vp(tc),
+                self._stream()))
         if t < 0:
             self.h.check(t, "b200ms_sharded_search_begin")
         return t

@@ -122,11 +122,9 @@ class ShardedMaxSim:
         (ticket, (scores, ids, counts)); the tensors are valid after ``end(ticket)``.  At most two tickets in flight."""
         if self.index is None:
             raise RuntimeError("begin/end need the CUDA index (ShardedMaxSim.from_index)")
-        n_q = len(q_lens)
-        if out is None:
-            dev = self.index.device
-            out = (torch.empty((n_q, k), dtype=torch.float32, device=dev), torch.empty((n_q, k), dtype=torch.int64, device=dev),
-                   torch.empty((n_q,), dtype=torch.int32, device=dev))
+        from .index import _topk_outputs
+
+        out = _topk_outputs(len(q_lens), k, self.index.device, out)
         t = self.index.sharded_search_begin(q, q_lens, k, self.id_base, out, allow_masks_dev, mask_index_dev)
         return t, out
 

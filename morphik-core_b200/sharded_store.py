@@ -39,7 +39,7 @@ import torch.distributed as dist
 from .catalog import PageCatalog, PageRecord
 from .models import DocumentChunk
 from .sharded import ShardedMaxSim, exchange_bytes, exchange_views, gathered_candidates
-from .store import BaseVectorStore, QueryCoalescer, _QueryRequest, as_query_matrix, build_store_metrics
+from .store import BaseVectorStore, QueryCoalescer, _document_chunk, _QueryRequest, as_query_matrix, build_store_metrics
 
 logger = logging.getLogger(__name__)
 RANK_SHIFT = 40
@@ -190,21 +190,15 @@ class ShardedB200MultiVectorStore(QueryCoalescer, BaseVectorStore):
     def _build_masks(self, filters) -> None:
         cat = self.catalogs[self.rank]
         n = len(cat)
-        rows, index, seen = [], [], {}
+        masks = []
         for doc_ids, app_id in filters:
             visible, words = cat.allow_words(doc_ids, app_id) if n else (False, None)
             if not visible:  # nothing authorised on this rank: an all-zero mask keeps the query out of the local top-k
                 words = np.zeros((n + 31) // 32, dtype=np.uint32)
-            if words is None:
-                index.append(-1)
-                continue
-            key = words.tobytes()
-            if key not in seen:
-                seen[key] = len(rows)
-                rows.append(words)
-            index.append(seen[key])
-        if rows and n:
-            self._mask_matrix = torch.from_numpy(np.stack(rows).view(np.int32)).to(self.data_device)
+            masks.append(words)
+        mat, index = PageCatalog.stack_masks(masks)
+        if mat is not None and n:
+            self._mask_matrix = torch.from_numpy(mat.view(np.int32)).to(self.data_device)
             self._mask_index = torch.tensor(index, dtype=torch.int32, device=self.data_device)
         else:
             self._mask_matrix = self._mask_index = None
@@ -401,9 +395,7 @@ class ShardedB200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 hits = []
                 for j in range(min(int(tc[i]), r.k)):
                     rk, local = split_global_id(ti[i, j])
-                    rec = self.catalogs[rk].records[local]
-                    hits.append(DocumentChunk(document_id=rec.document_id, chunk_number=rec.chunk_number, content=rec.content,
-                                              embedding=[], metadata=dict(rec.metadata), score=float(ts[i, j])))
+                    hits.append(_document_chunk(self.catalogs[rk].records[local], ts[i, j]))
                 out.append(hits)
         t2 = time.perf_counter()
         self.last_query_timing = {"coalesced_queries": float(len(batch)), "gpu_search_ms": (t1 - t0) * 1e3,
@@ -428,8 +420,7 @@ class ShardedB200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 rec = self.catalogs[r].records[pid]
                 if app_id is not None and rec.app_id is not None and rec.app_id != app_id:
                     continue
-                out.append(DocumentChunk(document_id=rec.document_id, chunk_number=rec.chunk_number, content=rec.content,
-                                         embedding=[], metadata=dict(rec.metadata), score=0.0))
+                out.append(_document_chunk(rec, 0.0))
         return out
 
     async def delete_chunks_by_document_id(self, document_id: str, app_id: Optional[str] = None) -> bool:

@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import asyncio
 import collections
+import dataclasses
 import json
 import logging
 import threading
@@ -37,6 +38,7 @@ from .catalog import PageCatalog, PageRecord
 from .models import DocumentChunk
 
 logger = logging.getLogger(__name__)
+MAX_K = 4096  # B200MS_MAX_K
 
 try:  # inside a Morphik checkout the reference ABC is the real base class
     from core.vector_store.base_vector_store import BaseVectorStore  # type: ignore
@@ -65,6 +67,19 @@ def build_store_metrics(**kw) -> Dict[str, Any]:
                 cache_write_objects=0)
     base.update(kw)
     return base
+
+
+def _document_chunk(rec: PageRecord, score) -> DocumentChunk:
+    """The DocumentChunk a search returns for a stored page (its embedding is not sent back)."""
+    return DocumentChunk(document_id=rec.document_id, chunk_number=rec.chunk_number, content=rec.content, embedding=[],
+                         metadata=dict(rec.metadata), score=float(score))
+
+
+def _capped_k(k: int) -> int:
+    """k limited to what one top-k call returns (B200MS_MAX_K), with a warning when that truncates it."""
+    if k > MAX_K:
+        logger.warning("k=%d requested; truncated to %d (B200MS_MAX_K)", k, MAX_K)
+    return min(int(k), MAX_K)
 
 
 def as_query_matrix(query_embedding) -> np.ndarray:
@@ -277,12 +292,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 recs.append(rec)
             if self._journal is not None:  # durable store: this call becomes one append-only segment
                 fde = self._two_stage.fde_rows(first, n) if self._two_stage is not None else None
-                self._journal.log_add(self._index, first, n, [self._record_json(r) for r in recs], fde)
-
-    @staticmethod
-    def _record_json(r: PageRecord) -> Dict[str, Any]:
-        return {"document_id": r.document_id, "chunk_number": r.chunk_number, "content": r.content, "metadata": r.metadata,
-                "app_id": r.app_id, "n_rows": r.n_rows}
+                self._journal.log_add(self._index, first, n, [dataclasses.asdict(r) for r in recs], fde)
 
     # ------------------------------------------------------------------ read path
     async def query_similar(self, query_embedding, k: int, doc_ids: Optional[List[str]] = None,
@@ -309,9 +319,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 else:
                     live.append((i, r, words))
             if live:
-                kk = min(max(r.k for _, r, _ in live), n, 4096)
-                if max(r.k for _, r, _ in live) > 4096:
-                    logger.warning("k > 4096 requested; truncated to 4096 (B200MS_MAX_K)")
+                kk = min(_capped_k(max(r.k for _, r, _ in live)), n)
                 queries = [r.q for _, r, _ in live]
                 masks = [w for _, _, w in live]
                 if self._two_stage is None and hasattr(self._index, "search_host_masked") and len(live) > 1:
@@ -336,9 +344,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         for j in range(count):
             if min_score is not None and float(scores[j]) < min_score:
                 break  # sorted by score descending
-            rec = self.catalog.records[int(ids[j])]
-            hits.append(DocumentChunk(document_id=rec.document_id, chunk_number=rec.chunk_number, content=rec.content,
-                                      embedding=[], metadata=dict(rec.metadata), score=float(scores[j])))
+            hits.append(_document_chunk(self.catalog.records[int(ids[j])], scores[j]))
         return hits
 
     async def query_similar_batch(self, query_embeddings: Sequence[Any], k: int, doc_ids: Optional[List[str]] = None,
@@ -364,9 +370,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             visible, words = self.catalog.allow_words(doc_ids, app_id)
             if not visible:
                 return [[] for _ in queries]
-            if k > 4096:
-                logger.warning("k=%d requested; truncated to 4096 (B200MS_MAX_K)", k)
-            kk = min(int(k), n, 4096)
+            kk = min(_capped_k(k), n)
             t1 = time.perf_counter()
             ts, ti, tc = self._search_unlocked(queries, kk, words)
             t2 = time.perf_counter()
@@ -417,10 +421,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             visible, words = self.catalog.allow_words(doc_ids, app_id)
             if not visible:
                 return []
-            if k > 4096:
-                logger.warning("k=%d requested; truncated to 4096 (B200MS_MAX_K)", k)
             n_docs = self.catalog.n_documents
-            kk = min(k, n_docs, 4096)
+            kk = min(_capped_k(k), n_docs)
             if self._page_doc_cache is None or self._page_doc_cache[0] != self.catalog.version:
                 table = torch.from_numpy(self.catalog.page_documents()).to(self._index.device)
                 self._page_doc_cache = (self.catalog.version, table)
@@ -441,6 +443,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                                skip_image_content: bool = False) -> List[DocumentChunk]:
         if not chunk_identifiers:
             return []
+        return [_document_chunk(rec, 0.0) for _, rec in self._visible_records(chunk_identifiers, app_id)]
+
+    def _visible_records(self, chunk_identifiers, app_id) -> List[Tuple[int, PageRecord]]:
+        """(page id, record) of every live chunk named, in first-mention order, duplicates collapsed, skipping chunks stored
+        under another app_id."""
         out = []
         for doc_id, chunk_num in dict.fromkeys((d, int(n)) for d, n in chunk_identifiers):
             pid = self.catalog.lookup(doc_id, chunk_num)
@@ -449,8 +456,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             rec = self.catalog.records[pid]
             if app_id is not None and rec.app_id is not None and rec.app_id != app_id:
                 continue
-            out.append(DocumentChunk(document_id=rec.document_id, chunk_number=rec.chunk_number, content=rec.content,
-                                     embedding=[], metadata=dict(rec.metadata), score=0.0))
+            out.append((pid, rec))
         return out
 
     async def explain_chunks(self, query_embedding, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
@@ -468,15 +474,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
     def _explain_locked(self, q, chunk_identifiers, app_id, with_map):
         with self._lock:
-            recs = []
-            for doc_id, chunk_num in dict.fromkeys((d, int(n)) for d, n in chunk_identifiers):
-                pid = self.catalog.lookup(doc_id, chunk_num)
-                if pid is None:
-                    continue
-                rec = self.catalog.records[pid]
-                if app_id is not None and rec.app_id is not None and rec.app_id != app_id:
-                    continue
-                recs.append((pid, rec))
+            recs = self._visible_records(chunk_identifiers, app_id)
             if not recs:
                 return []
             map_rows = max(rec.n_rows for _, rec in recs) if with_map else 0
@@ -532,12 +530,12 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             shardfile.save_index(self._index, os.path.join(directory, "corpus.b2ms"))
             with open(os.path.join(directory, "catalog.jsonl"), "w") as f:
                 for r in self.catalog.records:
-                    f.write(json.dumps(self._record_json(r)) + "\n")
+                    f.write(json.dumps(dataclasses.asdict(r)) + "\n")
             if self._journal is not None and os.path.abspath(self._journal.dir) == os.path.abspath(directory):
                 self._journal.reset()
                 if len(self.catalog):
                     fde = self._two_stage.fde_rows(0, len(self.catalog)) if self._two_stage is not None else None
-                    self._journal.log_add(self._index, 0, len(self.catalog), [self._record_json(r) for r in self.catalog.records], fde)
+                    self._journal.log_add(self._index, 0, len(self.catalog), [dataclasses.asdict(r) for r in self.catalog.records], fde)
 
     @classmethod
     def load(cls, directory: str, device: int = 0, **kw) -> "B200MultiVectorStore":
@@ -549,8 +547,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         store = cls(device=device, mode=index.dtype_name, auto_initialize=False, index=index, **kw)
         with open(os.path.join(directory, "catalog.jsonl")) as f:
             for line in f:
-                d = json.loads(line)
-                store.catalog.add(PageRecord(d["document_id"], d["chunk_number"], d["content"], d["metadata"], d["app_id"], d["n_rows"]))
+                store.catalog.add(PageRecord(**json.loads(line)))
         if len(store.catalog) != index.n_pages:
             raise ValueError("catalogue and shard file disagree on the page count")
         store.initialize()  # two-stage mode: rebuilds the FDE matrix from the packed rows; applies zero_pad_compat
@@ -580,8 +577,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 shardfile.load_index(seg, device=device, into=store._index)
                 with open(cat) as f:
                     for line in f:
-                        d = json.loads(line)
-                        store.catalog.add(PageRecord(d["document_id"], d["chunk_number"], d["content"], d["metadata"], d["app_id"], d["n_rows"]))
+                        store.catalog.add(PageRecord(**json.loads(line)))
                 if store._two_stage is not None:
                     if os.path.exists(fde):
                         blob = torch.load(fde)
