@@ -29,6 +29,12 @@
  * returns a message for the last failure on that handle (or the last global failure for NULL).
  * A handle is bound to one CUDA device and is NOT thread-safe: the caller serialises calls per handle
  * (the Python store holds a lock and calls through asyncio.to_thread, SURVEY 8b "Threading").
+ * Calls on one handle run on the GPU in the order they were made, whatever streams they name: they share the handle's
+ * scratch.  Entry points taking a `stream` enqueue on it; b200ms_search_host*, b200ms_sharded_search_host_begin,
+ * b200ms_set_corpus* and b200ms_fde_configure* enqueue on the handle's own stream.  A call on stream B therefore waits
+ * for the handle's previous call on stream A to finish on the GPU, and so does the caller's later work on B (one event
+ * wait, and one event record per call).  Calls of different handles are not ordered against each other.  A stream that is
+ * being captured into a CUDA graph is neither ordered nor recorded: capturing the device entry points is not supported.
  * Device buffers passed in are caller-owned (torch tensors); the library only owns small scratch.
  * There is no CPU fallback: without a CUDA device every compute entry point fails with B200MS_ECUDA.
  */

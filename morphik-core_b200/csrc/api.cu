@@ -164,6 +164,33 @@ DeviceGuard::~DeviceGuard() {
   if (prev >= 0 && cur != prev) cudaSetDevice(prev);
 }
 
+StreamOrder::StreamOrder(b200ms_t* h, cudaStream_t s) : h_(h), s_(s) {
+  if (h->capturing) return;
+  if (s != h->stream) {  // the handle's own stream is only ever captured inside run_host_graph (h->capturing)
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(s, &st) != cudaSuccess) {  // the legacy stream while another stream captures globally
+      cudaGetLastError();
+      return;
+    }
+    if (st != cudaStreamCaptureStatusNone) return;
+  }
+  if (h->order_pending && s != h->order_stream)
+    err_ = check_cuda(h, cudaStreamWaitEvent(s, h->order_ev, 0), "wait for the handle's previous call");
+  active_ = err_ == B200MS_OK;
+}
+
+StreamOrder::~StreamOrder() {
+  if (!active_) return;
+  if (synced_) {
+    h_->order_pending = false;
+  } else if (cudaEventRecord(h_->order_ev, s_) == cudaSuccess) {
+    h_->order_stream = s_;
+    h_->order_pending = true;
+  } else {
+    cudaGetLastError();
+  }
+}
+
 void group_tokens(const int32_t* lens, int64_t n, const int32_t* goff, int64_t n_groups, int32_t* ntok) {
   for (int64_t i = 0; i < n; ++i) {
     int64_t left = lens[i];
@@ -207,6 +234,13 @@ SearchMeta build_search_meta(const int32_t* lens, int64_t n, bool with_groups) {
 }  // namespace bms
 
 using namespace bms;
+
+// search_core of a device entry point, ordered after the handle's previous call
+static int search_ordered(b200ms_t* h, const SearchRequest& r, cudaStream_t s) {
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  return search_core(h, r, build_search_meta(r.q_lens, r.n_q), s);
+}
 
 #define B200MS_API extern "C" __attribute__((visibility("default")))
 
@@ -254,6 +288,10 @@ B200MS_API int b200ms_create(int device, b200ms_t** out) {
     delete h;
     return e;
   }
+  if (int e = check_cuda(h, cudaEventCreateWithFlags(&h->order_ev, cudaEventDisableTiming), "create: cudaEventCreate")) {
+    b200ms_destroy(h);
+    return e;
+  }
   for (int i = 0; i < b200ms_t::kEvRing; ++i) {
     if (cudaEventCreate(&h->ev0[i]) != cudaSuccess || cudaEventCreate(&h->ev1[i]) != cudaSuccess) {
       const int e = check_cuda(nullptr, cudaGetLastError(), "create: cudaEventCreate");
@@ -286,6 +324,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
     if (h->ev0[i]) cudaEventDestroy(h->ev0[i]);
     if (h->ev1[i]) cudaEventDestroy(h->ev1[i]);
   }
+  if (h->order_ev) cudaEventDestroy(h->order_ev);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return B200MS_OK;
@@ -373,6 +412,8 @@ B200MS_API int b200ms_sign_pack(b200ms_t* h, const void* x, int src_dtype, int64
   if (rows == 0) return B200MS_OK;
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   const int64_t st[2] = {0, rows};
   if (int e = upload(h, h->meta_b, st, sizeof(st), s)) return e;
   const int64_t* d = static_cast<const int64_t*>(h->meta_b.p);
@@ -386,6 +427,8 @@ B200MS_API int b200ms_hamming_batch(b200ms_t* h, const uint8_t* q_bits, const ui
       (reinterpret_cast<uintptr_t>(cand_bits) & 15))
     return set_error(h, B200MS_EINVAL, "hamming_batch: bad arguments (16-byte aligned packed rows)");
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return launch_hamming_batch(h, q_bits, cand_bits, n, out, static_cast<cudaStream_t>(stream));
 }
 
@@ -396,6 +439,8 @@ B200MS_API int b200ms_pack_pages(b200ms_t* h, const void* src, int src_dtype, co
     return set_error(h, B200MS_EINVAL, "pack_pages: bad arguments");
   if (n_pages == 0) return B200MS_OK;
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return pack_items(h, src, src_dtype, build_search_meta(page_lens, n_pages, false), false, dst, dst_dtype, i8_scale,
                     static_cast<cudaStream_t>(stream));
 }
@@ -407,6 +452,8 @@ B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, co
   if (!src_dtype_ok(src_dtype) || !corpus_dtype_ok(dst_dtype) || n_q < 0 || (n_q > 0 && (!q_lens || !q_packed)))
     return set_error(h, B200MS_EINVAL, "pack_queries: bad arguments");
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   const SearchMeta m = build_search_meta(q_lens, n_q);
   if (m.groups_padded > 0)
     if (int e = pack_items(h, q, src_dtype, m, true, q_packed, dst_dtype, i8_scale, static_cast<cudaStream_t>(stream))) return e;
@@ -421,6 +468,8 @@ B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, co
 static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages, bool host) {
   DeviceGuard g(h->device);
   cudaStream_t s = h->stream;
+  StreamOrder order(h, s);  // a call still in flight may read the tables rewritten below
+  if (int e = order.error()) return e;
   Corpus c;
   c.rows = rows;
   c.dtype = dtype;
@@ -441,6 +490,7 @@ static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t
     if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
     h->page_len_host.assign(page_lens, page_lens + n_pages);
     if (int e = check_cuda(h, cudaStreamSynchronize(s), "set_corpus_host: stream sync")) return e;
+    order.finished();
     h->corpus = c;
     h->generation++;
     return B200MS_OK;
@@ -476,6 +526,7 @@ static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t
     c.has_tmap = true;
   }
   if (int e = check_cuda(h, cudaStreamSynchronize(s), "set_corpus: stream sync")) return e;
+  order.finished();
   h->corpus = c;
   h->generation++;
   return B200MS_OK;
@@ -693,6 +744,8 @@ B200MS_API int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, con
   if (h->corpus.host) return set_error(h, B200MS_ESTATE, kHostFullScan);
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   const int32_t* ntok_dev = nullptr;
   if (h->corpus.dtype == B200MS_B1) {
     if (!q_lens || !group_offsets || n_q <= 0) return set_error(h, B200MS_EINVAL, "score: B1 needs q_lens and group_offsets");
@@ -744,6 +797,8 @@ B200MS_API int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtyp
   if (n_q == 0) return B200MS_OK;
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   if (int e = upload(h, h->meta, group_offsets, size_t(n_q + 1) * 4, s)) return e;
   return launch_topk(h, group_scores, score_dtype, n_pages, ld, static_cast<const int32_t*>(h->meta.p), n_q, allow_mask,
                      k, scale, id_base, nullptr, top_scores, top_ids, top_counts, s);
@@ -756,6 +811,8 @@ B200MS_API int b200ms_merge_topk(b200ms_t* h, const float* cand_scores, const in
       (n_q > 0 && (!cand_scores || !cand_ids || !top_scores || !top_ids || !top_counts)))
     return set_error(h, B200MS_EINVAL, "merge_topk: bad arguments (m <= 8192, k <= 4096)");
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return launch_merge_topk(h, cand_scores, cand_ids, n_q, m, k, top_scores, top_ids, top_counts,
                            static_cast<cudaStream_t>(stream));
 }
@@ -854,7 +911,7 @@ B200MS_API int b200ms_rerank_device(b200ms_t* h, const void* q_dev, int src_dtyp
   DeviceGuard g(h->device);
   SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev};
   r.cand = CandSpec{cand_ids_dev, n_cand, 0};
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
@@ -867,7 +924,7 @@ B200MS_API int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int sr
   DeviceGuard g(h->device);
   SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev};
   r.cand = cand;
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_search_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
@@ -878,7 +935,7 @@ B200MS_API int b200ms_search_device(b200ms_t* h, const void* q_dev, int src_dtyp
   DeviceGuard g(h->device);
   SearchRequest r{q_dev, src_dtype, q_lens, n_q, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev, top_counts_dev, id_base};
   r.allow = allow_mask_dev;
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
@@ -896,7 +953,7 @@ B200MS_API int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int s
     r.allow = allow_masks_dev;
     r.mask_index = mask_index_dev;
   }
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 // ---- grouping results by document
@@ -917,6 +974,8 @@ B200MS_API int b200ms_topk_docs(b200ms_t* h, const void* group_scores, int score
   if (n_q == 0) return B200MS_OK;
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   if (int e = upload(h, h->meta, group_offsets, size_t(n_q + 1) * 4, s)) return e;
   const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
   return launch_topk_docs(h, group_scores, score_dtype, n_pages, ld, static_cast<const int32_t*>(h->meta.p), n_q, allow_mask,
@@ -940,7 +999,7 @@ B200MS_API int b200ms_search_docs_device(b200ms_t* h, const void* q_dev, int src
   }
   const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
   r.docs = &d;
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 B200MS_API int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
@@ -958,7 +1017,7 @@ B200MS_API int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, i
   r.cand = cand;
   const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
   r.docs = &d;
-  return search_core(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream));
+  return search_ordered(h, r, static_cast<cudaStream_t>(stream));
 }
 
 // Small unmasked zero-copy calls repeat with the same shapes (interactive queries): the second call of a shape is captured
@@ -1050,6 +1109,8 @@ static int search_host_impl(b200ms_t* h, const float* q_host, const int32_t* q_l
     return set_error(h, B200MS_EINVAL, "search_host: bad arguments (n_q >= 1, 1 <= k <= 4096)");
   DeviceGuard g(h->device);
   cudaStream_t s = h->stream;
+  StreamOrder order(h, s);  // before the first upload, and outside the graph capture of run_host_graph
+  if (int e = order.error()) return e;
   const SearchMeta m = build_search_meta(q_lens, n_q);
   const ResultBlock rb(n_q, k);
   const size_t q_bytes = size_t(m.rows) * kDim * 4;
@@ -1094,6 +1155,7 @@ static int search_host_impl(b200ms_t* h, const float* q_host, const int32_t* q_l
   if (!zc)
     if (int e = check_cuda(h, cudaMemcpyAsync(st + out_off, out, rb.bytes(), cudaMemcpyDeviceToHost, s), "search_host: D2H results")) return e;
   if (int e = check_cuda(h, cudaStreamSynchronize(s), "search_host: stream sync")) return e;
+  order.finished();
   rb.unpack(st + out_off, top_scores_host, top_ids_host, top_counts_host);
   return B200MS_OK;
 }

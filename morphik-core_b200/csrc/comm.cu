@@ -235,6 +235,8 @@ B200MS_API int b200ms_bcast_device(b200ms_t* h, void* buf, int64_t bytes, int ro
   if (bytes < 0 || (bytes > 0 && !buf) || root < 0 || root >= c->world) return set_error(h, B200MS_EINVAL, "bcast: bad arguments");
   if (c->world == 1 || bytes == 0) return B200MS_OK;
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   h->launches++;
   return check_nccl(h, nccl_api().Broadcast(buf, buf, size_t(bytes), kNcclChar, root, c->comm, static_cast<cudaStream_t>(stream)), "ncclBroadcast");
 }
@@ -248,6 +250,8 @@ B200MS_API int b200ms_send_device(b200ms_t* h, const void* buf, int64_t bytes, i
     return set_error(h, B200MS_EINVAL, "send: bad arguments (or ncclSend unavailable)");
   if (bytes == 0) return B200MS_OK;
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   h->launches++;
   return check_nccl(h, nccl_api().Send(buf, size_t(bytes), kNcclChar, peer, c->comm, static_cast<cudaStream_t>(stream)), "ncclSend");
 }
@@ -260,6 +264,8 @@ B200MS_API int b200ms_recv_device(b200ms_t* h, void* buf, int64_t bytes, int pee
     return set_error(h, B200MS_EINVAL, "recv: bad arguments (or ncclRecv unavailable)");
   if (bytes == 0) return B200MS_OK;
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   h->launches++;
   return check_nccl(h, nccl_api().Recv(buf, size_t(bytes), kNcclChar, peer, c->comm, static_cast<cudaStream_t>(stream)), "ncclRecv");
 }
@@ -276,6 +282,8 @@ B200MS_API int b200ms_allgather_topk(b200ms_t* h, void* nccl_comm, const void* x
   ncclComm_t comm = nccl_comm ? static_cast<ncclComm_t>(nccl_comm) : c->comm;
   if (world > 1 && !comm) return set_error(h, B200MS_ESTATE, "allgather_topk: no communicator");
   if (int e = reserve(h, c->gath[0], xchg_bytes(n_q, k) * size_t(world))) return e;
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return allgather_merge(h, comm, world, xchg_local, c->gath[0].p, n_q, k, top_scores, top_ids, top_counts,
                          static_cast<cudaStream_t>(stream));
 }
@@ -342,7 +350,13 @@ B200MS_API int64_t b200ms_sharded_search_begin(b200ms_t* h, const void* q_dev, i
     r.mask_index = mask_index_dev;
   }
   int slot = 0;
-  if (int e = sharded_begin(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream), &slot)) return e;
+  {
+    // ordered on the caller's stream, where the local search runs; the merge on the communication stream reads only
+    // this slot's buffers
+    StreamOrder order(h, static_cast<cudaStream_t>(stream));
+    if (int e = order.error()) return e;
+    if (int e = sharded_begin(h, r, build_search_meta(q_lens, n_q), static_cast<cudaStream_t>(stream), &slot)) return e;
+  }
   Comm* c = h->comm;
   if (int e = check_cuda(h, cudaEventRecord(c->ev_done[slot], c->cstream), "sharded_search: record done")) return e;
   return c->ticket++;
@@ -373,6 +387,8 @@ B200MS_API int64_t b200ms_sharded_search_host_begin(b200ms_t* h, const float* q_
     return set_error(h, B200MS_ESTATE, "sharded_search_host_begin: two searches are in flight -- collect the older one with "
                                        "b200ms_sharded_search_host_end first");
   cudaStream_t s = h->stream;
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   const SearchMeta m = build_search_meta(q_lens, n_q);
   const ResultBlock rb(n_q, k);
   if (int e = reserve(h, c->q_raw[slot], size_t(m.rows > 0 ? m.rows : 1) * kDim * 4)) return e;

@@ -197,6 +197,11 @@ struct b200ms {
   int zero_copy = 1;       // host entry points: small calls read queries / write results through mapped pinned memory
   bms::Comm* comm = nullptr;
   cudaStream_t stream = nullptr;  // internal stream for *_host entry points
+  // the order of the handle's calls across streams (bms::StreamOrder): order_ev is recorded at the end of the last call
+  // that enqueued work, on order_stream; order_pending = false once that call is known to be finished
+  cudaEvent_t order_ev = nullptr;
+  cudaStream_t order_stream = nullptr;
+  bool order_pending = false;
   // ring of CUDA-event pairs bracketing the scoring kernels of the most recent b200ms_score / search calls
   static constexpr int kEvRing = 256;
   cudaEvent_t ev0[kEvRing] = {}, ev1[kEvRing] = {};
@@ -238,6 +243,27 @@ struct b200ms {
 };
 
 namespace bms {
+
+// Calls on one handle run on the GPU in the order they were made, whatever streams they name: they share the handle's
+// scratch.  Every entry point that enqueues work holds one of these, on the stream it enqueues on, for the whole call.  On
+// entry the stream waits for the handle's previous call if that call ran on another stream; on exit the handle's event is
+// recorded on the stream, or, after finished() (the call synchronised its stream), nothing is left pending.  A stream that
+// is being captured into a graph neither waits nor records: an event recorded outside a capture cannot be waited on inside.
+class StreamOrder {
+ public:
+  StreamOrder(b200ms_t* h, cudaStream_t s);
+  ~StreamOrder();
+  StreamOrder(const StreamOrder&) = delete;
+  StreamOrder& operator=(const StreamOrder&) = delete;
+  int error() const { return err_; }  // the wait could not be enqueued: the call must not enqueue anything
+  void finished() { synced_ = true; }
+
+ private:
+  b200ms_t* h_;
+  cudaStream_t s_;
+  bool active_ = false, synced_ = false;
+  int err_ = 0;
+};
 
 int set_error(b200ms_t* h, int code, const std::string& msg);
 int check_cuda(b200ms_t* h, cudaError_t e, const char* what);

@@ -528,6 +528,8 @@ B200MS_API int b200ms_fde_configure_ex(b200ms_t* h, int reps, int ksim, int proj
   }
   DeviceGuard g(h->device);
   cudaStream_t s = h->stream;
+  StreamOrder order(h, s);  // a call still in flight may read the matrices replaced below
+  if (int e = order.error()) return e;
   // a failure from here on may leave the device matrices half replaced: the handle is unconfigured until a call succeeds
   h->fde_dim = 0;
   if (int e = upload(h, h->fde_simhash, simhash, size_t(reps) * kDim * ksim * 4, s)) return e;
@@ -538,6 +540,7 @@ B200MS_API int b200ms_fde_configure_ex(b200ms_t* h, int reps, int ksim, int proj
     if (int e = upload(h, h->fde_final_sign, sg.data(), sg.size() * 4, s)) return e;
   }
   if (int e = check_cuda(h, cudaStreamSynchronize(s), "fde_configure: sync")) return e;
+  order.finished();
   h->fde_reps = reps;
   h->fde_ksim = ksim;
   h->fde_proj = proj_dim;
@@ -576,6 +579,8 @@ B200MS_API int b200ms_fde_encode(b200ms_t* h, const void* rows, int src_dtype, c
   if (n_items == 0) return B200MS_OK;
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   std::vector<int64_t> st(size_t(n_items) + 1);
   st[0] = 0;
   for (int64_t i = 0; i < n_items; ++i) st[i + 1] = st[i] + (item_lens[i] > 0 ? item_lens[i] : 0);
@@ -596,6 +601,8 @@ B200MS_API int b200ms_fde_encode_corpus(b200ms_t* h, int64_t first_page, int64_t
     return set_error(h, B200MS_EINVAL, "fde_encode_corpus: bad page range (at most 65535 pages per call)");
   if (n_pages == 0) return B200MS_OK;
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return encode_and_project(h, c.rows, B200MS_BF16, static_cast<const int64_t*>(h->page_start.p) + first_page,
                             static_cast<const int32_t*>(h->page_len.p) + first_page, n_pages, 1, out,
                             static_cast<cudaStream_t>(stream));
@@ -606,6 +613,8 @@ B200MS_API int b200ms_fde_finalize(b200ms_t* h, const float* fde, int64_t n, voi
   if (h->fde_dim == 0) return set_error(h, B200MS_ESTATE, "fde_finalize: call b200ms_fde_configure first");
   if (n < 0 || (n > 0 && (!fde || !out_rows || !inv_norm))) return set_error(h, B200MS_EINVAL, "fde_finalize: bad arguments");
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return launch_fde_finalize(h, fde, n, out_rows, inv_norm, static_cast<cudaStream_t>(stream));
 }
 
@@ -617,5 +626,7 @@ B200MS_API int b200ms_fde_scan(b200ms_t* h, const void* fde_rows, const float* i
       (reinterpret_cast<uintptr_t>(fde_rows) & 15))
     return set_error(h, B200MS_EINVAL, "fde_scan: bad arguments (rows 16-byte aligned, ld >= n_pages)");
   DeviceGuard g(h->device);
+  StreamOrder order(h, static_cast<cudaStream_t>(stream));
+  if (int e = order.error()) return e;
   return launch_fde_scan(h, fde_rows, inv_norm, n_pages, q_fde, n_q, scores, ld, static_cast<cudaStream_t>(stream));
 }

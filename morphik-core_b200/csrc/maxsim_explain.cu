@@ -374,6 +374,8 @@ B200MS_API int b200ms_explain_device(b200ms_t* h, const void* q_dev, int src_dty
   if (t_max == 0) return B200MS_OK;  // every output is empty
   DeviceGuard g(h->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
   // the queries, packed as b200ms_search_device packs them
   const SearchMeta m = build_search_meta(q_lens, n_q);
   const int64_t q_rows = m.groups_padded * kGroup;
