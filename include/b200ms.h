@@ -49,7 +49,8 @@ extern "C" {
 
 #define B200MS_VERSION 200 /* 0.2.0: + multi-GPU entry points (b200ms_comm_*, b200ms_allgather_topk, b200ms_sharded_search_*),
                               b200ms_rerank_batch_device, b200ms_fde_configure_ex, B200MS_F8 corpora, option "zero_pad_compat";
-                              options "a_in_tmem" / "split4" / "epi_w4" removed with the kernels they selected */
+                              options "a_in_tmem" / "split4" / "epi_w4" removed with the kernels they selected;
+                              + b200ms_last_scan_stats: a search with an allow mask scans only the pages the mask allows */
 
 /* element types */
 #define B200MS_F32 0  /* float32 source rows (ingest / query side only)            */
@@ -154,7 +155,13 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
  * q_packed: device [roundup(n_groups,4)*32, 128] of the corpus dtype; q_lens/group_offsets (HOST) as produced by
  * b200ms_pack_queries (B1 needs the true token counts; may be NULL for BF16/I8).
  * group_scores: device [n_groups_padded, ld] with ld >= n_pages, n_groups_padded = roundup(n_groups,4).
- * Pages with zero rows score 0 (COALESCE(...,0.0), multi_vector_store.py:308). */
+ * Pages with zero rows score 0 (COALESCE(...,0.0), multi_vector_store.py:308).
+ * b200ms_score scans every page.  The search entry points below that take an allow mask (b200ms_search_host*,
+ * b200ms_search_device*, b200ms_search_docs_device, b200ms_sharded_search_*) scan only the pages some query of the call may
+ * see: the work units of the scan are rebuilt from the masks on the device in every call (the masks may change behind the
+ * same pointer), without a synchronisation, and the results are bit for bit those of b200ms_score + b200ms_topk.  A query
+ * without a mask in the batch (mask index -1) makes the call scan every page.  Corpora whose scan is a single wave of work
+ * units keep the full scan. */
 int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* q_lens, const int32_t* group_offsets,
                  int n_q, void* group_scores, int64_t ld, void* stream);
 
@@ -374,6 +381,9 @@ float b200ms_last_score_ms(b200ms_t* h);
  * `achieved` from these: CUDA events on the launching stream, recorded inside the timed region. */
 int64_t b200ms_score_call_count(const b200ms_t* h);
 int b200ms_score_times_ms(b200ms_t* h, float* out_ms, int n);
+/* Work units and padded rows walked by the handle's last full scan (b200ms_score or a search without candidates): those of
+ * the whole corpus, or of the allowed pages when the search scanned a filtered plan; synchronises with that call. */
+int b200ms_last_scan_stats(b200ms_t* h, int64_t* units, int64_t* rows);
 /* Tuning knobs (0 keeps the default): rows per work unit, CTAs to launch. */
 int b200ms_set_tuning(b200ms_t* h, int64_t unit_rows, int max_ctas);
 /* Named options:

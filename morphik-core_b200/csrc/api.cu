@@ -315,7 +315,8 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->cand_pad, &h->cand_start, &h->cand_end, &h->cand_mask, &h->topk_keys, &h->topk_ids, &h->docs_best, &h->docs_mask, &h->docs_top, &h->docs_pick, &h->b1_q_i8, &h->b1_tok_const, &h->f8_q_f16,
                        &h->fde_simhash, &h->fde_ams_index, &h->fde_ams_sign, &h->fde_tmp, &h->fde_q_bf16, &h->fde_final_index,
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
-                       &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage};
+                       &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
+                       &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (cudaEvent_t e : h->ht_ev) cudaEventDestroy(e);
@@ -518,6 +519,7 @@ static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t
   if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
   h->page_len_host.assign(page_lens, page_lens + n_pages);
   if (int e = reserve(h, h->chunk_page, size_t(c.n_chunks > 0 ? c.n_chunks : 1) * 4)) return e;
+  if (int e = reserve_scan_plan(h, c)) return e;
   if (int e = launch_chunk_page(h, static_cast<const int64_t*>(h->page_start.p), n_pages,
                                 static_cast<int32_t*>(h->chunk_page.p), s))
     return e;
@@ -605,6 +607,14 @@ B200MS_API int b200ms_last_gather_stats(b200ms_t* h, int64_t* unique_pages, int6
   return B200MS_OK;
 }
 
+B200MS_API int b200ms_last_scan_stats(b200ms_t* h, int64_t* units, int64_t* rows) {
+  if (!h) return B200MS_EINVAL;
+  DeviceGuard g(h->device);
+  if (h->order_pending)
+    if (int e = check_cuda(h, cudaEventSynchronize(h->order_ev), "last_scan_stats: wait for the scan")) return e;
+  return read_scan_stats(h, units, rows);
+}
+
 // zero_pad_compat, full scan: pages are "batched" in page-id order, zero_pad_batch at a time (score_multi_vector's
 // batch_size, 128 upstream); a page shorter than the longest of its batch gets its per-token maxima clamped at 0.
 // Built on the host once per (corpus, batch size) and cached on the device.
@@ -682,10 +692,11 @@ static int score_wgmma_per_query(b200ms_t* h, const CorpusView& v, const UnitPla
 }
 
 // Scores the rows of v.  unit_ids: the candidate slots as page ids of v (cs.ids unless v is a staging block); fill = false
-// skips the zero-fill (a later gather round of a host-resident corpus adds its slots to the same matrix).
+// skips the zero-fill (a later gather round of a host-resident corpus adds its slots to the same matrix).  scan (full scans
+// only): the filtered plan to walk in place of the corpus' own; the scores of the pages it leaves out are not written.
 static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* goff, int n_q, const int32_t* ntok_dev,
                       void* group_scores, int64_t ld, const CandSpec& cs, cudaStream_t s, const CorpusView& v,
-                      const int64_t* unit_ids, bool fill = true) {
+                      const int64_t* unit_ids, bool fill = true, const UnitPlan* scan = nullptr) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "score: no corpus attached (call b200ms_set_corpus first)");
   const int64_t n_items = cs.ids ? cs.n_slots(n_q) : c.n_pages;
@@ -706,7 +717,8 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   if (zero_fill && fill)
     if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(groups_padded(n_groups)) * size_t(ld) * 4, s), "score: memset"))
       return e;
-  UnitPlan plan = full_scan_plan(h);
+  UnitPlan plan = scan ? *scan : full_scan_plan(h);
+  if (!cs.ids) h->scan_planned = scan != nullptr;
   if (!b1) {
     if (int e = cs.ids ? candidate_plan(h, v, unit_ids, cs, n_q, s, &plan) : ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
   }
@@ -717,14 +729,14 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
     if (int e = check_cuda(h, cudaEventRecord(h->ev0[slot], s), "score: event record")) return e;
   int e = B200MS_OK;
   if (b1_wgmma) {
-    e = launch_score_b1_wgmma(h, q_packed, ntok_dev, n_groups, group_scores, ld, s);
+    e = launch_score_b1_wgmma(h, plan, q_packed, ntok_dev, n_groups, group_scores, ld, s);
   } else if (b1 && cs.per_query) {
     for (int q = 0; q < n_q && !e; ++q)
       if (goff[q + 1] > goff[q])
         e = launch_score_b1(h, v, unit_ids + int64_t(q) * cs.stride(), cs.n_cand, q_packed, n_groups, ntok_dev,
                             static_cast<int32_t*>(group_scores) + int64_t(q) * cs.stride(), ld, s, goff[q], goff[q + 1]);
   } else if (b1) {
-    e = launch_score_b1(h, v, unit_ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups);
+    e = launch_score_b1(h, v, unit_ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups, scan);
   } else if (cs.per_query) {
     e = score_wgmma_per_query(h, v, plan, cs, q_packed, n_groups, goff, n_q, group_scores, ld, s);
   } else {
@@ -859,7 +871,17 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
       return e;
   const int ng = int(m.groups);
   if (!c.host) {
-    if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s, corpus_view(h), cs.ids)) return e;
+    // A filtered full scan reads only the pages some query of the call may see.  The other pages keep whatever h->scores
+    // held before, and that is never read: the selection below skips a page whose allow bit is clear before it touches
+    // the page's score, in the flat form (page_key) and in the document form (doc_item) alike.  A corpus whose own plan
+    // is one wave of units gains nothing from a shorter one, so it keeps it (and a small search its launch count).
+    UnitPlan filtered;
+    const bool plan_scan = !cs.ids && r.allow && ng > 0 && c.n_units > (h->max_ctas > 0 ? h->max_ctas : h->num_sms);
+    if (plan_scan)
+      if (int e = launch_scan_plan(h, r.allow, r.mask_index, n_q, s, &filtered)) return e;
+    if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s, corpus_view(h), cs.ids, true,
+                           plan_scan ? &filtered : nullptr))
+      return e;
   } else if (ng > 0 && n_items > 0) {
     struct Ctx {
       const void* q;

@@ -122,10 +122,17 @@ inline size_t xchg_bytes(int n_q, int k) { return (size_t(n_q) * size_t(k) * 12 
 
 // Which chunk ranges a scoring launch walks.  Full scan: the corpus' own unit plan, scores indexed by page id.
 // Candidate ("slot") mode: unit j = the chunk range of candidate page j, scores indexed by j.
+// Filtered full scan (launch_scan_plan): units over the allowed pages only, counted on the device; scores by page id.
 struct UnitPlan {
   const int32_t* start = nullptr;
   const int32_t* end = nullptr;
   int n_units = 0;
+  // != NULL: the unit count is this device word, written by an earlier kernel of the stream; n_units is then only an
+  // upper bound (it sizes the launch)
+  const int32_t* n_units_dev = nullptr;
+  // filtered full scan, POPC kernel (one warp per page, no units): the allowed pages in ascending order and their count
+  const int64_t* pages = nullptr;
+  const int32_t* n_pages_dev = nullptr;
   int slot_mode = 0;
   // zero_pad_compat: bit i set = page i (slot_mode: candidate slot i) is shorter than the longest page of its scoring
   // batch, so its per-token maxima are clamped at 0 like the reference's zero padding does; NULL = clean MaxSim
@@ -175,6 +182,11 @@ struct b200ms {
   bms::DeviceBuf clamp_pages;  // uint32 words: zero_pad_compat clamp bit per page (full scan), built lazily
   bms::DeviceBuf clamp_slots;  // uint32 words: clamp bit per candidate slot (rerank), rebuilt per call
   std::vector<int32_t> page_len_host;
+  // filtered full scan (scan_plan.cu), sized by set_corpus and rebuilt by every filtered search: the union of the call's
+  // masks, per full-plan unit the count and offset of its filtered units, the filtered units, and {units, pages, rows}
+  bms::DeviceBuf scan_union, scan_cnt, scan_off, scan_start, scan_end, scan_hdr;
+  bms::DeviceBuf scan_word_off, scan_pages;  // 1-bit corpora: per-word offsets into, and the list of, the allowed pages
+  bool scan_planned = false;                 // the last full scan walked a filtered plan (b200ms_last_scan_stats)
   // scratch for pack / search
   bms::DeviceBuf meta, meta_b;  // per-call metadata block of a search (one upload) / of a pack call
   bms::DeviceBuf q_raw, q_packed, scores, mask, mask_index, out_all;
@@ -320,14 +332,23 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
 int launch_score_wgmma(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const void* q_packed, int n_groups_real,
                        void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
+// scan != NULL (full scans, cand_ids == NULL): only the pages scan->pages lists, scores still indexed by page id
 int launch_score_b1(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
                     int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,
-                    int g_hi);
+                    int g_hi, const UnitPlan* scan = nullptr);
 int launch_pad_cands(b200ms_t* h, const int64_t* src, int n_cand, int n_lists, int64_t stride, int64_t* dst, cudaStream_t s);
 int launch_clamp_slots(b200ms_t* h, const int64_t* cand_ids, int n_cand, int n_lists, int64_t list_stride, int batch,
                        uint32_t* clamp_bits, cudaStream_t s);
-int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
-                          void* group_scores, int64_t ld, cudaStream_t s);
+int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
+                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s);
+// Scratch of launch_scan_plan for the corpus c (set_corpus reserves it, so that no search grows it)
+int reserve_scan_plan(b200ms_t* h, const Corpus& c);
+// Work units of a full scan that reads only the pages the call's masks allow (scan_plan.cu), built on stream s without a
+// synchronisation: allow / mask_index as in SearchRequest (allow != NULL).  *plan keeps its clamp_bits.
+int launch_scan_plan(b200ms_t* h, const uint32_t* allow, const int32_t* mask_index, int n_q, cudaStream_t s, UnitPlan* plan);
+// Full-plan units and padded rows the last full scan walked; reads the device words of a filtered plan (the caller has
+// waited for the scan)
+int read_scan_stats(b200ms_t* h, int64_t* units, int64_t* rows);
 int launch_cand_units(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int n_cand, int32_t* unit_start,
                       int32_t* unit_end, uint32_t* slot_mask, cudaStream_t s);
 int launch_hamming_batch(b200ms_t* h, const void* q, const void* cand, int64_t n, uint32_t* out, cudaStream_t s);

@@ -14,10 +14,10 @@
 //              empty units); the top-k afterwards sees the original ids, so ids, ties and zero_pad_compat are those of HBM.
 // A round holds at most host_stage_bytes of rows; W = budget - largest page + 32 rows, so a round's last page always fits.
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace bms {
 
-constexpr int kScanThreads = 1024;
 constexpr int kGatherUnroll = 4;  // independent 16-byte PCIe reads in flight per thread
 
 __device__ __forceinline__ int64_t lower_bound_i64(const int64_t* __restrict__ a, int64_t n, int64_t key) {
@@ -27,32 +27,6 @@ __device__ __forceinline__ int64_t lower_bound_i64(const int64_t* __restrict__ a
     if (a[mid] < key) lo = mid + 1; else hi = mid;
   }
   return lo;
-}
-
-// Exclusive prefix sum of val(0..n) into out[0..n] (out[n] = total) by one block of kScanThreads threads, each summing a
-// contiguous span: the order of additions is fixed, so the result is deterministic.
-template <class F>
-__device__ void block_scan(F val, int64_t n, int64_t* __restrict__ out) {
-  __shared__ int64_t part[kScanThreads];
-  const int t = threadIdx.x;
-  const int64_t per = (n + kScanThreads - 1) / kScanThreads;
-  const int64_t i0 = min(n, int64_t(t) * per), i1 = min(n, i0 + per);
-  int64_t sum = 0;
-  for (int64_t i = i0; i < i1; ++i) sum += val(i);
-  part[t] = sum;
-  __syncthreads();
-  for (int off = 1; off < kScanThreads; off <<= 1) {
-    const int64_t v = t >= off ? part[t - off] : 0;
-    __syncthreads();
-    part[t] += v;
-    __syncthreads();
-  }
-  int64_t run = part[t] - sum;
-  for (int64_t i = i0; i < i1; ++i) {
-    out[i] = run;
-    run += val(i);
-  }
-  if (t == kScanThreads - 1) out[n] = part[t];
 }
 
 __global__ void ht_mark_kernel(const int64_t* __restrict__ ids, int64_t n_slots, int64_t n_pages, uint32_t* __restrict__ bitmap) {

@@ -24,6 +24,8 @@ template <int G>
 __global__ void __launch_bounds__(kB1Warps * 32)
 maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ page_start, int64_t n_pages,
                  const int64_t* __restrict__ cand_ids /* NULL: every page; else n_pages candidates, output slot = index */,
+                 const int32_t* __restrict__ n_cand_dev /* != NULL: the candidate count, a device word (n_pages bounds it) */,
+                 int by_page /* candidates write their page's column, not their slot's (a filtered full scan) */,
                  int64_t corpus_pages /* candidate ids outside [0, corpus_pages) are unused slots */,
                  const uint4* __restrict__ q_bits /*[n_groups*32]*/, const int32_t* __restrict__ group_ntok, int g_base,
                  int n_groups, int32_t* __restrict__ group_scores, int64_t ld) {
@@ -44,6 +46,7 @@ maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ pag
     qs[g] = q[g].x ^ q[g].y ^ q[g].z;
     ntok[g] = live ? __ldg(group_ntok + gg) : 0;
   }
+  if (n_cand_dev) n_pages = __ldg(n_cand_dev);
   const int64_t warp_global = int64_t(blockIdx.x) * kB1Warps + warp;
   const int64_t warp_stride = int64_t(gridDim.x) * kB1Warps;
   for (int64_t p = warp_global; p < n_pages; p += warp_stride) {
@@ -77,15 +80,21 @@ maxsim_b1_kernel(const uint4* __restrict__ rows, const int64_t* __restrict__ pag
       if (gg >= n_groups) break;
       int v = (r1 > r0 && lane < ntok[g]) ? (128 - best[g]) : 0;  // empty page -> 0 (COALESCE)
       v = warp_sum(v);
-      if (lane == 0) group_scores[int64_t(gg) * ld + p] = v;
+      if (lane == 0 && (live_page || !by_page)) group_scores[int64_t(gg) * ld + (by_page ? pg : p)] = v;
     }
   }
 }
 
 int launch_score_b1(b200ms_t* h, const CorpusView& c, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
                     int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,
-                    int g_hi) {
-  const int64_t n_items = cand_ids ? n_cand : c.n_pages;
+                    int g_hi, const UnitPlan* scan) {
+  const int32_t* n_dev = nullptr;
+  if (scan && !cand_ids) {
+    cand_ids = scan->pages;
+    n_dev = scan->n_pages_dev;
+  }
+  const int by_page = n_dev != nullptr;
+  const int64_t n_items = cand_ids && !by_page ? n_cand : c.n_pages;
   if (n_items == 0 || n_groups == 0) return B200MS_OK;
   int64_t want = (n_items + kB1Warps - 1) / kB1Warps;
   const int64_t cap = int64_t(h->num_sms) * 8;
@@ -100,16 +109,16 @@ int launch_score_b1(b200ms_t* h, const CorpusView& c, const int64_t* cand_ids, i
   for (int base = g_lo; base < g_hi;) {
     const int rem = g_hi - base;
     if (rem >= 8) {
-      maxsim_b1_kernel<8><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<8><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, n_dev, by_page, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 8;
     } else if (rem >= 4) {
-      maxsim_b1_kernel<4><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<4><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, n_dev, by_page, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 4;
     } else if (rem >= 2) {
-      maxsim_b1_kernel<2><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<2><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, n_dev, by_page, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 2;
     } else {
-      maxsim_b1_kernel<1><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
+      maxsim_b1_kernel<1><<<grid, kB1Warps * 32, 0, s>>>(rows, ps, n_items, cand_ids, n_dev, by_page, c.n_pages, qb, group_ntok_dev, base, n_groups, out, ld);
       base += 1;
     }
     h->launches++;

@@ -142,12 +142,15 @@ __global__ void __launch_bounds__(kThreads, 1)
 maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_constant__ CUtensorMap tmap_q,
                     const uint4* __restrict__ bit_rows, int64_t n_rows, const int32_t* __restrict__ tok_const,
                     const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start,
-                    const int32_t* __restrict__ unit_end, int slot_mode, int n_units, int m_tile_base, int n_groups_real,
+                    const int32_t* __restrict__ unit_end, int slot_mode, int n_units,
+                    const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,
                     const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
                     int num_stages) {
   using K = Kind<KIND>;
   using Acc = typename K::Acc;
   static_assert(!BITS || KIND == 1, "1-bit corpora run on the int8 MMA");
+  // a filtered scan's units are counted on the device (scan_plan.cu); a CTA past the count finds no tile and falls through
+  if (n_units_dev) n_units = __ldg(n_units_dev);
   constexpr int NWG = NM >= 2 ? 2 : 1;   // consumer warpgroups with work
   constexpr int MPW = (NM + 1) / 2;      // query tiles per consumer warpgroup
 
@@ -488,11 +491,11 @@ static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, cons
   if (int e = ensure_smem(h, reinterpret_cast<const void*>(kern), int(smem), "cudaFuncSetAttribute(maxsim_wgmma)"))
     return e;
   int grid = h->max_ctas > 0 ? h->max_ctas : h->num_sms;
-  if (grid > up.n_units) grid = up.n_units;
+  if (grid > up.n_units) grid = up.n_units;  // with n_units_dev an upper bound: the count is not known here
   if (grid < 1) return B200MS_OK;
   static const CUtensorMap kNoTmap{};  // 1-bit rows: the producer expands bits and never issues TMA loads for them
   kern<<<grid, kThreads, smem, s>>>(c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
-                                   c.chunk_page, up.start, up.end, up.slot_mode, up.n_units,
+                                   c.chunk_page, up.start, up.end, up.slot_mode, up.n_units, up.n_units_dev,
                                    m_tile_base, n_groups_real, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
                                    stages);
   h->launches++;
@@ -572,8 +575,8 @@ int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, con
 
 // 1-bit full scan: the query bits become +-1 int8 rows (b1_q_i8) and per-token constants, then the int8 kernel with the
 // expanding producer.
-int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_ntok_dev, int n_groups_real,
-                          void* group_scores, int64_t ld, cudaStream_t s) {
+int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
+                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
   const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_rows = n_groups_padded * kGroup;
   if (int e = reserve(h, h->b1_q_i8, size_t(n_rows) * 128 + 1024)) return e;
@@ -585,7 +588,7 @@ int launch_score_b1_wgmma(b200ms_t* h, const void* q_bits, const int32_t* group_
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
   if (int e = query_tmap(h, q_i8, B200MS_I8, n_rows)) return e;
-  return launch_tiles<1, true>(h, corpus_view(h), full_scan_plan(h), h->tmap_q, tok_const, n_groups_real, 0,
+  return launch_tiles<1, true>(h, corpus_view(h), plan, h->tmap_q, tok_const, n_groups_real, 0,
                                n_groups_padded / 4, group_scores, ld, s);
 }
 

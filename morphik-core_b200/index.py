@@ -482,6 +482,13 @@ class MaxSimIndex:
                                                       ctypes.byref(ms)), "b200ms_last_gather_stats")
         return {"unique_pages": int(u.value), "bytes": int(b.value), "rounds": int(r.value), "ms": float(ms.value)}
 
+    def scan_stats(self) -> dict:
+        """Of the last full scan (score_groups or a search without candidates): work units and padded rows it walked -- the
+        whole corpus, or only the pages its allow masks named; synchronises with that call."""
+        u, r = ctypes.c_int64(), ctypes.c_int64()
+        self.h.check(nat.lib.b200ms_last_scan_stats(self.h.ptr, ctypes.byref(u), ctypes.byref(r)), "b200ms_last_scan_stats")
+        return {"units": int(u.value), "rows": int(r.value)}
+
     # ------------------------------------------------------------------ queries
     @staticmethod
     def _q_lens(queries: Sequence[ArrayLike]) -> List[int]:

@@ -208,6 +208,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         self.device = int(device)
         self.mode = mode
         self.storage = storage  # attribute kept for DualMultiVectorStore / DocumentService compatibility
+        # Tombstoned pages cost HBM until the compaction, but no scan time once any filter is given: the catalogue's masks
+        # clear them (PageCatalog.allow_mask starts from `alive`), and a filtered search reads only the pages its mask allows.
         self.compact_dead_fraction = float(compact_dead_fraction)
         self.catalog = PageCatalog()
         self._index = index  # injectable for host-logic tests; the product builds a MaxSimIndex in initialize()
