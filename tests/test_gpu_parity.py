@@ -447,7 +447,8 @@ def test_merge_topk_matches_oracle():
 
 # ------------------------------------------------------------------------------------------------ size-independent properties
 def test_properties_at_scale_bf16():
-    """At a size the oracle cannot sweep in seconds (16k pages x 1024 patches, 4 GiB bf16), check invariants of MaxSim."""
+    """16k pages x 1024 patches (4 GiB bf16): invariants of MaxSim.  Every page of larger corpora is compared with a float64
+    reference in tests/test_gpu_scale.py."""
     n_pages, p = 16384, 1024
     g = torch.Generator(device="cuda").manual_seed(1234)
     rows = torch.randn((n_pages * p, 128), generator=g, device="cuda", dtype=torch.float32)
@@ -469,11 +470,6 @@ def test_properties_at_scale_bf16():
     s = idx.score_matrix([qn])[0]
     assert s.argmax() == 777 and abs(s[777] - 32.0) < 0.05
     assert s[9000] == s[5] and s[43] == s[42]
-    # oracle on a bounded sample of pages (every 512th + the special ones)
-    sample = sorted(set(range(0, n_pages, 512)) | {5, 42, 43, 777, 9000})
-    rows_h = torch.stack([rows[i * p:(i + 1) * p].float().cpu() for i in sample]).numpy().reshape(-1, 128)
-    want = orc.float_maxsim_c(orc.bf16_round_np(qn), rows_h, orc.page_offsets([p] * len(sample)))
-    assert_close_rel(s[sample], want, 2e-5)
     # linearity in the query scale: scoring 2q doubles every score exactly (power-of-two scaling is exact in bf16/fp32)
     s2 = idx.score_matrix([2.0 * qn])[0]
     assert np.array_equal(s2, 2.0 * s)
@@ -524,8 +520,9 @@ def test_sliced_topk_is_exact_with_ties_and_large_ints(dtype):
 
 @pytest.mark.parametrize("dtype", ["int8", "binary"])
 def test_properties_at_scale_int8_binary(dtype):
-    """16384 pages x 1024 patches (int8 2 GiB / 1-bit 256 MiB): invariants + oracle on a sample, single query and a batch
-    (the batch takes the tensor-core 1-bit path and the sliced top-k)."""
+    """16384 pages x 1024 patches (int8 2 GiB / 1-bit 256 MiB): invariants, single query and a batch (the batch takes the
+    tensor-core 1-bit path and the sliced top-k).  Every page of larger corpora is compared with a float64 reference in
+    tests/test_gpu_scale.py."""
     n_pages, p = 16384, 1024
     g = torch.Generator(device="cuda").manual_seed(99)
     rows = torch.nn.functional.normalize(torch.randn((n_pages * p, 128), generator=g, device="cuda"), dim=1)
@@ -545,15 +542,6 @@ def test_properties_at_scale_int8_binary(dtype):
     assert s1.argmax() == 4242 and s1[9000] == s1[5] and s1[43] == s1[42]
     if dtype == "binary":
         assert s1[4242] == 32.0  # every token finds itself: Hamming 0
-    sample = sorted(set(range(0, n_pages, 1024)) | {5, 42, 43, 4242, 9000})
-    rows_h = torch.stack([rows[i * p:(i + 1) * p].cpu() for i in sample]).numpy().reshape(-1, 128)
-    off = orc.page_offsets([p] * len(sample))
-    if dtype == "binary":
-        want = orc.binary_maxsim_c(orc.sign_pack_c(qn), orc.sign_pack_c(rows_h), off)[0]
-        assert np.array_equal(s1[sample], want)
-    else:
-        want = orc.int8_maxsim_c(orc.quantize_int8_np(qn, 127.0), orc.quantize_int8_np(rows_h, 127.0), off)
-        assert np.array_equal(np.rint(s1[sample] * 127.0 * 127.0).astype(np.int64), want)
     ts, ti, tc = idx.search_host([qn] + others, k=10)
     for qi in range(8):
         _, oi = orc.topk_np(sb[qi], 10)
