@@ -35,7 +35,7 @@
  * for the handle's previous call on stream A to finish on the GPU, and so does the caller's later work on B (one event
  * wait, and one event record per call).  Calls of different handles are not ordered against each other.  A stream that is
  * being captured into a CUDA graph is neither ordered nor recorded: capturing the device entry points is not supported.
- * Device buffers passed in are caller-owned (torch tensors); the library only owns small scratch.
+ * Device buffers passed in are caller-owned (torch tensors); the library only owns small scratch and the blocks of the "corpus storage" section.
  * There is no CPU fallback: without a CUDA device every compute entry point fails with B200MS_ECUDA.
  */
 #ifndef B200MS_H_
@@ -141,6 +141,42 @@ int b200ms_host_free(b200ms_t* h, void* p);
 int b200ms_last_gather_stats(b200ms_t* h, int64_t* unique_pages, int64_t* bytes, int* rounds, float* ms);
 int64_t b200ms_corpus_pages(const b200ms_t* h);
 int64_t b200ms_corpus_rows(const b200ms_t* h);
+
+/* ---- corpus storage: a device buffer that grows without a copy, and compaction in place ------------------------------------
+ * Replaces what the reference's stores give for free (Postgres rows and .npy objects take INSERT and DELETE ... WHERE
+ * document_id at any fill level, multi_vector_store.py:681-703, :929-933): a live corpus in a cudaMalloc'd buffer needs a
+ * second buffer to grow or to drop deleted pages, so it could use less than half of the card.
+ *
+ * A block is a reserved range of device virtual addresses, owned by the library and backed by physical memory in chunks of
+ * B200MS_BLOCK_CHUNK_BYTES (a multiple of the device's allocation granularity; there is no option for it).  Its pointer is
+ * ordinary device memory for every entry point here (b200ms_pack_pages, b200ms_set_corpus, the FDE calls) and for torch.
+ *   block_create:  reserve max_bytes of address space (no physical memory yet).  The base address is 1024-byte aligned.
+ *   block_resize:  make exactly the first roundup(bytes, chunk) bytes of the range backed: maps new chunks behind the mapped
+ *     ones, or unmaps chunks from the tail and RELEASES them to the driver.  Bytes that stay mapped keep their contents and
+ *     their address.  Ordered like every other call of the handle: a shrink waits for the handle's earlier work before it
+ *     unmaps (work the caller enqueued on the range by other means is the caller's to wait for).  Growing compares the bytes
+ *     it has to add with cudaMemGetInfo first and returns B200MS_ENOMEM without creating anything when they do not fit; a
+ *     chunk that cannot be created all the same gives the same code.  Either way the block is left as it was.
+ *   block_ptr / block_mapped_bytes: the base address (constant for the block's life) and the backed bytes; NULL -> NULL / 0.
+ *   block_destroy: waits like a shrink, releases everything.  b200ms_destroy releases the blocks the caller forgot.
+ * B200MS_EINVAL: a NULL handle, out or block, a negative size, bytes > max_bytes, a block of another handle.
+ *
+ * compact_rows: move n_runs runs of rows down so that they become contiguous from row 0, in order, inside one buffer:
+ *   run i = rows [run_start[i], run_start[i] + run_rows[i]), run_start ascending, runs disjoint (HOST arrays, checked; a run
+ *   may be empty).  row_bytes is a multiple of 16 (at most 64 MiB), rows 16-byte aligned.  Source and destination overlap; the
+ *   result is byte for byte what copying the runs into a second buffer gives, and rows past the last moved row keep whatever
+ *   they held.  Asynchronous on cuda_stream; the only scratch is a library-owned bounce buffer of 64 MiB (allocated by the
+ *   first call that needs it), never a second copy of the data: the destination is walked in ascending windows, a window whose
+ *   sources all lie past its end is gathered directly, the others go through the bounce buffer. */
+#define B200MS_BLOCK_CHUNK_BYTES (32 << 20)
+typedef struct b200ms_block b200ms_block_t;
+int b200ms_block_create(b200ms_t* h, int64_t max_bytes, b200ms_block_t** out);
+int b200ms_block_resize(b200ms_t* h, b200ms_block_t* b, int64_t bytes);
+void* b200ms_block_ptr(const b200ms_block_t* b);
+int64_t b200ms_block_mapped_bytes(const b200ms_block_t* b);
+int b200ms_block_destroy(b200ms_t* h, b200ms_block_t* b);
+int b200ms_compact_rows(b200ms_t* h, void* rows, int64_t row_bytes, const int64_t* run_start, const int64_t* run_rows,
+                        int64_t n_runs, void* cuda_stream);
 
 /* Pack n_q queries stored back to back at q (device, [sum len,128] F32|BF16) into 32-row groups of the
  * corpus dtype at q_packed (device, capacity >= roundup(groups,4)*32 rows; tail rows are zeroed).

@@ -108,6 +108,12 @@ _SIGNATURES = {
     "b200ms_host_alloc": (c_int, [vp, c_int64, POINTER(c_void_p)]),
     "b200ms_host_free": (c_int, [vp, vp]),
     "b200ms_last_gather_stats": (c_int, [vp, i64p, i64p, POINTER(c_int), f32p]),
+    "b200ms_block_create": (c_int, [vp, c_int64, POINTER(c_void_p)]),
+    "b200ms_block_resize": (c_int, [vp, vp, c_int64]),
+    "b200ms_block_ptr": (c_void_p, [vp]),
+    "b200ms_block_mapped_bytes": (c_int64, [vp]),
+    "b200ms_block_destroy": (c_int, [vp, vp]),
+    "b200ms_compact_rows": (c_int, [vp, vp, c_int64, i64p, i64p, c_int64, vp]),
     "b200ms_last_scan_stats": (c_int, [vp, i64p, i64p]),
     "b200ms_explain_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, c_float, vp, vp, vp, c_int64, vp]),
     "b200ms_topk_docs": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, vp, c_int64, c_int, c_int, c_float, c_int64,

@@ -316,9 +316,11 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->fde_simhash, &h->fde_ams_index, &h->fde_ams_sign, &h->fde_tmp, &h->fde_q_bf16, &h->fde_final_index,
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
-                       &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages};
+                       &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
+                       &h->compact_meta, &h->compact_bounce};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
+  release_blocks(h);
   for (cudaEvent_t e : h->ht_ev) cudaEventDestroy(e);
   if (h->stage.p) cudaFreeHost(h->stage.p);
   for (int i = 0; i < b200ms_t::kEvRing; ++i) {

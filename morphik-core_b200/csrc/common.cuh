@@ -252,6 +252,10 @@ struct b200ms {
   std::vector<cudaEvent_t> ht_ev;    // event pairs around each round's gather (last call)
   int64_t ht_unique = 0, ht_bytes = 0;
   int ht_rounds = 0;
+  // corpus storage: the growable blocks created on this handle (block.cu), and b200ms_compact_rows' run tables and bounce
+  // buffer (compact.cu)
+  std::vector<b200ms_block_t*> blocks;
+  bms::DeviceBuf compact_meta, compact_bounce;
 };
 
 namespace bms {
@@ -288,6 +292,7 @@ int ensure_smem(b200ms_t* h, const void* kernel, int smem, const char* what);
 int make_tmap_rows(b200ms_t* h, CUtensorMap* out, const void* base, int dtype, int64_t n_rows, int box_rows,
                    int64_t row_bytes = 0);
 void comm_teardown(b200ms_t* h);
+void release_blocks(b200ms_t* h);  // block.cu: unmap, release and free every block still alive on the handle
 // pack -> score -> top-k of r on stream s (api.cu); m = build_search_meta(r.q_lens, r.n_q).  meta_dev != NULL: m's block
 // already sits in device-readable memory at this address (mapped pinned staging) -- no upload; else ONE cudaMemcpyAsync.
 int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev = nullptr);

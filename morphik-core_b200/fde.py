@@ -37,7 +37,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .index import MaxSimIndex, _check_device_masks, _host_mask_to_device, _topk_outputs, _vp
+from .index import DeviceBlock, MaxSimIndex, _check_device_masks, _host_mask_to_device, _runs, _topk_outputs, _vp
 
 
 @dataclass(frozen=True)
@@ -206,6 +206,7 @@ class TwoStageIndex:
         configure_handle(self.index, self.cfg, matrices)
         self.device = self.index.device
         self.fde_dim = self.cfg.fde_dimension
+        self._Fblock: Optional[DeviceBlock] = None  # owner of the memory self._F views
         self._F: Optional[torch.Tensor] = None  # bf16 [cap, fde_dim]
         self._inv: Optional[torch.Tensor] = None  # float32 [cap]
         self._n = 0
@@ -219,13 +220,25 @@ class TwoStageIndex:
         cap = 0 if self._F is None else self._F.shape[0]
         if need <= cap:
             return
-        new_cap = max(need, int(cap * 1.5), 256)
-        F = torch.empty((new_cap, self.fde_dim), dtype=torch.bfloat16, device=self.device)
-        inv = torch.empty((new_cap,), dtype=torch.float32, device=self.device)
-        if self._n:
-            F[: self._n].copy_(self._F[: self._n])
-            inv[: self._n].copy_(self._inv[: self._n])
-        self._F, self._inv = F, inv
+        self._resize(need)
+
+    def _resize(self, rows: int) -> None:
+        """Back `rows` FDE rows (rounded up to whole chunks) of the matrix's block -- no copy of the matrix, as for the
+        patch rows (MaxSimIndex._resize_block); _F is a view of the block.  The inverse norms (4 bytes per page) are a
+        torch tensor of the same capacity and are copied."""
+        if self._Fblock is None:
+            self._Fblock = DeviceBlock(self.index.h, self.device)
+        self._Fblock.resize(rows * 2 * self.fde_dim)
+        if self._Fblock.tensor is None:
+            self._F = self._inv = None
+            return
+        cap = self._Fblock.tensor.numel() // (2 * self.fde_dim)
+        self._F = self._Fblock.tensor[: cap * 2 * self.fde_dim].view(torch.bfloat16).view(cap, self.fde_dim)
+        inv = torch.empty((cap,), dtype=torch.float32, device=self.device)
+        if self._inv is not None:
+            n = min(self._n, cap)
+            inv[:n].copy_(self._inv[:n])
+        self._inv = inv
 
     def add_pages(self, pages: Sequence) -> Tuple[int, int]:
         first, n = self.index.add_pages(pages)
@@ -311,12 +324,24 @@ class TwoStageIndex:
         return scores
 
     def compact(self, keep: Sequence[int]) -> None:
-        """Keep only pages `keep` (ascending old ids) in both the patch corpus and the FDE matrix."""
-        keep_t = torch.as_tensor([int(p) for p in keep], dtype=torch.int64, device=self.device)
+        """Keep only pages `keep` (ascending old ids) in both the patch corpus and the FDE matrix, each in place."""
+        keep = [int(p) for p in keep]
         self.index.compact(keep)
-        if self._F is not None and len(keep):
-            self._F = self._F[: self._n].index_select(0, keep_t).contiguous()
-            self._inv = self._inv[: self._n].index_select(0, keep_t).contiguous()
+        if self._F is not None:
+            runs = list(_runs(keep))
+            run_start = np.array([a for a, _ in runs], dtype=np.int64)
+            run_rows = np.array([b - a + 1 for a, b in runs], dtype=np.int64)
+            keep_t = torch.as_tensor(keep, dtype=torch.int64, device=self.device)
+            self._inv[: len(keep)] = self._inv.index_select(0, keep_t)
+            with torch.cuda.device(self.device):
+                self.index.h.check(
+                    nat.lib.b200ms_compact_rows(self.index.h.ptr, _vp(self._F), 2 * self.fde_dim,
+                                                run_start.ctypes.data_as(nat.i64p), run_rows.ctypes.data_as(nat.i64p),
+                                                len(runs), self.index._stream()),
+                    "b200ms_compact_rows")
+            self._n = len(keep)
+            torch.cuda.current_stream(self.device).synchronize()  # as MaxSimIndex.compact: torch's own copies into _F
+            self._resize(len(keep))
         self._n = len(keep)
 
     def _fde_topk(self, q_fde: torch.Tensor, kc: int, mask: Optional[torch.Tensor]):

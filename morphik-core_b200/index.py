@@ -161,6 +161,50 @@ class HostBlock:
             pass
 
 
+class _CudaBytes:
+    """`nbytes` device bytes at `ptr` as an object torch.as_tensor accepts; it owns nothing."""
+
+    def __init__(self, ptr: int, nbytes: int):
+        self.__cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1", "data": (int(ptr), False), "version": 2}
+
+
+class DeviceBlock:
+    """Growable HBM block (b200ms_block_*): address space for the whole card is reserved once, and ``resize`` backs exactly
+    as much of it as asked (in chunks of 32 MiB), so a corpus grows without a copy or a second buffer and shrinks by handing
+    memory back to the driver; the address never changes.  The memory lives outside torch's allocator.
+
+    ``tensor`` is a uint8 device view of the backed bytes (None while nothing is backed), made anew by every ``resize``:
+    views taken from it must not outlive the block, nor a shrink that cuts them off."""
+
+    def __init__(self, handle: "nat.Handle", device: torch.device):
+        p = ctypes.c_void_p()
+        total = torch.cuda.get_device_properties(device).total_memory
+        handle.check(nat.lib.b200ms_block_create(handle.ptr, int(total), ctypes.byref(p)), "b200ms_block_create")
+        self.handle, self.device, self.ptr = handle, device, p
+        self.tensor: Optional[torch.Tensor] = None
+
+    def resize(self, nbytes: int):
+        self.tensor = None
+        try:
+            self.handle.check(nat.lib.b200ms_block_resize(self.handle.ptr, self.ptr, int(nbytes)), "b200ms_block_resize")
+        finally:  # a refused resize leaves the block as it was
+            mapped = int(nat.lib.b200ms_block_mapped_bytes(self.ptr))
+            if mapped:
+                self.tensor = torch.as_tensor(_CudaBytes(nat.lib.b200ms_block_ptr(self.ptr), mapped), device=self.device)
+
+    def free(self):
+        self.tensor = None
+        if self.ptr and self.handle.ptr:  # a closed handle has released its blocks already
+            nat.lib.b200ms_block_destroy(self.handle.ptr, self.ptr)
+        self.ptr = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 class MaxSimIndex:
     """Packed corpus of pages (each a [P_i, 128] matrix of patch embeddings) on one GPU.
 
@@ -172,6 +216,10 @@ class MaxSimIndex:
     pages over PCIe into an HBM staging block, with scores bit-identical to the HBM tier); the ``search_*`` full scans
     raise ``NativeError``.  Growing the block allocates a new one and copies, so it briefly needs twice the corpus in
     pinned memory; ``capacity_rows`` sizes the block once up front and avoids that.
+
+    ``tier="hbm"`` keeps the rows in a ``DeviceBlock``: growing backs more of the block (no copy, no second buffer),
+    ``compact`` moves the surviving rows down in place and returns the freed tail to the driver, so a corpus that is
+    ingested into and deleted from can fill the card.  ``capacity_rows`` / ``reserve_rows`` only back the memory early.
     """
 
     def __init__(self, device: int = 0, dtype: str = "bf16", i8_scale: float = 127.0, capacity_rows: int = 0,
@@ -183,7 +231,9 @@ class MaxSimIndex:
         if not torch.cuda.is_available():
             raise nat.NativeError("MaxSimIndex needs a CUDA device (H100); there is no CPU fallback")
         self.tier = tier
-        self._block: Optional[HostBlock] = None  # host tier: owner of the memory self._buf views
+        # owner of the memory self._buf views: a HostBlock (host tier) or a DeviceBlock; None while an HBM index is empty
+        # or uses a caller's tensor (adopt_packed)
+        self._block: Union[HostBlock, DeviceBlock, None] = None
         self.device = torch.device("cuda", int(device))
         self.dtype = nat.DTYPE_NAMES[dtype]
         self.dtype_name = dtype
@@ -260,27 +310,45 @@ class MaxSimIndex:
     def _grow(self, need_rows: int, exact: bool = False):
         if need_rows <= self._cap_rows:
             return
+        if self.tier == "hbm":
+            self._resize_block(need_rows)
+            return
         new_cap = need_rows if exact else max(need_rows, int(self._cap_rows * 1.5), 4096)
-        if self.tier == "host":
-            self._host_barrier()
-            block = HostBlock(self.h, new_cap * self.row_bytes)
-            new_buf = block.tensor
-        else:
-            new_buf = _aligned_bytes(new_cap * self.row_bytes, self.device)
+        self._host_barrier()
+        block = HostBlock(self.h, new_cap * self.row_bytes)
+        new_buf = block.tensor
         if self._buf is not None and self._rows:
             new_buf[: self._rows * self.row_bytes].copy_(self._buf[: self._rows * self.row_bytes])
-        if self.tier == "host":
-            if self._block is not None:
-                self._buf = None
-                self._block.free()
-            self._block = block
+        if self._block is not None:
+            self._buf = None
+            self._block.free()
+        self._block = block
         self._buf = new_buf
         self._cap_rows = new_cap
         self._attached = False
 
+    def _resize_block(self, rows: int):
+        """HBM tier: back exactly `rows` rows (rounded up to whole chunks) of the index's block; the rows that stay keep
+        their contents and address.  Rows held in a caller's tensor (``adopt_packed``) move into a block of their own
+        first, which is the one copy such a corpus ever makes."""
+        block = self._block
+        if block is None:
+            block = DeviceBlock(self.h, self.device)
+        try:
+            block.resize(rows * self.row_bytes)
+        except Exception:
+            if self._block is None:
+                block.free()
+            raise
+        if self._block is None and self._buf is not None and self._rows:
+            block.tensor[: self._rows * self.row_bytes].copy_(self._buf[: self._rows * self.row_bytes])
+        self._block, self._buf = block, block.tensor
+        self._cap_rows = 0 if self._buf is None else self._buf.numel() // self.row_bytes
+        self._attached = False
+
     def reserve_rows(self, rows: int):
         """Make room for `rows` padded rows in total with one allocation of exactly that size (host tier: avoids the
-        transient second copy that growth needs)."""
+        transient second copy that growth needs; HBM tier: backs the block's memory now instead of as the pages arrive)."""
         self._grow(int(rows), exact=True)
 
     def _host_barrier(self):
@@ -330,8 +398,9 @@ class MaxSimIndex:
         self._grow(self._rows + add_rows)
         o = self._rows * self.row_bytes
         # host tier: pack on the GPU into a device temporary, then one D2H copy into the block
-        dst = self._buf[o:] if self.tier == "hbm" else torch.empty(max(add_rows * self.row_bytes, 1), dtype=torch.uint8,
-                                                                     device=self.device)
+        # (an HBM index none of whose pages has a row owns no memory yet: the call then needs a destination all the same)
+        dst = self._buf[o:] if self.tier == "hbm" and self._buf is not None else torch.empty(
+            max(add_rows * self.row_bytes, 1), dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
             self.h.check(
                 nat.lib.b200ms_pack_pages(self.h.ptr, _vp(src), src_dtype, lens_c, len(lens), _vp(dst), self.dtype,
@@ -393,6 +462,10 @@ class MaxSimIndex:
         need = int(nat.lib.b200ms_padded_rows(lens_c, len(lens)))
         if buf.numel() < need * self.row_bytes:
             raise ValueError("packed buffer smaller than the page lengths imply")
+        if self._block is not None:  # the index's own block goes; work queued on its rows must be over first
+            torch.cuda.synchronize(self.device)
+            self._block.free()
+            self._block = None
         self._buf, self._cap_rows, self._rows = buf, buf.numel() // self.row_bytes, need
         self._page_lens = lens
         self._attached = False
@@ -408,7 +481,8 @@ class MaxSimIndex:
         first = self.n_pages
         self._grow(self._rows + need)
         self._host_barrier()
-        self._buf[self._rows * self.row_bytes:(self._rows + need) * self.row_bytes].copy_(flat[: need * self.row_bytes])
+        if need:
+            self._buf[self._rows * self.row_bytes:(self._rows + need) * self.row_bytes].copy_(flat[: need * self.row_bytes])
         self._rows += need
         self._page_lens.extend(lens)
         self._attached = False
@@ -441,29 +515,38 @@ class MaxSimIndex:
         self._attached = False
 
     def compact(self, keep: Sequence[int]):
-        """Keep only the pages in `keep` (ascending old ids), renumbering them 0..len(keep)-1: device-to-device copies of
-        the surviving page runs into a fresh buffer (DELETE ... WHERE document_id, multi_vector_store.py:929-933)."""
+        """Keep only the pages in `keep` (ascending old ids), renumbering them 0..len(keep)-1, in place (DELETE ... WHERE
+        document_id, multi_vector_store.py:929-933): the maximal runs of consecutive surviving pages move down inside the
+        buffer -- on the GPU with one b200ms_compact_rows call, after which the block's freed tail goes back to the driver;
+        on the host tier with one forward (overlap-safe) memmove per run."""
         keep = [int(p) for p in keep]
         lens = self._page_lens
         pad = _padded_lens(lens)
         starts = np.concatenate([[0], np.cumsum(pad)]).astype(np.int64)
         new_rows = int(pad[keep].sum())
-        if self.tier == "host":  # in place: surviving runs move down with forward (overlap-safe) host copies
+        runs = [(int(starts[first]), int(starts[last + 1])) for first, last in _runs(keep)]  # row ranges [a, b)
+        if self.tier == "host":
             self._host_barrier()
-            base = self._buf.data_ptr()
-        else:
-            new_buf = _aligned_bytes(max(new_rows, 4096) * self.row_bytes, self.device)
-        dst = 0
-        for first, last in _runs(keep):  # one copy per maximal run of consecutive surviving pages
-            a, b = int(starts[first]) * self.row_bytes, int(starts[last + 1]) * self.row_bytes
-            if self.tier == "host":
-                if dst != a:
-                    ctypes.memmove(base + dst, base + a, b - a)
-            else:
-                new_buf[dst:dst + (b - a)].copy_(self._buf[a:b])
-            dst += b - a
-        if self.tier == "hbm":
-            self._buf, self._cap_rows = new_buf, new_buf.numel() // self.row_bytes
+            base, dst = self._buf.data_ptr(), 0
+            for a, b in runs:
+                if dst != a * self.row_bytes:
+                    ctypes.memmove(base + dst, base + a * self.row_bytes, (b - a) * self.row_bytes)
+                dst += (b - a) * self.row_bytes
+        elif self._buf is not None:
+            if self._block is None:  # a caller's tensor (adopt_packed) is not compacted behind the caller's back
+                self._resize_block(self._rows)
+            run_start = np.array([a for a, _ in runs], dtype=np.int64)
+            run_rows = np.array([b - a for a, b in runs], dtype=np.int64)
+            with torch.cuda.device(self.device):
+                self.h.check(
+                    nat.lib.b200ms_compact_rows(self.h.ptr, _vp(self._buf), self.row_bytes,
+                                                run_start.ctypes.data_as(nat.i64p), run_rows.ctypes.data_as(nat.i64p),
+                                                len(runs), self._stream()),
+                    "b200ms_compact_rows")
+            # the shrink unmaps the freed tail once the handle's calls are over; copies torch itself queued on those rows
+            # (append_packed) are only known to this stream
+            torch.cuda.current_stream(self.device).synchronize()
+            self._resize_block(new_rows)
         self._rows = new_rows
         self._page_lens = [lens[p] for p in keep]
         self._attached = False
