@@ -75,8 +75,14 @@ b1_query_expand_kernel(const uint8_t* __restrict__ q_bits /*[rows,16]*/, const i
 }
 
 // ------------------------------------------------------------------ tile iterator shared by all warp roles
+// units u, u + step, u + 2 step, ... (start: the CTA's first unit and the stride of the launch, see maxsim_wgmma_kernel)
 struct TileIter {
-  int u, t, n_tiles, c0, c1;
+  int u, step, t, n_tiles, c0, c1;
+  __device__ __forceinline__ void start(int splits, const int32_t* us, const int32_t* ue, int n_units) {
+    u = blockIdx.x / splits;
+    step = gridDim.x / splits;
+    load(us, ue, n_units);
+  }
   __device__ __forceinline__ void load(const int32_t* us, const int32_t* ue, int n_units) {
     n_tiles = 0;
     while (u < n_units) {
@@ -84,14 +90,14 @@ struct TileIter {
       c1 = __ldg(ue + u);
       n_tiles = (c1 - c0 + 3) >> 2;
       if (n_tiles > 0) break;
-      u += gridDim.x;
+      u += step;
     }
     t = 0;
   }
   __device__ __forceinline__ bool valid(int n_units) const { return u < n_units; }
   __device__ __forceinline__ void next(const int32_t* us, const int32_t* ue, int n_units) {
     if (++t == n_tiles) {
-      u += gridDim.x;
+      u += step;
       load(us, ue, n_units);
     }
   }
@@ -145,12 +151,14 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
                     const int32_t* __restrict__ unit_end, int slot_mode, int n_units,
                     const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,
                     const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
-                    int num_stages) {
+                    int num_stages, int splits) {
   using K = Kind<KIND>;
   using Acc = typename K::Acc;
   static_assert(!BITS || KIND == 1, "1-bit corpora run on the int8 MMA");
   // a filtered scan's units are counted on the device (scan_plan.cu); a CTA past the count finds no tile and falls through
   if (n_units_dev) n_units = __ldg(n_units_dev);
+  // splits = 2: CTAs 2k and 2k + 1 walk the same units, CTA 2k + 1 with the NM query tiles after CTA 2k's (see launch_one)
+  m_tile_base += NM * int(blockIdx.x % splits);
   constexpr int NWG = NM >= 2 ? 2 : 1;   // consumer warpgroups with work
   constexpr int MPW = (NM + 1) / 2;      // query tiles per consumer warpgroup
 
@@ -196,12 +204,12 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
     }
     if constexpr (!kExpand) {
       if (threadIdx.x == 0) {
-        const uint64_t pol_rows = policy_evict_first();
+        // a patch tile read by both CTAs of a split pair stays in L2 for the second read
+        const uint64_t pol_rows = splits > 1 ? policy_evict_normal() : policy_evict_first();
         int stage = 0;
         uint32_t phase = 0;
         TileIter it;
-        it.u = blockIdx.x;
-        it.load(unit_start, unit_end, n_units);
+        it.start(splits, unit_start, unit_end, n_units);
         for (; it.valid(n_units); it.next(unit_start, unit_end, n_units)) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], K::kTileBytes);
@@ -223,8 +231,7 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
       const uint32_t sw = uint32_t(r & 7);
       const uint4* rows16 = reinterpret_cast<const uint4*>(bit_rows);  // [n_rows, 8] x 16 B
       TileIter cur, pf;
-      cur.u = blockIdx.x;
-      cur.load(unit_start, unit_end, n_units);
+      cur.start(splits, unit_start, unit_end, n_units);
       pf = cur;
       uint4 nxt[8];
       auto fetch = [&](uint4 (&v)[8]) {
@@ -273,8 +280,7 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
       const uint32_t row_off = uint32_t(r >> 3) * 1024u + uint32_t(r & 7) * 128u;
       const uint32_t sw = uint32_t(r & 7);
       TileIter cur, pf;
-      cur.u = blockIdx.x;
-      cur.load(unit_start, unit_end, n_units);
+      cur.start(splits, unit_start, unit_end, n_units);
       pf = cur;
       constexpr int kRing = 8;
       uint4 ring[kRing];
@@ -388,8 +394,7 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
   int pg[4];          // page of each chunk of the tile; -1: past the end of the unit
   bool same = false;  // all four chunks continue cur_page (the common case)
   TileIter it;
-  it.u = blockIdx.x;
-  it.load(unit_start, unit_end, n_units);
+  it.start(splits, unit_start, unit_end, n_units);
   auto begin_tile = [&]() {
     if (it.u != last_u) {  // new unit: units end on page boundaries
 #pragma unroll
@@ -478,9 +483,12 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
 }
 
 // ---------------------------------------------------------------------------------------------- host side
+// Query tiles [m_tile_base, m_tile_base + splits * NM) in one launch.  splits = 2: CTAs 2k and 2k + 1 walk the same units,
+// CTA 2k with the first NM tiles and CTA 2k + 1 with the next NM, so the pair reads every patch tile from HBM once and
+// the second read hits L2 -- two back-to-back passes over the corpus would read it from HBM twice.
 template <int KIND, int NM, bool BITS>
 static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
-                      int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s) {
+                      int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s, int splits = 1) {
   using K = Kind<KIND>;
   const uint32_t avail = kSmemLimit - 1024 /*align*/ - kBarrierBytes - NM * K::kTileBytes;
   int stages = int(avail / K::kTileBytes);
@@ -491,25 +499,33 @@ static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, cons
   if (int e = ensure_smem(h, reinterpret_cast<const void*>(kern), int(smem), "cudaFuncSetAttribute(maxsim_wgmma)"))
     return e;
   int grid = h->max_ctas > 0 ? h->max_ctas : h->num_sms;
-  if (grid > up.n_units) grid = up.n_units;  // with n_units_dev an upper bound: the count is not known here
+  if (grid > splits * up.n_units) grid = splits * up.n_units;  // with n_units_dev an upper bound: the count is not known here
+  grid -= grid % splits;
   if (grid < 1) return B200MS_OK;
   static const CUtensorMap kNoTmap{};  // 1-bit rows: the producer expands bits and never issues TMA loads for them
   kern<<<grid, kThreads, smem, s>>>(c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
                                    c.chunk_page, up.start, up.end, up.slot_mode, up.n_units, up.n_units_dev,
                                    m_tile_base, n_groups_real, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
-                                   stages);
+                                   stages, splits);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch maxsim_wgmma");
 }
 
 // Query tiles [base, base + nm) in one pass over the corpus.  nm is rounded up to a power of two: a phantom (all-zero) tile
-// costs less than a second pass over the corpus.
+// costs less than a second pass over the corpus.  Two full passes' worth of tiles run as one split launch (launch_one) when
+// the grid holds a pair of CTAs.
 template <int KIND, bool BITS>
 static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
                         int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
   constexpr int kMaxNM = Kind<KIND>::kMaxNM;
+  const bool pairs = (h->max_ctas > 0 ? h->max_ctas : h->num_sms) >= 2;
   for (int base = m_lo; base < m_hi;) {
     const int rem = m_hi - base;
+    if (pairs && rem >= 2 * kMaxNM) {
+      if (int e = launch_one<KIND, kMaxNM, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s, 2)) return e;
+      base += 2 * kMaxNM;
+      continue;
+    }
     int nm = 1;
     while (nm < rem && nm < kMaxNM) nm <<= 1;
     int e;
