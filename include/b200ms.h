@@ -406,6 +406,39 @@ int b200ms_fde_finalize(b200ms_t* h, const float* fde, int64_t n, void* out_rows
 int b200ms_fde_scan(b200ms_t* h, const void* fde_rows, const float* inv_norm, int64_t n_pages, const float* q_fde, int n_q,
                     float* scores, int64_t ld, void* stream);
 
+/* ---- sign candidates: asymmetric 1-bit MaxSim over an HBM sign copy of the corpus (new; no reference counterpart) --------
+ * A first stage for a two-stage search besides the FDE scan: full-precision queries against the sign bits of every page,
+ * then b200ms_rerank_batch_device / b200ms_rerank_docs_batch_device over the candidates.  A sign row is 16 B per patch
+ * vector (1/16 of bf16), so the signs of a host-resident corpus many times the size of HBM fit in HBM and are scanned
+ * exhaustively; only the candidates cross PCIe.
+ *   sign_rows: the sign rows of pages [first_page, first_page + n_pages) of the attached BF16 / I8 / F8 corpus into out
+ *     (device, padded rows page_start[first_page] .. page_start[first_page + n_pages], 16 B each, MSB first -- the layout of
+ *     a B1 corpus; padding rows repeat the page's last true row).  Bit i of row r = element i of the PACKED row r > 0:
+ *     BF16 > +0 (+-0 and NaN give 0), I8 > 0, F8 e4m3 sign clear and magnitude nonzero (NaN 0x7f gives 0).  Signs come from
+ *     the packed values, not the float source, so a corpus loaded from a shard file gets the signs of the live one; in I8 /
+ *     F8 corpora values that quantised to 0 give 0.  Host-resident rows are read through the mapping (one PCIe read of the
+ *     named pages).  B200MS_ESTATE: no corpus, or a B1 corpus (it has no more precise rows to rerank with).
+ *   set_sign_rows: attach caller-owned device sign rows (16-byte aligned, n_rows == b200ms_corpus_rows) for the corpus
+ *     attached now; every b200ms_set_corpus* detaches them.  A host-resident corpus gets its work units, chunk table and
+ *     scan-plan scratch here, on cuda_stream.  B200MS_ESTATE: no corpus, or a B1 corpus.
+ *   sign_candidates_device: per query q (q_dev F32 | BF16 rows [sum q_lens, 128], q_lens HOST)
+ *       q8 = clamp(rint(fp32(x * i8_q_scale)), -63, 63) per element (ties to even; NaN -> 0, +-inf -> +-63),
+ *       S[q, p] = sum over the query's tokens t of max over the TRUE rows r of page p of sum_i q8[t,i] * (bit(r,i) ? +1 : -1),
+ *     an exact int32 (a page without rows scores 0, a query without tokens scores 0 everywhere); the candidates are the
+ *     n_cand best pages by S among those q's mask allows, in b200ms_topk's order (S DESC, page id ASC), reported score
+ *     float32(S) * score_scale.  Outputs (device) cand_scores / cand_ids [n_q, n_cand] (unused: -inf / -1), cand_counts
+ *     [n_q]: the candidate layout b200ms_rerank_batch_device takes.  Masks as b200ms_search_device_masked (n_masks = 0:
+ *     unfiltered); only the allowed pages are scanned, without a synchronisation.  Works on host-resident corpora.
+ *     B200MS_EINVAL: src dtype, n_q < 1, a negative query length, n_cand outside [1, B200MS_MAX_K], i8_q_scale not finite
+ *     and > 0, NULL outputs, n_masks > 0 without masks and index;  B200MS_ESTATE: no corpus, or no sign rows attached to it.
+ * Nothing is launched when a call is refused. */
+int b200ms_sign_rows(b200ms_t* h, int64_t first_page, int64_t n_pages, uint8_t* out, void* cuda_stream);
+int b200ms_set_sign_rows(b200ms_t* h, const void* sign_rows, int64_t n_rows, void* cuda_stream);
+int b200ms_sign_candidates_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int n_cand,
+                                  const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev, float i8_q_scale,
+                                  float score_scale, float* cand_scores, int64_t* cand_ids, int32_t* cand_counts,
+                                  void* cuda_stream);
+
 /* ---- instrumentation ------------------------------------------------------------------------- */
 /* Kernels launched by this handle since creation (bench.py's gpu_launches claim). */
 int64_t b200ms_launch_count(const b200ms_t* h);

@@ -122,6 +122,10 @@ _SIGNATURES = {
                                           c_int64, vp, vp, vp, vp, vp]),
     "b200ms_rerank_docs_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, c_float,
                                                 c_float, vp, vp, vp, vp, vp]),
+    "b200ms_sign_rows": (c_int, [vp, c_int64, c_int64, vp, vp]),
+    "b200ms_set_sign_rows": (c_int, [vp, vp, c_int64, vp]),
+    "b200ms_sign_candidates_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, vp, vp, vp,
+                                              vp]),
 }
 
 

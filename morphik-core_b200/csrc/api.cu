@@ -466,6 +466,36 @@ B200MS_API int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, co
 }
 
 // ------------------------------------------------------------------------------------------------ corpus
+// ps_host: the corpus' padded page offsets [n_pages + 1]; page_start must already hold them on the device (ordered before s)
+int bms::build_scan_tables(b200ms_t* h, Corpus& c, const int64_t* ps_host, cudaStream_t s) {
+  // work units: runs of whole pages of about unit_rows rows; unit_start in chunks
+  // (small corpora: shrink the units so that every SM still gets about four of them -- a 100-page corpus as 25 units
+  // of 4096 rows would leave 123 SMs idle)
+  int64_t unit_rows = c.n_rows / (4 * int64_t(h->num_sms > 0 ? h->num_sms : 1));
+  if (unit_rows < kTileN) unit_rows = kTileN;
+  if (unit_rows > h->unit_rows) unit_rows = h->unit_rows;
+  std::vector<int32_t> us;
+  us.push_back(0);
+  int64_t acc = 0;
+  for (int64_t i = 0; i < c.n_pages; ++i) {
+    acc += ps_host[i + 1] - ps_host[i];
+    if (acc >= unit_rows) {
+      us.push_back(int32_t(ps_host[i + 1] / kGroup));
+      acc = 0;
+    }
+  }
+  if (us.back() != int32_t(c.n_chunks)) us.push_back(int32_t(c.n_chunks));
+  c.n_units = int(us.size()) - 1;
+  if (int e = upload(h, h->unit_start, us.data(), us.size() * 4, s)) return e;
+  if (int e = reserve(h, h->chunk_page, size_t(c.n_chunks > 0 ? c.n_chunks : 1) * 4)) return e;
+  if (int e = reserve_scan_plan(h, c)) return e;
+  if (int e = launch_chunk_page(h, static_cast<const int64_t*>(h->page_start.p), c.n_pages,
+                                static_cast<int32_t*>(h->chunk_page.p), s))
+    return e;
+  c.scan_tables = true;
+  return B200MS_OK;
+}
+
 // Page tables of a corpus; an HBM corpus also gets its work-unit plan, chunk table and TMA descriptor.  A host-resident one
 // (rows = the device address of mapped pinned memory) is only ever read by the candidate gather, which needs page_start.
 static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t* page_lens, int64_t n_pages, bool host) {
@@ -488,43 +518,17 @@ static int attach_corpus(b200ms_t* h, const void* rows, int dtype, const int32_t
   c.n_rows = ps[n_pages];
   c.n_chunks = c.n_rows / kGroup;
   if (c.n_chunks >= (int64_t(1) << 31)) return set_error(h, B200MS_EINVAL, "set_corpus: more than 2^31 chunks");
+  if (int e = upload(h, h->page_start, ps.data(), ps.size() * 8, s)) return e;
+  if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
+  h->page_len_host.assign(page_lens, page_lens + n_pages);
   if (host) {
-    if (int e = upload(h, h->page_start, ps.data(), ps.size() * 8, s)) return e;
-    if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
-    h->page_len_host.assign(page_lens, page_lens + n_pages);
     if (int e = check_cuda(h, cudaStreamSynchronize(s), "set_corpus_host: stream sync")) return e;
     order.finished();
     h->corpus = c;
     h->generation++;
     return B200MS_OK;
   }
-  // work units: runs of whole pages of about unit_rows rows; unit_start in chunks
-  // (small corpora: shrink the units so that every SM still gets about four of them -- a 100-page corpus as 25 units
-  // of 4096 rows would leave 123 SMs idle)
-  int64_t unit_rows = c.n_rows / (4 * int64_t(h->num_sms > 0 ? h->num_sms : 1));
-  if (unit_rows < kTileN) unit_rows = kTileN;
-  if (unit_rows > h->unit_rows) unit_rows = h->unit_rows;
-  std::vector<int32_t> us;
-  us.push_back(0);
-  int64_t acc = 0;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    acc += ps[i + 1] - ps[i];
-    if (acc >= unit_rows) {
-      us.push_back(int32_t(ps[i + 1] / kGroup));
-      acc = 0;
-    }
-  }
-  if (us.back() != int32_t(c.n_chunks)) us.push_back(int32_t(c.n_chunks));
-  c.n_units = int(us.size()) - 1;
-  if (int e = upload(h, h->page_start, ps.data(), ps.size() * 8, s)) return e;
-  if (int e = upload(h, h->unit_start, us.data(), us.size() * 4, s)) return e;
-  if (int e = upload(h, h->page_len, page_lens, size_t(n_pages) * 4, s)) return e;
-  h->page_len_host.assign(page_lens, page_lens + n_pages);
-  if (int e = reserve(h, h->chunk_page, size_t(c.n_chunks > 0 ? c.n_chunks : 1) * 4)) return e;
-  if (int e = reserve_scan_plan(h, c)) return e;
-  if (int e = launch_chunk_page(h, static_cast<const int64_t*>(h->page_start.p), n_pages,
-                                static_cast<int32_t*>(h->chunk_page.p), s))
-    return e;
+  if (int e = build_scan_tables(h, c, ps.data(), s)) return e;
   if (dtype != B200MS_B1 && c.n_rows > 0) {
     if (int e = make_tmap_rows(h, &c.tmap, rows, dtype, c.n_rows, kTileN)) return e;
     c.has_tmap = true;

@@ -152,6 +152,10 @@ struct Corpus {
   int64_t clamp_batch = 0;  // zero_pad_compat batch size the full-scan clamp bitmask (b200ms::clamp_pages) was built for
   bool host = false;        // rows live in mapped pinned host memory (b200ms_set_corpus_host): candidate scoring only
   int64_t max_page_rows = 0;  // largest padded page
+  bool scan_tables = false;   // n_units, unit_start, chunk_page and the scan-plan scratch are built (HBM corpora always; a
+                              // host-resident one once sign rows are attached to it)
+  bool signs = false;               // b200ms_set_sign_rows was called since the corpus was attached (set_corpus* detaches)
+  const void* sign_rows = nullptr;  // its device [n_rows, 16 B] sign bits
 };
 
 // The packed rows a scoring launch reads: the attached corpus, or -- for a host-resident corpus -- the HBM staging block
@@ -346,6 +350,15 @@ int launch_clamp_slots(b200ms_t* h, const int64_t* cand_ids, int n_cand, int n_l
                        uint32_t* clamp_bits, cudaStream_t s);
 int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
                           int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s);
+// The A operand of the 1-bit wgmma scan: int8 rows q_i8 [n_rows,128] (1024-byte aligned) and one int32 constant per row,
+// in the handle's scratch
+int reserve_b1_query(b200ms_t* h, int64_t n_rows, int8_t** q_i8, int32_t** tok_const);
+// The 1-bit wgmma scan of the sign rows of v (v.rows: 16 B per row) for prepared A rows: group_scores[g, p] = sum over the
+// group's rows t of (tok_const[t] + max over the page's rows r of <q_i8[t], bits(r) as {0,1}>)
+int launch_b1_tiles(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const int8_t* q_i8, const int32_t* tok_const,
+                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s);
+// Corpus tables a full scan needs (unit_start, chunk_page, scan-plan scratch), enqueued on s; c.n_units is set
+int build_scan_tables(b200ms_t* h, Corpus& c, const int64_t* ps_host, cudaStream_t s);
 // Scratch of launch_scan_plan for the corpus c (set_corpus reserves it, so that no search grows it)
 int reserve_scan_plan(b200ms_t* h, const Corpus& c);
 // Work units of a full scan that reads only the pages the call's masks allow (scan_plan.cu), built on stream s without a

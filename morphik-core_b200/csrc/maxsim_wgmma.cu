@@ -589,23 +589,34 @@ int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, con
   }
 }
 
+int reserve_b1_query(b200ms_t* h, int64_t n_rows, int8_t** q_i8, int32_t** tok_const) {
+  if (int e = reserve(h, h->b1_q_i8, size_t(n_rows) * 128 + 1024)) return e;
+  if (int e = reserve(h, h->b1_tok_const, size_t(n_rows) * 4)) return e;
+  *q_i8 = reinterpret_cast<int8_t*>((reinterpret_cast<uintptr_t>(h->b1_q_i8.p) + 1023) & ~uintptr_t(1023));
+  *tok_const = static_cast<int32_t*>(h->b1_tok_const.p);
+  return B200MS_OK;
+}
+
+int launch_b1_tiles(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const int8_t* q_i8, const int32_t* tok_const,
+                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
+  const int n_groups_padded = int(groups_padded(n_groups_real));
+  if (int e = query_tmap(h, q_i8, B200MS_I8, n_groups_padded * kGroup)) return e;
+  return launch_tiles<1, true>(h, v, plan, h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
+}
+
 // 1-bit full scan: the query bits become +-1 int8 rows (b1_q_i8) and per-token constants, then the int8 kernel with the
 // expanding producer.
 int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
                           int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
-  const int n_groups_padded = int(groups_padded(n_groups_real));
-  const int n_rows = n_groups_padded * kGroup;
-  if (int e = reserve(h, h->b1_q_i8, size_t(n_rows) * 128 + 1024)) return e;
-  if (int e = reserve(h, h->b1_tok_const, size_t(n_rows) * 4)) return e;
-  int8_t* q_i8 = reinterpret_cast<int8_t*>((reinterpret_cast<uintptr_t>(h->b1_q_i8.p) + 1023) & ~uintptr_t(1023));
-  int32_t* tok_const = static_cast<int32_t*>(h->b1_tok_const.p);
+  const int n_rows = int(groups_padded(n_groups_real)) * kGroup;
+  int8_t* q_i8 = nullptr;
+  int32_t* tok_const = nullptr;
+  if (int e = reserve_b1_query(h, n_rows, &q_i8, &tok_const)) return e;
   b1_query_expand_kernel<<<(n_rows * 16 + 255) / 256, 256, 0, s>>>(static_cast<const uint8_t*>(q_bits), group_ntok_dev, n_rows,
                                                                   q_i8, tok_const);
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
-  if (int e = query_tmap(h, q_i8, B200MS_I8, n_rows)) return e;
-  return launch_tiles<1, true>(h, corpus_view(h), plan, h->tmap_q, tok_const, n_groups_real, 0,
-                               n_groups_padded / 4, group_scores, ld, s);
+  return launch_b1_tiles(h, corpus_view(h), plan, q_i8, tok_const, n_groups_real, group_scores, ld, s);
 }
 
 }  // namespace bms

@@ -15,19 +15,6 @@
 
 namespace bms {
 
-__device__ __forceinline__ float4 load_row4(const void* src, int src_dtype, int64_t row, int lane) {
-  if (src_dtype == B200MS_F32) {
-    return __ldg(reinterpret_cast<const float4*>(src) + row * 32 + lane);
-  }
-  const uint2 raw = __ldg(reinterpret_cast<const uint2*>(src) + row * 32 + lane);
-  float4 v;
-  v.x = __uint_as_float(raw.x << 16);
-  v.y = __uint_as_float(raw.x & 0xffff0000u);
-  v.z = __uint_as_float(raw.y << 16);
-  v.w = __uint_as_float(raw.y & 0xffff0000u);
-  return v;
-}
-
 // NaN -> 0: it has neither sign nor magnitude (fmaxf(NaN, -127) alone would make it -127, the strongest negative value)
 __device__ __forceinline__ int quant_i8(float x, float scale) {
   const float r = rintf(x * scale);  // round-half-even, like numpy.rint in the oracle

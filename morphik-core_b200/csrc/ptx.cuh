@@ -8,6 +8,8 @@
 #include <cstdio>
 #include <type_traits>
 
+#include "../../include/b200ms.h"
+
 namespace bms {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -236,6 +238,20 @@ __device__ __forceinline__ float warp_sum(float v) {
 __device__ __forceinline__ int warp_sum(int v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// elements 4 lane .. 4 lane + 3 of row `row` of a [rows,128] F32 | BF16 matrix as float32 (bf16 widened exactly)
+__device__ __forceinline__ float4 load_row4(const void* src, int src_dtype, int64_t row, int lane) {
+  if (src_dtype == B200MS_F32) {
+    return __ldg(reinterpret_cast<const float4*>(src) + row * 32 + lane);
+  }
+  const uint2 raw = __ldg(reinterpret_cast<const uint2*>(src) + row * 32 + lane);
+  float4 v;
+  v.x = __uint_as_float(raw.x << 16);
+  v.y = __uint_as_float(raw.x & 0xffff0000u);
+  v.z = __uint_as_float(raw.y << 16);
+  v.w = __uint_as_float(raw.y & 0xffff0000u);
   return v;
 }
 

@@ -195,14 +195,18 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
     def __init__(self, uri: str = "b200://0", device: int = 0, mode: str = "bf16", storage: Any = None,
                  auto_initialize: bool = True, compact_dead_fraction: float = 0.3, index: Any = None,
                  fde_candidates: Optional[int] = None, coalesce_queries: bool = True, max_coalesced_tokens: int = 1024,
-                 max_coalesced_queries: int = 64, zero_pad_compat: int = 0, corpus_tier: str = "hbm"):
-        # corpus_tier "host": patch rows in pinned host memory, bounded by host RAM instead of HBM; only the FDE candidates of
-        # a query cross PCIe (the reference's load_multivector_from_storage, fast_multivector_store.py:545-548), so it needs
+                 max_coalesced_queries: int = 64, zero_pad_compat: int = 0, corpus_tier: str = "hbm",
+                 sign_candidates: Optional[int] = None):
+        # corpus_tier "host": patch rows in pinned host memory, bounded by host RAM instead of HBM; only the candidates of a
+        # query cross PCIe (the reference's load_multivector_from_storage, fast_multivector_store.py:545-548), so it needs
         # the two-stage search
         if corpus_tier not in ("hbm", "host"):
             raise ValueError(f"corpus_tier must be 'hbm' or 'host', got {corpus_tier!r}")
-        if corpus_tier == "host" and not fde_candidates:
-            raise ValueError("corpus_tier='host' needs fde_candidates: a host-resident corpus is only scored on candidate lists")
+        if fde_candidates and sign_candidates:
+            raise ValueError("fde_candidates and sign_candidates are two first stages of the two-stage search: pass one")
+        if corpus_tier == "host" and not (fde_candidates or sign_candidates):
+            raise ValueError("corpus_tier='host' needs fde_candidates or sign_candidates: a host-resident corpus is only scored "
+                             "on candidate lists")
         self.corpus_tier = corpus_tier
         self.uri = uri
         self.device = int(device)
@@ -216,6 +220,9 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         # None: exhaustive MaxSim over every authorised page (Postgres-provider behaviour).  An int: two-stage search like
         # the "morphik" provider -- FDE candidates (the reference asks Turbopuffer for min(10*k, 75)) then MaxSim rerank.
         self.fde_candidates = fde_candidates
+        # An int: the same two-stage search with the asymmetric sign scan as its first stage (signs.SignTwoStageIndex:
+        # full-precision queries against an HBM sign copy of every page) instead of the FDE scan.
+        self.sign_candidates = sign_candidates
         self._two_stage = None
         # > 0: reproduce colpali_engine score_multi_vector's zero-padding quirk with this batch size (128 upstream): a page
         # shorter than the longest page of its scoring batch scores sum_t max(max_r <q_t,d_r>, 0)  (SURVEY App. A.2;
@@ -240,6 +247,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
                 self._two_stage = TwoStageIndex(device=self.device, dtype=self.mode, tier=self.corpus_tier)
                 self._index = self._two_stage.index
+            elif self.sign_candidates:
+                from .signs import SignTwoStageIndex
+
+                self._two_stage = SignTwoStageIndex(device=self.device, dtype=self.mode, tier=self.corpus_tier)
+                self._index = self._two_stage.index
             else:
                 self._index = MaxSimIndex(device=self.device, dtype=self.mode)
         elif self.fde_candidates and self._two_stage is None and hasattr(self._index, "h"):
@@ -247,6 +259,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             from .fde import TwoStageIndex
 
             self._two_stage = TwoStageIndex(index=self._index)
+            self._two_stage.rebuild_from_index()
+        elif self.sign_candidates and self._two_stage is None and hasattr(self._index, "h"):
+            from .signs import SignTwoStageIndex  # likewise the sign rows
+
+            self._two_stage = SignTwoStageIndex(index=self._index)
             self._two_stage.rebuild_from_index()
         if self.zero_pad_compat and hasattr(self._index, "set_option"):
             self._index.set_option("zero_pad_compat", self.zero_pad_compat)
@@ -293,8 +310,15 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 assert pid == first + i, "catalogue and device corpus out of step"
                 recs.append(rec)
             if self._journal is not None:  # durable store: this call becomes one append-only segment
-                fde = self._two_stage.fde_rows(first, n) if self._two_stage is not None else None
-                self._journal.log_add(self._index, first, n, [dataclasses.asdict(r) for r in recs], fde)
+                self._journal.log_add(self._index, first, n, [dataclasses.asdict(r) for r in recs], self._fde_rows(first, n))
+
+    def _fde_rows(self, first: int, n: int):
+        """What a journal segment persists of the first stage: the FDE rows (sign rows are derived again on replay)."""
+        return self._two_stage.fde_rows(first, n) if self._two_stage is not None and self.fde_candidates else None
+
+    @property
+    def _n_candidates(self) -> int:
+        return int(self.fde_candidates or self.sign_candidates)
 
     # ------------------------------------------------------------------ read path
     async def query_similar(self, query_embedding, k: int, doc_ids: Optional[List[str]] = None,
@@ -380,7 +404,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             t3 = time.perf_counter()
         self.last_query_timing = {"prepare_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3,
                                   "build_chunks_ms": (t3 - t2) * 1e3, "total_ms": (t3 - t0) * 1e3}
-        if self._two_stage is not None:  # the reference's stage names (fast_multivector_store.py:523,534,550,574,589,604)
+        if self._two_stage is not None and self.sign_candidates:
+            st = self._two_stage.last_timing_ms
+            self.last_query_timing.update({k: float(st.get(k, 0.0)) for k in (
+                "sign_candidates_ms", "maxsim_rerank_ms", "load_multivectors_ms", "rerank_scoring_ms")})
+        elif self._two_stage is not None:  # the reference's stage names (fast_multivector_store.py:523,534,550,574,589,604)
             st = self._two_stage.last_timing_ms
             self.last_query_timing.update(encode_query_ms=st.get("encode_query_ms", 0.0), ns_query_ms=st.get("ns_query_ms", 0.0),
                                           load_multivectors_ms=0.0, rerank_scoring_ms=st.get("rerank_scoring_ms", 0.0),
@@ -394,7 +422,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
     def _search_unlocked(self, queries, k, words):
         if self._two_stage is not None:
-            return self._two_stage.search(queries, k, n_candidates=max(int(self.fde_candidates), k), allow_mask=words)
+            return self._two_stage.search(queries, k, n_candidates=max(self._n_candidates, k), allow_mask=words)
         return self._index.search_host(queries, k, allow_mask=words)
 
     async def query_similar_documents(self, query_embedding, k: int, pages_per_document: int = 1,
@@ -431,7 +459,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             page_doc = self._page_doc_cache[1]
             if self._two_stage is not None:
                 ts, ti, pc, dc = self._two_stage.search_docs([q], kk, per, page_doc, n_docs,
-                                                             n_candidates=max(int(self.fde_candidates), kk * per), allow_mask=words)
+                                                             n_candidates=max(self._n_candidates, kk * per), allow_mask=words)
             else:
                 ts, ti, pc, dc = self._index.search_docs([q], kk, per, page_doc, n_docs, allow_mask=words)
             out = []
@@ -536,8 +564,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             if self._journal is not None and os.path.abspath(self._journal.dir) == os.path.abspath(directory):
                 self._journal.reset()
                 if len(self.catalog):
-                    fde = self._two_stage.fde_rows(0, len(self.catalog)) if self._two_stage is not None else None
-                    self._journal.log_add(self._index, 0, len(self.catalog), [dataclasses.asdict(r) for r in self.catalog.records], fde)
+                    self._journal.log_add(self._index, 0, len(self.catalog), [dataclasses.asdict(r) for r in self.catalog.records],
+                                          self._fde_rows(0, len(self.catalog)))
 
     @classmethod
     def load(cls, directory: str, device: int = 0, **kw) -> "B200MultiVectorStore":
@@ -580,7 +608,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 with open(cat) as f:
                     for line in f:
                         store.catalog.add(PageRecord(**json.loads(line)))
-                if store._two_stage is not None:
+                if store._two_stage is not None and store.fde_candidates:
                     if os.path.exists(fde):
                         blob = torch.load(fde)
                         store._two_stage.append_fde_rows(blob["rows"].view(torch.bfloat16), blob["inv"])
@@ -590,6 +618,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                     raise ValueError(f"{seg}: segment and journal disagree on the page count")
             elif op["op"] == "delete":
                 store.catalog.delete_document(op["document_id"])
+        if store._two_stage is not None and store.sign_candidates:
+            store._two_stage.rebuild_from_index()  # once, over every replayed segment
         with store._lock:
             if store.catalog.dead_fraction > store.compact_dead_fraction:
                 store._compact_locked()
