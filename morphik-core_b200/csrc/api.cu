@@ -721,8 +721,7 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   // POPC launches write only their own query's groups and slots
   const bool zero_fill = b1 ? (b1_wgmma && c.has_empty) || cs.per_query : c.has_empty || cs.ids;
   if (zero_fill && fill)
-    if (int e = check_cuda(h, cudaMemsetAsync(group_scores, 0, size_t(groups_padded(n_groups)) * size_t(ld) * 4, s), "score: memset"))
-      return e;
+    if (int e = zero_scores(h, group_scores, groups_padded(n_groups), ld, s, "score: memset")) return e;
   UnitPlan plan = scan ? *scan : full_scan_plan(h);
   if (!cs.ids) h->scan_planned = scan != nullptr;
   if (!b1) {
@@ -837,6 +836,20 @@ B200MS_API int b200ms_merge_topk(b200ms_t* h, const float* cand_scores, const in
 
 namespace bms {
 
+int zero_scores(b200ms_t* h, void* scores, int64_t gp, int64_t ld, cudaStream_t s, const char* what) {
+  return check_cuda(h, cudaMemsetAsync(scores, 0, size_t(gp) * size_t(ld) * 4, s), what);
+}
+
+// A filtered full scan reads only the pages some query of the call may see.  The other pages keep whatever the score matrix
+// held before, and that is never read: the selection skips a page whose allow bit is clear before it touches the page's
+// score, in the flat form (page_key) and in the document form (doc_item) alike.  A corpus whose own plan is one wave of
+// units gains nothing from a shorter one, so it keeps it (and a small search its launch count).
+int plan_full_scan(b200ms_t* h, const uint32_t* allow, const int32_t* mask_index, int n_q, cudaStream_t s, UnitPlan* plan) {
+  *plan = full_scan_plan(h);
+  h->scan_planned = allow && h->corpus.n_units > (h->max_ctas > 0 ? h->max_ctas : h->num_sms);
+  return h->scan_planned ? launch_scan_plan(h, allow, mask_index, n_q, s, plan) : B200MS_OK;
+}
+
 int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "search: no corpus attached (call b200ms_set_corpus first)");
@@ -857,9 +870,8 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
     if (int e = launch_pad_cands(h, r.cand.ids, cs.n_cand, n_q, cs.stride(), static_cast<int64_t*>(h->cand_pad.p), s)) return e;
     cs.ids = static_cast<const int64_t*>(h->cand_pad.p);
   }
-  const int64_t gp = m.groups_padded > 0 ? m.groups_padded : 4;
   const int64_t n_items = cs.ids ? cs.n_slots(n_q) : c.n_pages;
-  const int64_t ld = ((n_items + 31) & ~int64_t(31)) > 0 ? ((n_items + 31) & ~int64_t(31)) : 32;
+  const auto [gp, ld] = score_layout(m, n_items);
   if (int e = reserve(h, h->q_packed, size_t(gp) * kGroup * size_t(b200ms_row_bytes(c.dtype)))) return e;
   if (int e = reserve(h, h->scores, size_t(gp) * size_t(ld) * 4)) return e;
   if (!meta_dev) {
@@ -877,16 +889,12 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
       return e;
   const int ng = int(m.groups);
   if (!c.host) {
-    // A filtered full scan reads only the pages some query of the call may see.  The other pages keep whatever h->scores
-    // held before, and that is never read: the selection below skips a page whose allow bit is clear before it touches
-    // the page's score, in the flat form (page_key) and in the document form (doc_item) alike.  A corpus whose own plan
-    // is one wave of units gains nothing from a shorter one, so it keeps it (and a small search its launch count).
-    UnitPlan filtered;
-    const bool plan_scan = !cs.ids && r.allow && ng > 0 && c.n_units > (h->max_ctas > 0 ? h->max_ctas : h->num_sms);
-    if (plan_scan)
-      if (int e = launch_scan_plan(h, r.allow, r.mask_index, n_q, s, &filtered)) return e;
+    UnitPlan scan;
+    const bool full_scan = !cs.ids && ng > 0;
+    if (full_scan)
+      if (int e = plan_full_scan(h, r.allow, r.mask_index, n_q, s, &scan)) return e;
     if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s, corpus_view(h), cs.ids, true,
-                           plan_scan ? &filtered : nullptr))
+                           full_scan && h->scan_planned ? &scan : nullptr))
       return e;
   } else if (ng > 0 && n_items > 0) {
     struct Ctx {
@@ -905,10 +913,8 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
     };
     if (int e = score_host_tier(h, cs, n_q, gp, ld, h->scores.p, s, round, &ctx)) return e;
   }
-  if (ng == 0 || n_items == 0) {
-    // nothing scored: every page (if any) has score 0 -- still a defined ranking
-    if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "search: memset")) return e;
-  }
+  if (ng == 0 || n_items == 0)
+    if (int e = zero_scores(h, h->scores.p, gp, ld, s, "search: memset")) return e;
   const int sdt = (c.dtype == B200MS_BF16 || c.dtype == B200MS_F8) ? B200MS_F32 : B200MS_I32;
   if (r.docs)
     return cs.ids ? launch_topk_docs(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, nullptr, nullptr, cs.ids, cs.stride(),

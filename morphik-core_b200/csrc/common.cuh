@@ -310,6 +310,21 @@ inline UnitPlan full_scan_plan(const b200ms_t* h) {
   return p;
 }
 
+// Score matrix of a call: gp padded query groups (at least 4) by ld items (n_items rounded up to 32, at least 32), 4 bytes each
+struct ScoreLayout {
+  int64_t gp, ld;
+};
+inline ScoreLayout score_layout(const SearchMeta& m, int64_t n_items) {
+  const int64_t ld = (n_items + 31) & ~int64_t(31);
+  return {m.groups_padded > 0 ? m.groups_padded : 4, ld > 0 ? ld : 32};
+}
+// Zeroes gp x ld scores: the scores no launch writes (the tile kernels skip pages without rows), or all of them when a call
+// scores nothing -- every page then scores 0, still a defined ranking
+int zero_scores(b200ms_t* h, void* scores, int64_t gp, int64_t ld, cudaStream_t s, const char* what);
+// The units a full scan of the attached corpus walks, into *plan: the corpus' own, or with allow masks the filtered plan
+// (launch_scan_plan).  Sets h->scan_planned to which one it is (b200ms_last_scan_stats).
+int plan_full_scan(b200ms_t* h, const uint32_t* allow, const int32_t* mask_index, int n_q, cudaStream_t s, UnitPlan* plan);
+
 // The attached corpus as the scorers see it
 inline CorpusView corpus_view(const b200ms_t* h) {
   const Corpus& c = h->corpus;

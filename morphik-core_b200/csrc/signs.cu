@@ -160,8 +160,7 @@ B200MS_API int b200ms_sign_candidates_device(b200ms_t* h, const void* q_dev, int
   if (int e = order.error()) return e;
   const SearchMeta m = build_search_meta(q_lens, n_q);
   const int ng = int(m.groups);
-  const int64_t gp = m.groups_padded > 0 ? m.groups_padded : 4;
-  const int64_t ld = ((c.n_pages + 31) & ~int64_t(31)) > 0 ? ((c.n_pages + 31) & ~int64_t(31)) : 32;
+  const auto [gp, ld] = score_layout(m, c.n_pages);
   if (int e = reserve(h, h->scores, size_t(gp) * size_t(ld) * 4)) return e;
   if (int e = upload(h, h->meta, m.host.data(), m.host.size(), s)) return e;
   const uint8_t* md = static_cast<const uint8_t*>(h->meta.p);
@@ -179,22 +178,17 @@ B200MS_API int b200ms_sign_candidates_device(b200ms_t* h, const void* q_dev, int
         i8_q_scale, reinterpret_cast<uint32_t*>(q_i8), tok_const);
     h->launches++;
     if (int e = check_cuda(h, cudaGetLastError(), "launch sign_query")) return e;
-    // the tile kernel writes no score for a page without rows; a filtered plan leaves the other pages' scores unwritten,
-    // and the selection never reads them (scan_plan.cu)
     if (c.has_empty)
-      if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "sign_candidates: memset"))
-        return e;
-    UnitPlan plan = full_scan_plan(h);
-    h->scan_planned = allow && c.n_units > (h->max_ctas > 0 ? h->max_ctas : h->num_sms);  // as search_core decides
-    if (h->scan_planned)
-      if (int e = launch_scan_plan(h, allow, mask_index, n_q, s, &plan)) return e;
+      if (int e = zero_scores(h, h->scores.p, gp, ld, s, "sign_candidates: memset")) return e;
+    UnitPlan plan;
+    if (int e = plan_full_scan(h, allow, mask_index, n_q, s, &plan)) return e;
     CorpusView v = corpus_view(h);
     v.rows = c.sign_rows;
     v.dtype = B200MS_B1;
     v.tmap = nullptr;
     if (int e = launch_b1_tiles(h, v, plan, q_i8, tok_const, ng, h->scores.p, ld, s)) return e;
-  } else if (int e = check_cuda(h, cudaMemsetAsync(h->scores.p, 0, size_t(gp) * size_t(ld) * 4, s), "sign_candidates: memset")) {
-    return e;  // nothing scored: every page scores 0, still a defined ranking
+  } else if (int e = zero_scores(h, h->scores.p, gp, ld, s, "sign_candidates: memset")) {
+    return e;
   }
   return launch_topk(h, h->scores.p, B200MS_I32, c.n_pages, ld, goff_dev, n_q, allow, n_cand, score_scale, 0, nullptr,
                      cand_scores, cand_ids, cand_counts, s, mask_index, (c.n_pages + 31) / 32);

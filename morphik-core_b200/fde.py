@@ -29,6 +29,7 @@ must stay interchangeable with vectors written by the reference dumps the extens
 from __future__ import annotations
 
 import ctypes
+import os
 import threading
 from dataclasses import dataclass
 from typing import Dict, Optional, Sequence, Tuple
@@ -37,7 +38,8 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .index import DeviceBlock, MaxSimIndex, _check_device_masks, _host_mask_to_device, _runs, _topk_outputs, _vp
+from .index import DeviceBlock, MaxSimIndex, _compact_rows, _runs, _topk_outputs, _vp
+from .two_stage import TwoStageSearch
 
 
 @dataclass(frozen=True)
@@ -144,20 +146,27 @@ def configure_handle(index: MaxSimIndex, cfg: FixedDimensionalEncodingConfig, ma
         "b200ms_fde_configure_ex")
 
 
-def encode_items(index: MaxSimIndex, items: Sequence, is_document: bool, fde_dim: int) -> torch.Tensor:
-    """FDEs of ragged [n_i,128] items -> float32 device tensor [len(items), fde_dim] (one kernel launch per 65535 items)."""
-    out = torch.empty((len(items), fde_dim), dtype=torch.float32, device=index.device)
-    step = 65535
-    for i0 in range(0, len(items), step):
-        part = items[i0:i0 + step]
-        lens = [int(x.shape[0]) for x in part]
-        src, src_dtype = index._stage_rows(part)
+def encode_rows(index: MaxSimIndex, src: torch.Tensor, src_dtype: int, lens: Sequence[int], is_document: bool,
+                fde_dim: int) -> torch.Tensor:
+    """FDEs of staged ragged items (``src`` [>= sum(lens), 128] on the device, item i = the next lens[i] rows) -> float32
+    device tensor [len(lens), fde_dim] (one kernel launch per 65535 items)."""
+    out = torch.empty((len(lens), fde_dim), dtype=torch.float32, device=index.device)
+    step, row0 = 65535, 0
+    for i0 in range(0, len(lens), step):
+        part = [int(n) for n in lens[i0:i0 + step]]
         with torch.cuda.device(index.device):
             index.h.check(
-                nat.lib.b200ms_fde_encode(index.h.ptr, _vp(src), src_dtype, nat.i32_array(lens), len(lens), int(is_document),
-                                          _vp(out[i0:i0 + len(part)]), index._stream()),
+                nat.lib.b200ms_fde_encode(index.h.ptr, _vp(src[row0:]), src_dtype, nat.i32_array(part), len(part),
+                                          int(is_document), _vp(out[i0:i0 + len(part)]), index._stream()),
                 "b200ms_fde_encode")
+        row0 += sum(part)
     return out
+
+
+def encode_items(index: MaxSimIndex, items: Sequence, is_document: bool, fde_dim: int) -> torch.Tensor:
+    """FDEs of ragged [n_i,128] items -> float32 device tensor [len(items), fde_dim]."""
+    src, src_dtype = index._stage_rows(list(items))
+    return encode_rows(index, src, src_dtype, [int(x.shape[0]) for x in items], is_document, fde_dim)
 
 
 # ------------------------------------------------------------------ module-level API (drop-in for the extension module)
@@ -190,27 +199,26 @@ def generate_document_encoding(point_cloud, config: FixedDimensionalEncodingConf
 
 
 # ------------------------------------------------------------------ two-stage index
-class TwoStageIndex:
+class TwoStageIndex(TwoStageSearch):
     """MaxSimIndex + a dense FDE matrix [N, fde_dim] bf16 with per-row inverse norms.
 
     search(): query FDE (device) -> exhaustive cosine scan of the FDE matrix (HBM-bound, 2*fde_dim bytes per page) -> top
-    ``n_candidates`` per query -> exact MaxSim over those pages only (b200ms_rerank_device) -> top-k.
+    ``n_candidates`` per query -> exact MaxSim over those pages only (TwoStageSearch) -> top-k.
     """
+    STAGE_TIMES = {"encode_query_ms": (0, 1), "ns_query_ms": (1, 2), "fde_candidates_ms": (0, 2)}
 
     def __init__(self, device: int = 0, dtype: str = "bf16", config: Optional[FixedDimensionalEncodingConfig] = None,
                  matrices: Optional[FdeMatrices] = None, index: Optional[MaxSimIndex] = None, tier: str = "hbm"):
         """tier="host": the patch rows live in pinned host memory (MaxSimIndex tier "host") and every search gathers only
         its candidate pages over PCIe; the FDE matrix stays in HBM either way."""
+        super().__init__(index if index is not None else MaxSimIndex(device=device, dtype=dtype, tier=tier))
         self.cfg = config or FixedDimensionalEncodingConfig()
-        self.index = index if index is not None else MaxSimIndex(device=device, dtype=dtype, tier=tier)
         configure_handle(self.index, self.cfg, matrices)
-        self.device = self.index.device
         self.fde_dim = self.cfg.fde_dimension
         self._Fblock: Optional[DeviceBlock] = None  # owner of the memory self._F views
         self._F: Optional[torch.Tensor] = None  # bf16 [cap, fde_dim]
         self._inv: Optional[torch.Tensor] = None  # float32 [cap]
         self._n = 0
-        self.last_timing_ms: Dict[str, float] = {}
 
     @property
     def n_pages(self) -> int:
@@ -226,17 +234,15 @@ class TwoStageIndex:
         """Back `rows` FDE rows (rounded up to whole chunks) of the matrix's block -- no copy of the matrix, as for the
         patch rows (MaxSimIndex._resize_block); _F is a view of the block.  The inverse norms (4 bytes per page) are a
         torch tensor of the same capacity and are copied."""
-        if self._Fblock is None:
-            self._Fblock = DeviceBlock(self.index.h, self.device)
-        self._Fblock.resize(rows * 2 * self.fde_dim)
-        if self._Fblock.tensor is None:
+        self._Fblock = DeviceBlock.resized(self._Fblock, self.index.h, self.device, rows * 2 * self.fde_dim)
+        F = self._Fblock.rows(2 * self.fde_dim)
+        if F is None:
             self._F = self._inv = None
             return
-        cap = self._Fblock.tensor.numel() // (2 * self.fde_dim)
-        self._F = self._Fblock.tensor[: cap * 2 * self.fde_dim].view(torch.bfloat16).view(cap, self.fde_dim)
-        inv = torch.empty((cap,), dtype=torch.float32, device=self.device)
+        self._F = F.view(torch.bfloat16)
+        inv = torch.empty((F.shape[0],), dtype=torch.float32, device=self.device)
         if self._inv is not None:
-            n = min(self._n, cap)
+            n = min(self._n, F.shape[0])
             inv[:n].copy_(self._inv[:n])
         self._inv = inv
 
@@ -328,23 +334,28 @@ class TwoStageIndex:
         keep = [int(p) for p in keep]
         self.index.compact(keep)
         if self._F is not None:
-            runs = list(_runs(keep))
-            run_start = np.array([a for a, _ in runs], dtype=np.int64)
-            run_rows = np.array([b - a + 1 for a, b in runs], dtype=np.int64)
             keep_t = torch.as_tensor(keep, dtype=torch.int64, device=self.device)
             self._inv[: len(keep)] = self._inv.index_select(0, keep_t)
-            with torch.cuda.device(self.device):
-                self.index.h.check(
-                    nat.lib.b200ms_compact_rows(self.index.h.ptr, _vp(self._F), 2 * self.fde_dim,
-                                                run_start.ctypes.data_as(nat.i64p), run_rows.ctypes.data_as(nat.i64p),
-                                                len(runs), self.index._stream()),
-                    "b200ms_compact_rows")
+            _compact_rows(self.index.h, self.device, self._F, 2 * self.fde_dim, [(a, b + 1) for a, b in _runs(keep)])
             self._n = len(keep)
-            torch.cuda.current_stream(self.device).synchronize()  # as MaxSimIndex.compact: torch's own copies into _F
             self._resize(len(keep))
         self._n = len(keep)
 
-    def _fde_topk(self, q_fde: torch.Tensor, kc: int, mask: Optional[torch.Tensor]):
+    journal_rows = fde_rows
+
+    def replay_segment(self, path: str) -> None:
+        if os.path.exists(path):
+            blob = torch.load(path)
+            self.append_fde_rows(blob["rows"].view(torch.bfloat16), blob["inv"])
+        else:
+            self.rebuild_from_index()
+
+    def _encode(self, queries: Sequence, staged) -> torch.Tensor:
+        if staged is None:
+            return encode_items(self.index, list(queries), False, self.fde_dim)
+        return encode_rows(self.index, *staged, False, self.fde_dim)
+
+    def _scan(self, q_fde: torch.Tensor, lens: Sequence[int], kc: int, mask: Optional[torch.Tensor]):
         """Scan of the FDE matrix for query FDEs [n_q, fde_dim] -> top kc pages per query among those `mask` (already
         checked) allows: (scores, page ids, counts) on the device."""
         n_q = q_fde.shape[0]
@@ -358,87 +369,3 @@ class TwoStageIndex:
                 "b200ms_topk(fde)")
         return ts, ti, tc
 
-    def candidates(self, queries: Sequence, n_candidates: int, allow_mask_dev: Optional[torch.Tensor] = None):
-        """First stage only: (candidate page ids int64 [n_q, n_candidates] (-1 padded), FDE scores, counts) on the device.
-        allow_mask_dev: optional uint32 page bitmask (the doc_ids filter, applied BEFORE candidate selection like the
-        reference's Turbopuffer filter, fast_multivector_store.py:527)."""
-        mask, _, _ = _check_device_masks(allow_mask_dev, None, len(queries), self._n, self.device)
-        q_fde = encode_items(self.index, list(queries), False, self.fde_dim)
-        ts, ti, tc = self._fde_topk(q_fde, int(min(n_candidates, nat.MAX_K)), mask)
-        return ti, ts, tc
-
-    def rerank(self, query, cand_ids: torch.Tensor, k: int):
-        """Exact MaxSim of ONE query over the candidate pages (device int64 [n_cand], -1 = unused) -> top-k."""
-        src, _ = self.index._stage_rows([query])
-        return self.index.rerank(src, [int(query.shape[0])], cand_ids.contiguous(), k)
-
-    def search_device(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
-                      id_base: int = 0):
-        """Two-stage search, everything on the device and asynchronous: query FDEs -> ONE scan of the FDE matrix for the
-        whole batch (wgmma) -> top-n_candidates per query -> ONE batched rerank call (each query against its own list)
-        -> top-k.  Returns device tensors (scores [n_q,kk], page ids + id_base [n_q,kk], counts [n_q]) and the CUDA events
-        that bracket the stages (for last_timing_ms)."""
-        mask, _, _ = _check_device_masks(allow_mask_dev, None, len(queries), self._n, self.device)
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-        ev[0].record()
-        q_fde = encode_items(self.index, list(queries), False, self.fde_dim)
-        ev[1].record()
-        kc = int(min(max(n_candidates, k), nat.MAX_K, max(self._n, 1)))
-        _, ci, _ = self._fde_topk(q_fde, kc, mask)
-        ev[2].record()
-        src, _ = self.index._stage_rows(list(queries))
-        ts, ti, tc = self.index.rerank_batch(src, [int(q.shape[0]) for q in queries], ci, k)
-        if id_base:
-            ti = torch.where(ti >= 0, ti + int(id_base), ti)
-        ev[3].record()
-        return ts, ti, tc, ev
-
-    def search_docs_device(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
-                           n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None):
-        """Two-stage search grouped by document: max(n_candidates, k * per_doc) FDE candidates per query (at most MAX_K),
-        then MaxSimIndex.rerank_docs_batch over them.  Returns its four device tensors."""
-        kc = int(min(max(n_candidates, k * per_doc), nat.MAX_K, max(self._n, 1)))
-        ci, _, _ = self.candidates(queries, kc, allow_mask_dev)
-        src, _ = self.index._stage_rows(list(queries))
-        return self.index.rerank_docs_batch(src, [int(q.shape[0]) for q in queries], ci, k, per_doc, page_doc_dev, n_docs)
-
-    def search_docs(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
-                    n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
-        """search_docs_device with a host allow mask (uint32 words, restricting both stages); synchronous, returns host
-        arrays (scores [n_q,k,per_doc], page ids [n_q,k,per_doc], pages per document [n_q,k], documents [n_q])."""
-        mask_dev = _host_mask_to_device(allow_mask, self._n, self.device)
-        ts, ti, pc, dc = self.search_docs_device(queries, k, per_doc, page_doc_dev, n_docs, n_candidates, mask_dev)
-        n_q, kk = len(queries), ts.shape[1]
-        out_s = np.full((n_q, k, per_doc), -np.inf, dtype=np.float32)
-        out_i = np.full((n_q, k, per_doc), -1, dtype=np.int64)
-        out_pc = np.zeros((n_q, k), dtype=np.int32)
-        out_s[:, :kk], out_i[:, :kk], out_pc[:, :kk] = ts.cpu().numpy(), ti.cpu().numpy(), pc.cpu().numpy()
-        return out_s, out_i, out_pc, dc.cpu().numpy()
-
-    def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
-        """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
-        the same exact scorer that ranked them."""
-        return self.index.explain(queries, page_ids, map_rows)
-
-    def search(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
-        """Two-stage search; returns host arrays (scores [n_q,k], page ids [n_q,k], counts [n_q]) and fills last_timing_ms
-        with the reference's stage names (fast_multivector_store.py:523,534,550,574): encode_query / ns.query (here: FDE scan
-        + candidate top-k on the GPU) / load_multivectors (0: resident in HBM) / rerank_scoring.
-        allow_mask: optional uint32 words (page bitmask) restricting BOTH stages (the reference filters inside the ANN query)."""
-        n_q = len(queries)
-        mask_dev = _host_mask_to_device(allow_mask, self._n, self.device)
-        ts, ti, tc, ev = self.search_device(queries, k, n_candidates, mask_dev)
-        torch.cuda.synchronize(self.device)
-        kk = ts.shape[1]
-        out_s = np.full((n_q, k), -np.inf, dtype=np.float32)
-        out_i = np.full((n_q, k), -1, dtype=np.int64)
-        out_s[:, :kk], out_i[:, :kk] = ts.cpu().numpy(), ti.cpu().numpy()
-        out_c = tc.cpu().numpy().astype(np.int32)
-        rerank_ms = ev[2].elapsed_time(ev[3])
-        # load_multivectors: 0 with the rows resident in HBM; the host tier's PCIe gather of the candidate pages
-        gather = self.index.gather_stats() if self.index.tier == "host" else {"ms": 0.0, "bytes": 0, "unique_pages": 0}
-        self.last_timing_ms = {"encode_query_ms": ev[0].elapsed_time(ev[1]), "ns_query_ms": ev[1].elapsed_time(ev[2]),
-                               "load_multivectors_ms": gather["ms"], "rerank_scoring_ms": rerank_ms - gather["ms"],
-                               "fde_candidates_ms": ev[0].elapsed_time(ev[2]), "maxsim_rerank_ms": rerank_ms,
-                               "gather_bytes": gather["bytes"], "gather_pages": gather["unique_pages"]}
-        return out_s, out_i, out_c

@@ -52,6 +52,12 @@ def _runs(ids: Sequence[int]):
         i = j + 1
 
 
+def _row_runs(page_lens: Sequence[int], keep: Sequence[int]) -> List[Tuple[int, int]]:
+    """Packed row ranges [a, b) of the maximal runs of consecutive pages in ascending `keep`."""
+    starts = np.concatenate([[0], np.cumsum(_padded_lens(page_lens))]).astype(np.int64)
+    return [(int(starts[first]), int(starts[last + 1])) for first, last in _runs(keep)]
+
+
 # ---- argument checks of the device calls: tensor metadata only (no value is read, nothing synchronises or is allocated),
 # so a tensor the library would read past its end or in the wrong format is refused with ValueError before any launch
 def _check_queries(q_dev: torch.Tensor, q_lens: Sequence[int], device: torch.device) -> int:
@@ -192,6 +198,25 @@ class DeviceBlock:
             if mapped:
                 self.tensor = torch.as_tensor(_CudaBytes(nat.lib.b200ms_block_ptr(self.ptr), mapped), device=self.device)
 
+    @staticmethod
+    def resized(block: Optional["DeviceBlock"], handle: "nat.Handle", device: torch.device, nbytes: int) -> "DeviceBlock":
+        """`block` -- or, when None, a new block -- backing `nbytes`; a new block whose resize is refused is freed again."""
+        new = DeviceBlock(handle, device) if block is None else block
+        try:
+            new.resize(nbytes)
+        except Exception:
+            if block is None:
+                new.free()
+            raise
+        return new
+
+    def rows(self, row_bytes: int) -> Optional[torch.Tensor]:
+        """The backed bytes as whole rows: uint8 [backed // row_bytes, row_bytes], None while nothing is backed."""
+        if self.tensor is None:
+            return None
+        n = self.tensor.numel() // row_bytes
+        return self.tensor[: n * row_bytes].view(n, row_bytes)
+
     def free(self):
         self.tensor = None
         if self.ptr and self.handle.ptr:  # a closed handle has released its blocks already
@@ -203,6 +228,22 @@ class DeviceBlock:
             self.free()
         except Exception:
             pass
+
+
+def _compact_rows(h: "nat.Handle", device: torch.device, rows: torch.Tensor, row_bytes: int,
+                  runs: Sequence[Tuple[int, int]]) -> None:
+    """Move the row ranges [a, b) of `runs` (ascending) down to the front of `rows`, in place on the GPU, with one
+    b200ms_compact_rows call.  Returns once torch's stream is idle: the block's shrink that follows unmaps the freed tail
+    after the handle's calls, but copies torch itself queued on those rows (append_packed, the FDE rows' copies) are only
+    known to this stream."""
+    run_start = np.array([a for a, _ in runs], dtype=np.int64)
+    run_rows = np.array([b - a for a, b in runs], dtype=np.int64)
+    stream = ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+    with torch.cuda.device(device):
+        h.check(nat.lib.b200ms_compact_rows(h.ptr, _vp(rows), row_bytes, run_start.ctypes.data_as(nat.i64p),
+                                            run_rows.ctypes.data_as(nat.i64p), len(runs), stream),
+                "b200ms_compact_rows")
+    torch.cuda.current_stream(device).synchronize()
 
 
 class MaxSimIndex:
@@ -331,15 +372,7 @@ class MaxSimIndex:
         """HBM tier: back exactly `rows` rows (rounded up to whole chunks) of the index's block; the rows that stay keep
         their contents and address.  Rows held in a caller's tensor (``adopt_packed``) move into a block of their own
         first, which is the one copy such a corpus ever makes."""
-        block = self._block
-        if block is None:
-            block = DeviceBlock(self.h, self.device)
-        try:
-            block.resize(rows * self.row_bytes)
-        except Exception:
-            if self._block is None:
-                block.free()
-            raise
+        block = DeviceBlock.resized(self._block, self.h, self.device, rows * self.row_bytes)
         if self._block is None and self._buf is not None and self._rows:
             block.tensor[: self._rows * self.row_bytes].copy_(self._buf[: self._rows * self.row_bytes])
         self._block, self._buf = block, block.tensor
@@ -521,10 +554,8 @@ class MaxSimIndex:
         on the host tier with one forward (overlap-safe) memmove per run."""
         keep = [int(p) for p in keep]
         lens = self._page_lens
-        pad = _padded_lens(lens)
-        starts = np.concatenate([[0], np.cumsum(pad)]).astype(np.int64)
-        new_rows = int(pad[keep].sum())
-        runs = [(int(starts[first]), int(starts[last + 1])) for first, last in _runs(keep)]  # row ranges [a, b)
+        runs = _row_runs(lens, keep)
+        new_rows = sum(b - a for a, b in runs)
         if self.tier == "host":
             self._host_barrier()
             base, dst = self._buf.data_ptr(), 0
@@ -535,17 +566,7 @@ class MaxSimIndex:
         elif self._buf is not None:
             if self._block is None:  # a caller's tensor (adopt_packed) is not compacted behind the caller's back
                 self._resize_block(self._rows)
-            run_start = np.array([a for a, _ in runs], dtype=np.int64)
-            run_rows = np.array([b - a for a, b in runs], dtype=np.int64)
-            with torch.cuda.device(self.device):
-                self.h.check(
-                    nat.lib.b200ms_compact_rows(self.h.ptr, _vp(self._buf), self.row_bytes,
-                                                run_start.ctypes.data_as(nat.i64p), run_rows.ctypes.data_as(nat.i64p),
-                                                len(runs), self._stream()),
-                    "b200ms_compact_rows")
-            # the shrink unmaps the freed tail once the handle's calls are over; copies torch itself queued on those rows
-            # (append_packed) are only known to this stream
-            torch.cuda.current_stream(self.device).synchronize()
+            _compact_rows(self.h, self.device, self._buf, self.row_bytes, runs)
             self._resize_block(new_rows)
         self._rows = new_rows
         self._page_lens = [lens[p] for p in keep]

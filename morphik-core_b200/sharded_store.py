@@ -402,9 +402,7 @@ class ShardedB200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                                   "build_chunks_ms": (t2 - t1) * 1e3, "total_ms": (t2 - t0) * 1e3}
         ev = self._stage_events
         if self._two_stage is not None and ev is not None:  # the reference's stage names (fast_multivector_store.py:523-605)
-            self.last_query_timing.update(encode_query_ms=ev[0].elapsed_time(ev[1]), ns_query_ms=ev[1].elapsed_time(ev[2]),
-                                          load_multivectors_ms=0.0, rerank_scoring_ms=ev[2].elapsed_time(ev[3]),
-                                          load_contents_ms=0.0)
+            self.last_query_timing.update(self._two_stage.stage_timing_ms(ev), load_contents_ms=0.0)
         return out
 
     async def get_chunks_by_id(self, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,

@@ -223,7 +223,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         # An int: the same two-stage search with the asymmetric sign scan as its first stage (signs.SignTwoStageIndex:
         # full-precision queries against an HBM sign copy of every page) instead of the FDE scan.
         self.sign_candidates = sign_candidates
-        self._two_stage = None
+        self._n_candidates = int(fde_candidates or sign_candidates or 0)
+        self._two_stage = None  # the first stage with the rerank behind it (two_stage.TwoStageSearch) in two-stage mode
         # > 0: reproduce colpali_engine score_multi_vector's zero-padding quirk with this batch size (128 upstream): a page
         # shorter than the longest page of its scoring batch scores sum_t max(max_r <q_t,d_r>, 0)  (SURVEY App. A.2;
         # processing_colpali.py:350-362).  0 (default) = the clean MaxSim.
@@ -242,32 +243,24 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         if self._index is None:
             from .index import MaxSimIndex  # raises when libb200ms.so or the GPU is missing: no silent fallback
 
-            if self.fde_candidates:
-                from .fde import TwoStageIndex
-
-                self._two_stage = TwoStageIndex(device=self.device, dtype=self.mode, tier=self.corpus_tier)
-                self._index = self._two_stage.index
-            elif self.sign_candidates:
-                from .signs import SignTwoStageIndex
-
-                self._two_stage = SignTwoStageIndex(device=self.device, dtype=self.mode, tier=self.corpus_tier)
+            if self._n_candidates:
+                self._two_stage = self._first_stage(index=None, device=self.device, dtype=self.mode, tier=self.corpus_tier)
                 self._index = self._two_stage.index
             else:
                 self._index = MaxSimIndex(device=self.device, dtype=self.mode)
-        elif self.fde_candidates and self._two_stage is None and hasattr(self._index, "h"):
-            # a loaded / injected CUDA index in two-stage mode: rebuild the FDE matrix from its packed rows
-            from .fde import TwoStageIndex
-
-            self._two_stage = TwoStageIndex(index=self._index)
-            self._two_stage.rebuild_from_index()
-        elif self.sign_candidates and self._two_stage is None and hasattr(self._index, "h"):
-            from .signs import SignTwoStageIndex  # likewise the sign rows
-
-            self._two_stage = SignTwoStageIndex(index=self._index)
+        elif self._n_candidates and self._two_stage is None and hasattr(self._index, "h"):
+            # a loaded / injected CUDA index in two-stage mode: rebuild the first stage's rows from its packed rows
+            self._two_stage = self._first_stage(index=self._index)
             self._two_stage.rebuild_from_index()
         if self.zero_pad_compat and hasattr(self._index, "set_option"):
             self._index.set_option("zero_pad_compat", self.zero_pad_compat)
         return True
+
+    def _first_stage(self, **kw):
+        from .fde import TwoStageIndex
+        from .signs import SignTwoStageIndex
+
+        return (TwoStageIndex if self.fde_candidates else SignTwoStageIndex)(**kw)
 
     def close(self) -> None:
         if self._index is not None and hasattr(self._index, "close"):
@@ -310,15 +303,11 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 assert pid == first + i, "catalogue and device corpus out of step"
                 recs.append(rec)
             if self._journal is not None:  # durable store: this call becomes one append-only segment
-                self._journal.log_add(self._index, first, n, [dataclasses.asdict(r) for r in recs], self._fde_rows(first, n))
+                self._journal.log_add(self._index, first, n, [dataclasses.asdict(r) for r in recs], self._journal_rows(first, n))
 
-    def _fde_rows(self, first: int, n: int):
-        """What a journal segment persists of the first stage: the FDE rows (sign rows are derived again on replay)."""
-        return self._two_stage.fde_rows(first, n) if self._two_stage is not None and self.fde_candidates else None
-
-    @property
-    def _n_candidates(self) -> int:
-        return int(self.fde_candidates or self.sign_candidates)
+    def _journal_rows(self, first: int, n: int):
+        """What a journal segment persists of the first stage (FDE rows; sign rows are derived again on replay)."""
+        return self._two_stage.journal_rows(first, n) if self._two_stage is not None else None
 
     # ------------------------------------------------------------------ read path
     async def query_similar(self, query_embedding, k: int, doc_ids: Optional[List[str]] = None,
@@ -404,14 +393,8 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             t3 = time.perf_counter()
         self.last_query_timing = {"prepare_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3,
                                   "build_chunks_ms": (t3 - t2) * 1e3, "total_ms": (t3 - t0) * 1e3}
-        if self._two_stage is not None and self.sign_candidates:
-            st = self._two_stage.last_timing_ms
-            self.last_query_timing.update({k: float(st.get(k, 0.0)) for k in (
-                "sign_candidates_ms", "maxsim_rerank_ms", "load_multivectors_ms", "rerank_scoring_ms")})
-        elif self._two_stage is not None:  # the reference's stage names (fast_multivector_store.py:523,534,550,574,589,604)
-            st = self._two_stage.last_timing_ms
-            self.last_query_timing.update(encode_query_ms=st.get("encode_query_ms", 0.0), ns_query_ms=st.get("ns_query_ms", 0.0),
-                                          load_multivectors_ms=0.0, rerank_scoring_ms=st.get("rerank_scoring_ms", 0.0),
+        if self._two_stage is not None:  # the reference's stage names (fast_multivector_store.py:523,534,550,574,589,604)
+            self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()},
                                           load_contents_ms=0.0)
         logger.debug("query_similar timing %s", json.dumps(self.last_query_timing))
         return out
@@ -565,7 +548,7 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 self._journal.reset()
                 if len(self.catalog):
                     self._journal.log_add(self._index, 0, len(self.catalog), [dataclasses.asdict(r) for r in self.catalog.records],
-                                          self._fde_rows(0, len(self.catalog)))
+                                          self._journal_rows(0, len(self.catalog)))
 
     @classmethod
     def load(cls, directory: str, device: int = 0, **kw) -> "B200MultiVectorStore":
@@ -588,10 +571,6 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         """Durable store: replay ``directory``'s journal (segments appended by earlier store_embeddings calls, tombstones of
         earlier deletes -- fast_multivector_store.py:673-707 / multi_vector_store.py:929-933 persist the same two operations)
         and keep journaling.  Nothing is ever rewritten in place; ``save(directory)`` checkpoints."""
-        import os
-
-        import torch
-
         from . import shardfile
 
         journal = shardfile.StoreJournal(directory)
@@ -608,18 +587,14 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 with open(cat) as f:
                     for line in f:
                         store.catalog.add(PageRecord(**json.loads(line)))
-                if store._two_stage is not None and store.fde_candidates:
-                    if os.path.exists(fde):
-                        blob = torch.load(fde)
-                        store._two_stage.append_fde_rows(blob["rows"].view(torch.bfloat16), blob["inv"])
-                    else:
-                        store._two_stage.rebuild_from_index()
+                if store._two_stage is not None:
+                    store._two_stage.replay_segment(fde)
                 if store._index.n_pages - first != int(op["pages"]) or len(store.catalog) != store._index.n_pages:
                     raise ValueError(f"{seg}: segment and journal disagree on the page count")
             elif op["op"] == "delete":
                 store.catalog.delete_document(op["document_id"])
-        if store._two_stage is not None and store.sign_candidates:
-            store._two_stage.rebuild_from_index()  # once, over every replayed segment
+        if store._two_stage is not None:
+            store._two_stage.replay_done()
         with store._lock:
             if store.catalog.dead_fraction > store.compact_dead_fraction:
                 store._compact_locked()

@@ -1,0 +1,146 @@
+"""Two-stage search: a first stage (``fde.TwoStageIndex``, ``signs.SignTwoStageIndex``) picks candidate pages per query
+from side data it appends, rebuilds and compacts with the corpus; ``TwoStageSearch`` reranks them by exact MaxSim."""
+from __future__ import annotations
+
+from typing import Dict, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import _native as nat
+from .index import MaxSimIndex, _check_device_masks, _host_mask_to_device
+
+
+def _host(t: torch.Tensor, shape: Tuple[int, ...], fill) -> np.ndarray:
+    """Device results [n_q, kk, ...] -> host array of `shape` ([n_q, k, ...], k >= kk) and their dtype, `fill` past kk."""
+    a = t.cpu().numpy()
+    out = np.full(shape, fill, dtype=a.dtype)
+    out[:, :a.shape[1]] = a
+    return out
+
+
+class TwoStageSearch:
+    # last_timing_ms names of the first stage's windows: name -> (first event, last event) of search_device's events
+    STAGE_TIMES: Dict[str, Tuple[int, int]] = {}
+
+    def __init__(self, index: MaxSimIndex):
+        self.index = index
+        self.device = index.device
+        self.last_timing_ms: Dict[str, float] = {}
+
+    @property
+    def n_pages(self) -> int:
+        return self.index.n_pages
+
+    # ------------------------------------------------------------------ what a first stage supplies
+    def _encode(self, queries: Sequence, staged: Optional[Tuple[torch.Tensor, int, Sequence[int]]]):
+        """The queries as the scan takes them (part of the query preparation window): here their staged rows.  `staged`:
+        (rows, dtype code, lengths) when the caller staged them already for the rerank, else None."""
+        return staged[0] if staged else self.index._stage_rows(list(queries))[0]
+
+    def _scan(self, q, lens: Sequence[int], n_cand: int, mask: Optional[torch.Tensor]):
+        """Top n_cand pages per query among those `mask` (checked, one row for every query) allows: device tensors (scores
+        float32 [n_q, n_cand], page ids int64 [n_q, n_cand] (-1 padded), counts int32 [n_q])."""
+        raise NotImplementedError
+
+    def journal_rows(self, first: int, n: int):
+        """What a journal segment persists of the first stage for pages [first, first + n); None: nothing."""
+        return None
+
+    def replay_segment(self, path: str) -> None:
+        """Journal replay: the segment just loaded into the index had its first-stage rows persisted at `path`, if at all."""
+
+    def replay_done(self) -> None:
+        """Journal replay: every segment is loaded."""
+
+    # ------------------------------------------------------------------ the two-stage search
+    def _mask(self, allow_mask_dev: Optional[torch.Tensor], n_q: int) -> Optional[torch.Tensor]:
+        return _check_device_masks(allow_mask_dev, None, n_q, self.n_pages, self.device)[0]
+
+    def _prepare(self, queries: Sequence):
+        """Stages the query rows once: (rows, lengths, the rows as the scan takes them)."""
+        src, src_dtype = self.index._stage_rows(list(queries))
+        lens = [int(q.shape[0]) for q in queries]
+        return src, lens, self._encode(queries, (src, src_dtype, lens))
+
+    def _n_cand(self, want: int) -> int:
+        return int(min(want, nat.MAX_K, max(self.n_pages, 1)))
+
+    def candidates(self, queries: Sequence, n_candidates: int, allow_mask_dev: Optional[torch.Tensor] = None):
+        """First stage only: (candidate page ids int64 [n_q, n_candidates] (-1 padded), first-stage scores, counts) on the
+        device.  allow_mask_dev: optional uint32 page bitmask (the doc_ids filter, applied BEFORE candidate selection like the
+        reference's Turbopuffer filter, fast_multivector_store.py:527)."""
+        mask = self._mask(allow_mask_dev, len(queries))
+        q = self._encode(queries, None)  # no rerank follows: the rows are staged (at most) once, for the scan
+        ts, ti, tc = self._scan(q, [int(x.shape[0]) for x in queries], int(min(n_candidates, nat.MAX_K)), mask)
+        return ti, ts, tc
+
+    def rerank(self, query, cand_ids: torch.Tensor, k: int):
+        """Exact MaxSim of ONE query over the candidate pages (device int64 [n_cand], -1 = unused) -> top-k."""
+        src, _ = self.index._stage_rows([query])
+        return self.index.rerank(src, [int(query.shape[0])], cand_ids.contiguous(), k)
+
+    def search_device(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
+                      id_base: int = 0):
+        """Two-stage search, everything on the device and asynchronous: max(n_candidates, k) candidates per query (at most
+        MAX_K) from ONE first-stage scan for the whole batch -> ONE batched rerank call (each query against its own list) ->
+        top-k.  Returns device tensors (scores [n_q,kk], page ids + id_base [n_q,kk], counts [n_q]) and the CUDA events that
+        bracket the stages: query preparation, candidate scan + top-k, rerank."""
+        mask = self._mask(allow_mask_dev, len(queries))
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        ev[0].record()
+        src, lens, q = self._prepare(queries)
+        ev[1].record()
+        _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k)), mask)
+        ev[2].record()
+        ts, ti, tc = self.index.rerank_batch(src, lens, ci, k)
+        if id_base:
+            ti = torch.where(ti >= 0, ti + int(id_base), ti)
+        ev[3].record()
+        return ts, ti, tc, ev
+
+    def stage_timing_ms(self, ev) -> Dict[str, float]:
+        """Stage times of a finished search_device call from its events: the first stage's windows, maxsim_rerank_ms and,
+        of the rerank, load_multivectors_ms (the host tier's PCIe gather; 0 in HBM) and rerank_scoring_ms -- the reference's
+        stage names (fast_multivector_store.py:523,534,550,574)."""
+        out = {name: ev[a].elapsed_time(ev[b]) for name, (a, b) in self.STAGE_TIMES.items()}
+        rerank_ms = ev[2].elapsed_time(ev[3])
+        gather = self.index.gather_stats() if self.index.tier == "host" else {"ms": 0.0, "bytes": 0, "unique_pages": 0}
+        out.update(maxsim_rerank_ms=rerank_ms, load_multivectors_ms=gather["ms"], rerank_scoring_ms=rerank_ms - gather["ms"],
+                   gather_bytes=gather["bytes"], gather_pages=gather["unique_pages"])
+        return out
+
+    def search(self, queries: Sequence, k: int, n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
+        """Two-stage search with a host allow mask (uint32 words, restricting both stages); synchronous.  Returns host arrays
+        (scores [n_q,k], page ids [n_q,k], counts [n_q]) and fills last_timing_ms (stage_timing_ms)."""
+        n_q = len(queries)
+        mask_dev = _host_mask_to_device(allow_mask, self.n_pages, self.device)
+        ts, ti, tc, ev = self.search_device(queries, k, n_candidates, mask_dev)
+        torch.cuda.synchronize(self.device)
+        out = _host(ts, (n_q, k), -np.inf), _host(ti, (n_q, k), -1), tc.cpu().numpy().astype(np.int32)
+        self.last_timing_ms = self.stage_timing_ms(ev)
+        return out
+
+    def search_docs_device(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                           n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None):
+        """Two-stage search grouped by document: max(n_candidates, k * per_doc) candidates per query (at most MAX_K), then
+        MaxSimIndex.rerank_docs_batch over them.  Returns its four device tensors."""
+        mask = self._mask(allow_mask_dev, len(queries))
+        src, lens, q = self._prepare(queries)
+        _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k * per_doc)), mask)
+        return self.index.rerank_docs_batch(src, lens, ci, k, per_doc, page_doc_dev, n_docs)
+
+    def search_docs(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                    n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
+        """search_docs_device with a host allow mask (uint32 words, restricting both stages); synchronous, returns host
+        arrays (scores [n_q,k,per_doc], page ids [n_q,k,per_doc], pages per document [n_q,k], documents [n_q])."""
+        mask_dev = _host_mask_to_device(allow_mask, self.n_pages, self.device)
+        ts, ti, pc, dc = self.search_docs_device(queries, k, per_doc, page_doc_dev, n_docs, n_candidates, mask_dev)
+        n_q = len(queries)
+        return (_host(ts, (n_q, k, per_doc), -np.inf), _host(ti, (n_q, k, per_doc), -1), _host(pc, (n_q, k), 0),
+                dc.cpu().numpy())
+
+    def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
+        """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
+        the same exact scorer that ranked them."""
+        return self.index.explain(queries, page_ids, map_rows)
