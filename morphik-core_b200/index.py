@@ -390,18 +390,19 @@ class MaxSimIndex:
         if self.tier == "host" and self._block is not None:
             torch.cuda.synchronize(self.device)
 
-    def host_tail(self, nbytes: int) -> np.ndarray:
-        """Host tier: writable uint8 view of the `nbytes` past the used rows (grown to fit) -- a shard file is read straight
-        into it; ``commit_rows`` then appends the pages it holds."""
-        if self.tier != "host":
-            raise ValueError("host_tail needs a host-tier index")
-        self._grow(self._rows + (int(nbytes) + self.row_bytes - 1) // self.row_bytes)
+    def tail(self, nbytes: int) -> torch.Tensor:
+        """Writable uint8 view of the `nbytes` just past the used rows, grown to fit: of the pinned block on the host tier
+        (a CPU tensor), of the device block on the HBM tier.  ``commit_rows`` appends the packed pages written into it."""
+        nbytes = int(nbytes)
+        self._grow(self._rows + -(-nbytes // self.row_bytes))
         self._host_barrier()
+        if self._buf is None:  # nothing backed and nothing asked for
+            return torch.empty(0, dtype=torch.uint8, device=self.device if self.tier == "hbm" else "cpu")
         o = self._rows * self.row_bytes
-        return self._buf[o:o + int(nbytes)].numpy()
+        return self._buf[o:o + nbytes]
 
     def commit_rows(self, page_lens: Sequence[int]) -> Tuple[int, int]:
-        """Append pages whose packed rows were already written past the used rows (``host_tail``)."""
+        """Append pages whose packed rows were already written into ``tail``.  Returns (first id, count)."""
         lens = [int(x) for x in page_lens]
         need = int(nat.lib.b200ms_padded_rows(nat.i32_array(lens), len(lens)))
         if self._rows + need > self._cap_rows:
@@ -418,35 +419,28 @@ class MaxSimIndex:
         Mirrors the write half of store_embeddings (multi_vector_store.py:681-703 quantise+insert;
         fast_multivector_store.py:673-707 np.save of float32): one H2D copy of the ragged rows, one pack kernel.
         """
-        first = self.n_pages
         if len(pages) == 0:
-            return first, 0
+            return self.n_pages, 0
         lens = [int(p.shape[0]) for p in pages]
         for p in pages:
             if p.ndim != 2 or p.shape[1] != nat.DIM:
                 raise ValueError(f"page embeddings must be [P,{nat.DIM}], got {tuple(p.shape)}")
         src, src_dtype = self._stage_rows(pages)
         lens_c = nat.i32_array(lens)
-        add_rows = int(nat.lib.b200ms_padded_rows(lens_c, len(lens)))
-        self._grow(self._rows + add_rows)
-        o = self._rows * self.row_bytes
+        nbytes = int(nat.lib.b200ms_padded_rows(lens_c, len(lens))) * self.row_bytes
+        dst = self.tail(nbytes)
         # host tier: pack on the GPU into a device temporary, then one D2H copy into the block
-        # (an HBM index none of whose pages has a row owns no memory yet: the call then needs a destination all the same)
-        dst = self._buf[o:] if self.tier == "hbm" and self._buf is not None else torch.empty(
-            max(add_rows * self.row_bytes, 1), dtype=torch.uint8, device=self.device)
+        # (pages none of which has a row have no tail: the call then needs a destination all the same)
+        packed = dst if dst.is_cuda and nbytes else torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
             self.h.check(
-                nat.lib.b200ms_pack_pages(self.h.ptr, _vp(src), src_dtype, lens_c, len(lens), _vp(dst), self.dtype,
+                nat.lib.b200ms_pack_pages(self.h.ptr, _vp(src), src_dtype, lens_c, len(lens), _vp(packed), self.dtype,
                                           ctypes.c_float(self.i8_scale), self._stream()),
                 "b200ms_pack_pages",
             )
-            if self.tier == "host" and add_rows:
-                self._host_barrier()
-                self._buf[o:o + add_rows * self.row_bytes].copy_(dst[: add_rows * self.row_bytes])
-        self._rows += add_rows
-        self._page_lens.extend(lens)
-        self._attached = False
-        return first, len(lens)
+        if packed is not dst:
+            dst.copy_(packed[:nbytes])
+        return self.commit_rows(lens)
 
     def _stage_rows(self, mats: Sequence[ArrayLike]) -> Tuple[torch.Tensor, int]:
         """Concatenate ragged [n_i,128] matrices into one device tensor (float32 or bfloat16)."""
@@ -504,22 +498,15 @@ class MaxSimIndex:
         self._attached = False
 
     def append_packed(self, rows: torch.Tensor, page_lens: Sequence[int]) -> Tuple[int, int]:
-        """Append already packed rows (uint8 view of the corpus dtype's layout, pages padded to 32 rows) -- a shard-file
-        segment -- with one device copy.  Returns (first id, count)."""
+        """Append already packed rows (uint8 view of the corpus dtype's layout, pages padded to 32 rows) with one copy.
+        Returns (first id, count)."""
         lens = [int(x) for x in page_lens]
         flat = rows.view(torch.uint8).reshape(-1)
-        need = int(nat.lib.b200ms_padded_rows(nat.i32_array(lens), len(lens)))
-        if flat.numel() < need * self.row_bytes:
+        nbytes = int(nat.lib.b200ms_padded_rows(nat.i32_array(lens), len(lens))) * self.row_bytes
+        if flat.numel() < nbytes:
             raise ValueError("packed buffer smaller than the page lengths imply")
-        first = self.n_pages
-        self._grow(self._rows + need)
-        self._host_barrier()
-        if need:
-            self._buf[self._rows * self.row_bytes:(self._rows + need) * self.row_bytes].copy_(flat[: need * self.row_bytes])
-        self._rows += need
-        self._page_lens.extend(lens)
-        self._attached = False
-        return first, len(lens)
+        self.tail(nbytes).copy_(flat[:nbytes])
+        return self.commit_rows(lens)
 
     def page_row_range(self, first: int, n: int) -> Tuple[int, int]:
         """Padded row range [r0, r1) that pages [first, first+n) occupy in the packed buffer."""

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .index import MaxSimIndex, _aligned_bytes
+from .index import MaxSimIndex
 
 MAGIC = "B2MSHARD"
 HEADER_BYTES = 4096
@@ -71,9 +71,9 @@ def read_header(path: str) -> Tuple[dict, np.ndarray, int]:
 
 
 def load_index(path: str, device: int = 0, into: Optional[MaxSimIndex] = None, tier: str = "hbm") -> MaxSimIndex:
-    """Read a shard file straight into a 1024-byte-aligned device buffer and adopt it (no repacking); with ``into`` the
-    pages are APPENDED to an existing index of the same dtype (journal segments).  A host-tier index (``tier="host"``, or
-    ``into`` of that tier) reads the rows straight into its pinned host block, sized from the header, with no device copy."""
+    """Read a shard file into the index's own block (no repacking, no second copy of the corpus): a new index of the file's
+    dtype on tier `tier`, or with ``into`` an existing index of the same dtype that the pages are APPENDED to (journal
+    segments).  Host-tier rows are read straight into the pinned block; device rows go through two pinned staging buffers."""
     header, lens, payload_off = read_header(path)
     if into is not None and (into.dtype_name != header["dtype"] or float(into.i8_scale) != float(header["i8_scale"])):
         raise ValueError(f"{path}: segment dtype/scale differs from the index it is appended to")
@@ -84,37 +84,26 @@ def load_index(path: str, device: int = 0, into: Optional[MaxSimIndex] = None, t
         raise ValueError(f"{path}: page lengths do not match the row count")
     if os.path.getsize(path) < payload_off + total:
         raise ValueError(f"{path}: truncated payload")
-    if index.tier == "host":
-        index.reserve_rows(index.n_rows_padded + header["n_rows_padded"])
-        dst = memoryview(index.host_tail(total))
-        with open(path, "rb") as f:
-            f.seek(payload_off)
-            for o in range(0, total, CHUNK_BYTES):
-                n = min(CHUNK_BYTES, total - o)
-                if f.readinto(dst[o:o + n]) != n:
-                    raise ValueError(f"{path}: short read")
-        index.commit_rows(lens.tolist())
-        return index
-    buf = _aligned_bytes(total, index.device)
-    stages = [torch.empty(min(CHUNK_BYTES, max(total, 1)), dtype=torch.uint8).pin_memory() for _ in range(2)]
+    index.reserve_rows(index.n_rows_padded + header["n_rows_padded"])
+    dst = index.tail(total)
+    staged = dst.is_cuda  # double-buffered: chunk i+1 is read into one staging buffer while chunk i copies from the other
+    stages = [torch.empty(min(CHUNK_BYTES, max(total, 1)), dtype=torch.uint8).pin_memory()
+              for _ in range(2 if staged else 0)]
     events = [torch.cuda.Event(), torch.cuda.Event()]
     with open(path, "rb") as f, torch.cuda.device(index.device):
         f.seek(payload_off)
-        for i, o in enumerate(range(0, total, CHUNK_BYTES)):  # double-buffered: read chunk i+1 while chunk i is in flight
+        for i, o in enumerate(range(0, total, CHUNK_BYTES)):
             n = min(CHUNK_BYTES, total - o)
-            st = stages[i & 1]
-            if i >= 2:
+            if staged and i >= 2:
                 events[i & 1].synchronize()
-            got = f.readinto(memoryview(st.numpy())[:n])
-            if got != n:
+            target = stages[i & 1][:n] if staged else dst[o:o + n]
+            if f.readinto(memoryview(target.numpy())) != n:
                 raise ValueError(f"{path}: short read")
-            buf[o:o + n].copy_(st[:n], non_blocking=True)
-            events[i & 1].record()
+            if staged:
+                dst[o:o + n].copy_(target, non_blocking=True)
+                events[i & 1].record()
         torch.cuda.current_stream().synchronize()
-    if into is not None:
-        index.append_packed(buf, lens.tolist())
-    else:
-        index.adopt_packed(buf, lens.tolist())
+    index.commit_rows(lens.tolist())
     return index
 
 

@@ -576,9 +576,9 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         journal = shardfile.StoreJournal(directory)
         store = cls(device=device, mode=mode, **kw)
         ops = journal.read_ops()
-        if getattr(store._index, "tier", "hbm") == "host":  # size the host block once from the segment headers
-            segs = [shardfile.read_header(journal.segment_files(op["seq"])[0])[0] for op in ops if op["op"] == "segment"]
-            store._index.reserve_rows(sum(int(h["n_rows_padded"]) for h in segs))
+        # size the block once, from the segment headers
+        segs = [shardfile.read_header(journal.segment_files(op["seq"])[0])[0] for op in ops if op["op"] == "segment"]
+        store._index.reserve_rows(sum(int(h["n_rows_padded"]) for h in segs))
         for op in ops:
             if op["op"] == "segment":
                 seg, cat, fde = journal.segment_files(op["seq"])

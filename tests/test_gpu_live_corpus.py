@@ -7,10 +7,14 @@
     memory without taking memory from anyone.
   * MaxSimIndex / TwoStageIndex: an index grown page by page equals one sized up front; a compacted index equals one built
     from the kept pages alone -- rows, scores, top-k.
-  * Free device memory around growth and compaction: the block lives outside torch's allocator, so the tests sample
-    torch.cuda.mem_get_info.  Other jobs may share the card: the bounds carry a tolerance of 256 MiB.
+  * Shard files on both tiers, fresh and appended to an index, empty ones too: read into the index's own block, equal to
+    the index they were saved from.
+  * Free device memory around growth and compaction, and around a store's open / load: the block lives outside torch's
+    allocator, so the tests sample torch.cuda.mem_get_info.  Other jobs may share the card: the bounds carry a tolerance of
+    256 MiB.
   * One stream-order case: a search in flight on one stream, a compaction, a search after it.
 """
+import asyncio
 import ctypes
 
 import numpy as np
@@ -24,8 +28,11 @@ if not torch.cuda.is_available():  # pragma: no cover - the gpu marker normally 
 
 import compact_model as cm  # noqa: E402
 from morphik_core_b200 import _native as nat  # noqa: E402
+from morphik_core_b200 import shardfile  # noqa: E402
 from morphik_core_b200.fde import FixedDimensionalEncodingConfig, TwoStageIndex  # noqa: E402
 from morphik_core_b200.index import DeviceBlock, MaxSimIndex, _aligned_bytes  # noqa: E402
+from morphik_core_b200.models import DocumentChunk  # noqa: E402
+from morphik_core_b200.store import B200MultiVectorStore  # noqa: E402
 from test_compact_plan_cpu import page_runs, patterns  # noqa: E402
 
 DEV = torch.device("cuda", 0)
@@ -363,6 +370,76 @@ def test_two_stage_index_grows_and_compacts_in_place(pattern):
         t.index.close()
 
 
+# ------------------------------------------------------------------------------------------------ shard files
+def page_scores(idx, queries, tier):
+    """What an index scores: score_matrix and search_device on the HBM tier, rerank_batch over every page on the host tier
+    (the only search it has)."""
+    if tier == "hbm":
+        return [torch.from_numpy(idx.score_matrix(queries)), *search(idx, queries)]
+    cand = torch.arange(idx.n_pages, device=DEV).repeat(len(queries), 1)
+    out = idx.rerank_batch(torch.cat(queries).contiguous(), [int(x.shape[0]) for x in queries], cand, idx.n_pages)
+    torch.cuda.synchronize(DEV)
+    return [t.cpu() for t in out]
+
+
+def assert_loaded(got, want, queries, tier):
+    assert got.tier == tier
+    assert torch.equal(got.packed_rows().cpu(), want.packed_rows().cpu())
+    assert np.array_equal(got.page_lens, want.page_lens)
+    for x, y in zip(page_scores(got, queries, tier), page_scores(want, queries, tier)):
+        assert torch.equal(x, y)
+
+
+@pytest.mark.parametrize("tier", ["hbm", "host"])
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_shard_file_is_read_into_the_index_block(tmp_path, dtype, tier):
+    """Loaded fresh and appended (into=) to an index that holds pages: the same rows, page lengths and scores as the
+    index it was saved from; on HBM the rows sit in the index's DeviceBlock, which keeps its address as the index grows
+    and compacts."""
+    pages = make_pages(40, seed=81)  # one page of 0 rows, lengths that are not multiples of 32
+    head = make_pages(9, seed=82)
+    queries = make_queries(83)
+    saved = MaxSimIndex(dtype=dtype)
+    saved.add_pages(pages)
+    path = str(tmp_path / "pages.b2ms")
+    shardfile.save_index(saved, path)
+    both = MaxSimIndex(dtype=dtype)
+    both.add_pages(head + pages)
+    fresh = shardfile.load_index(path, tier=tier)
+    appended = MaxSimIndex(dtype=dtype, tier=tier)
+    appended.add_pages(head)
+    assert shardfile.load_index(path, into=appended) is appended
+    assert_loaded(fresh, saved, queries, tier)
+    assert_loaded(appended, both, queries, tier)
+    if tier == "hbm":
+        for idx in (fresh, appended):
+            assert isinstance(idx._block, DeviceBlock)
+            base = idx._buf.data_ptr()
+            idx.add_pages(pages[:5])
+            idx.compact(list(range(1, idx.n_pages, 2)))
+            assert idx._buf.data_ptr() == base
+    for idx in (saved, both, fresh, appended):
+        idx.close()
+
+
+@pytest.mark.parametrize("tier", ["hbm", "host"])
+def test_empty_shard_file_loads_and_the_index_takes_pages(tmp_path, tier):
+    path = str(tmp_path / "empty.b2ms")
+    empty = MaxSimIndex(dtype="bf16")
+    shardfile.save_index(empty, path)
+    pages = make_pages(12, seed=91)
+    queries = make_queries(92)
+    want = MaxSimIndex(dtype="bf16")
+    want.add_pages(pages)
+    idx = shardfile.load_index(path, tier=tier)
+    assert idx.n_pages == 0
+    idx.add_pages(pages)
+    shardfile.load_index(path, into=idx)
+    assert_loaded(idx, want, queries, tier)
+    for i in (empty, want, idx):
+        i.close()
+
+
 # ------------------------------------------------------------------------------------------------ free device memory
 def test_growth_and_compaction_never_hold_a_second_copy():
     """1.5 GiB of bf16 rows ingested 64 MiB at a time, 30 % of its pages deleted, compacted.  Free device memory (sampled
@@ -400,6 +477,53 @@ def test_growth_and_compaction_never_hold_a_second_copy():
     assert dead - bounce - CHUNK - TOL <= after - full <= dead + TOL  # the dead rows are back with the driver
     assert torch.cuda.memory_allocated(DEV) - torch_start < corpus // 2  # and none of the corpus sits in torch's allocator
     idx.close()
+
+
+def test_reopened_and_loaded_stores_never_hold_a_second_copy(tmp_path):
+    """A durable bf16 store of 1.5 GiB, checkpointed as one base segment, then opened (journal replay), ingested into and
+    compacted; and the same checkpoint loaded and ingested into.  The rows are read into the index's block: torch's
+    allocator never holds more than an ingest call's temporaries, and free device memory (sampled after every call,
+    synchronised) drops by at most the corpus, one chunk, the pack temporaries and the compaction's bounce buffer."""
+    page_rows, pages_per_call, calls, per_doc = 1024, 1024, 6, 64
+    g = torch.Generator(device=DEV)
+    g.manual_seed(101)
+
+    def chunks(first, n):
+        rows = torch.randn((n * page_rows, nat.DIM), generator=g, device=DEV)
+        rows = (rows / rows.norm(dim=1, keepdim=True)).bfloat16()
+        return [DocumentChunk(document_id=f"d{(first + i) // per_doc}", content="", chunk_number=(first + i) % per_doc,
+                              metadata={}, embedding=e) for i, e in enumerate(rows.split(page_rows))]
+
+    d = str(tmp_path / "store")
+    store = B200MultiVectorStore.open(d, mode="bf16")
+    for c in range(calls):
+        asyncio.run(store.store_embeddings(chunks(c * pages_per_call, pages_per_call)))
+    store.save(d)
+    store.close()
+    corpus = calls * pages_per_call * page_rows * 256
+    extra = chunks(calls * pages_per_call, per_doc)
+    extra_bytes = per_doc * page_rows * 256
+    bounce = 80 << 20  # the compaction's 64 MiB bounce buffer as the handle's scratch allocator rounds it
+    for reopen in ("open", "load"):
+        torch.cuda.empty_cache()
+        start = free_bytes()
+        torch.cuda.reset_peak_memory_stats(DEV)
+        torch_start = torch.cuda.memory_allocated(DEV)
+        if reopen == "open":
+            store = B200MultiVectorStore.open(d, mode="bf16", compact_dead_fraction=0.0)
+        else:
+            store = B200MultiVectorStore.load(d)
+        assert store._index.n_pages == calls * pages_per_call
+        lowest = free_bytes()
+        asyncio.run(store.store_embeddings(extra))
+        lowest = min(lowest, free_bytes())
+        if reopen == "open":
+            assert asyncio.run(store.delete_chunks_by_document_id("d0"))  # any dead page compacts
+            assert store._index.n_pages == calls * pages_per_call  # d0's pages are gone, the new document's are in
+            lowest = min(lowest, free_bytes())
+        assert torch.cuda.max_memory_allocated(DEV) - torch_start < corpus // 8, reopen
+        assert start - lowest <= corpus + extra_bytes + CHUNK + 2 * extra_bytes + bounce + TOL, reopen
+        store.close()
 
 
 # ------------------------------------------------------------------------------------------------ stream order
