@@ -2,6 +2,7 @@
 
     build(dtype, n_pages, seed)                              -> MaxSimIndex with the corpus packed by the library itself
     reference_scores(idx, q_packed, group_offsets, q_lens)  -> float64 [n_q, n_pages] on the score_matrix scale
+    sign_rows_of(dtype, rows_u8) / sign_reference(...)     -> the sign stage's sign rows and its exact integer S
 
 Corpus (generate_chunks): page lengths are mostly 1000 .. 1100 rows, with pages of 1 .. 1025 rows hitting the chunk and tile
 edges (31 / 32 / 33, 127 / 128 / 129) every 61st page and runs of four empty pages, so the corpora reach a few GB at a few
@@ -219,15 +220,24 @@ def reference_from_bytes(dtype: str, rows_u8: torch.Tensor, lens: Sequence[int],
     """float64 [n_q, n_pages] MaxSim of the packed query block q_u8 [>= 32 * groups, row_bytes] (query q's token j at row
     32 * group_offsets[q] + j) against the packed corpus rows_u8 [rows_padded, row_bytes] of pages of `lens` true rows
     (each padded to whole 32-row chunks), on the score_matrix scale.  `budget` caps the token x row products per step."""
-    device = rows_u8.device
-    lens_np = np.asarray(lens, dtype=np.int64)
-    n_pages, n_q = len(lens_np), len(q_lens)
     goff = np.asarray(group_offsets, dtype=np.int64)
     tok = np.concatenate([32 * goff[q] + np.arange(int(t)) for q, t in enumerate(q_lens)] + [np.zeros(0, np.int64)])
-    tok_query = torch.from_numpy(np.repeat(np.arange(n_q), np.asarray(q_lens, dtype=np.int64))).to(device)
     binary = dtype == "binary"
-    cdt = torch.float16 if binary and device.type == "cuda" else torch.float64
-    q = decode(dtype, q_u8[torch.from_numpy(tok).to(q_u8.device)].to(device), cdt)  # [T, 128]
+    cdt = torch.float16 if binary and rows_u8.device.type == "cuda" else torch.float64
+    q = decode(dtype, q_u8[torch.from_numpy(tok).to(q_u8.device)].to(rows_u8.device), cdt)  # [T, 128]
+    out = _page_maxsim(q, lambda r0, r1: decode(dtype, rows_u8[r0:r1], cdt), lens, q_lens, rows_u8.device, budget,
+                       (lambda m: (m + 128.0) / 2.0) if binary else None)  # 1-bit: 128 - hamming
+    return out / _score_divisor(dtype)
+
+
+def _page_maxsim(q: torch.Tensor, rows_of, lens: Sequence[int], q_lens: Sequence[int], device, budget: int,
+                 chunk_map=None) -> torch.Tensor:
+    """float64 [n_q, n_pages]: per query (q_lens consecutive tokens of q [T, 128]), the sum over its tokens of the max over
+    each page's true rows of q . row, with rows_of(r0, r1) the padded rows [r0, r1) as q's dtype.  chunk_map: applied to the
+    per-chunk maxima (float64).  Pages without rows and queries without tokens score 0."""
+    lens_np = np.asarray(lens, dtype=np.int64)
+    n_pages, n_q = len(lens_np), len(q_lens)
+    tok_query = torch.from_numpy(np.repeat(np.arange(n_q), np.asarray(q_lens, dtype=np.int64))).to(device)
     T = q.shape[0]
     out = torch.zeros((n_q, n_pages), dtype=torch.float64, device=device)
     if T == 0 or n_pages == 0:
@@ -241,22 +251,56 @@ def reference_from_bytes(dtype: str, rows_u8: torch.Tensor, lens: Sequence[int],
         p1 = min(max(p1, p0 + 1), n_pages)
         r0, r1 = int(start[p0]), int(start[p1])
         if r1 > r0:
-            x = decode(dtype, rows_u8[r0:r1], cdt)  # the chunk's padded rows; the pad rows are masked below
+            x = rows_of(r0, r1)  # the chunk's padded rows; the pad rows are masked below
             sim = q @ x.T  # [T, R]
             col = np.arange(r1 - r0) + r0
             page_of_row = np.repeat(np.arange(p0, p1), pad[p0:p1])
             is_pad = torch.from_numpy(col - start[page_of_row] >= lens_np[page_of_row]).to(device)
             sim.masked_fill_(is_pad[None, :], float("-inf"))
             chunk_max = sim.view(T, -1, 32).amax(dim=2).double()  # per 32-row chunk: every page owns whole chunks
-            if binary:
-                chunk_max = (chunk_max + 128.0) / 2.0  # 128 - hamming
+            if chunk_map is not None:
+                chunk_max = chunk_map(chunk_max)
             chunk_page = torch.from_numpy(page_of_row[::32] - p0).to(device)
             best = torch.zeros((T, p1 - p0), dtype=torch.float64, device=device)
             best.scatter_reduce_(1, chunk_page[None, :].expand(T, -1), chunk_max, "amax", include_self=False)
             out[:, p0:p1].index_add_(0, tok_query, best)
             del sim, chunk_max, best, x
         p0 = p1
-    return out / _score_divisor(dtype)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ sign stage
+_BIT_WEIGHTS = torch.tensor([128, 64, 32, 16, 8, 4, 2, 1], dtype=torch.int32)
+
+
+def sign_rows_of(dtype: str, rows_u8: torch.Tensor, step: int = 1 << 20) -> torch.Tensor:
+    """uint8 [n, 16]: the sign rows of packed rows uint8 [n, row_bytes] by the header's rule on the packed values (bf16
+    0x0001 .. 0x7f80, int8 1 .. 127, e4m3 0x01 .. 0x7e), MSB first, with torch integer ops, `step` rows at a time."""
+    out = torch.empty((rows_u8.shape[0], 16), dtype=torch.uint8, device=rows_u8.device)
+    w = _BIT_WEIGHTS.to(rows_u8.device)
+    for r0 in range(0, rows_u8.shape[0], step):
+        raw = rows_u8[r0:r0 + step]
+        if dtype == "bf16":
+            v = raw.view(torch.int16).to(torch.int32) & 0xFFFF
+            bits = (v >= 1) & (v <= 0x7F80)
+        else:
+            v = raw.to(torch.int32)
+            bits = (v >= 1) & (v <= {"int8": 0x7F, "fp8": 0x7E}[dtype])
+        out[r0:r0 + step] = (bits.view(-1, 16, 8).to(torch.int32) * w).sum(dim=2).to(torch.uint8)
+    return out
+
+
+def sign_reference(sign_rows: torch.Tensor, lens: Sequence[int], q8s: Sequence[np.ndarray],
+                   budget: int = 1 << 27) -> np.ndarray:
+    """int64 [n_q, n_pages]: the sign stage's S (include/b200ms.h, "sign candidates") of queries quantised to q8s (int
+    [T_q, 128] each) over the sign rows uint8 [rows_padded, 16] of pages of `lens` true rows: +-1 rows times q8 in float64,
+    where every product and partial sum is an integer of magnitude < 2^24, so exact."""
+    device = sign_rows.device
+    q8s = [np.asarray(q, dtype=np.int64).reshape(-1, 128) for q in q8s]
+    q = torch.from_numpy(np.concatenate(q8s + [np.zeros((0, 128), np.int64)]).astype(np.float64)).to(device)
+    out = _page_maxsim(q, lambda r0, r1: unpack_bits(sign_rows[r0:r1]).double() * 2 - 1, lens, [len(x) for x in q8s],
+                       device, budget)
+    return out.cpu().numpy().astype(np.int64)
 
 
 def reference_scores(idx, q_packed: torch.Tensor, group_offsets, q_lens: Sequence[int],

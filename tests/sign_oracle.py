@@ -56,17 +56,19 @@ def page_starts(page_lens: Sequence[int]) -> np.ndarray:
 
 def scores(q8s: Sequence[np.ndarray], bits: np.ndarray, page_lens: Sequence[int]) -> np.ndarray:
     """S [n_q, n_pages] int64: per query, sum over its tokens of the max over each page's TRUE rows of sum_i q8 * (+1 | -1).
-    bits: bool [padded rows, 128] in the padded page layout.  A page without rows and a query without tokens score 0."""
-    pm = np.where(np.asarray(bits, dtype=bool), 1, -1).astype(np.int64)
+    bits: bool [padded rows, 128] in the padded page layout.  A page without rows and a query without tokens score 0.
+    The products are taken in float64, which holds every one of them exactly (|q8 . row| <= 128 * 63)."""
+    pm = np.where(np.asarray(bits, dtype=bool), 1.0, -1.0)
     ps = page_starts(page_lens)
+    qf = [np.asarray(q8, dtype=np.float64).reshape(-1, 128) for q8 in q8s]
     out = np.zeros((len(q8s), len(page_lens)), dtype=np.int64)
     for p, n in enumerate(page_lens):
         if n <= 0:
             continue
         rows = pm[ps[p]:ps[p] + n]
-        for q, q8 in enumerate(q8s):
+        for q, q8 in enumerate(qf):
             if len(q8):
-                out[q, p] = (np.asarray(q8, dtype=np.int64) @ rows.T).max(axis=1).sum()
+                out[q, p] = (q8 @ rows.T).max(axis=1).astype(np.int64).sum()
     return out
 
 
@@ -75,6 +77,46 @@ def topk(s: np.ndarray, k: int, allowed: Optional[np.ndarray] = None) -> List[in
     ids = np.arange(len(s)) if allowed is None else np.flatnonzero(allowed)
     order = sorted(ids.tolist(), key=lambda p: (-int(s[p]), p))
     return order[:k]
+
+
+def probe_bits() -> np.ndarray:
+    """bool [129, 128]: the rows of the probe corpus, one single-row page each -- page 0 has every sign negative, page
+    1 + i only element i positive.  For a one-token query, S[1 + i] - S[0] = 2 q8_i (probe_q8)."""
+    bits = np.zeros((129, 128), dtype=bool)
+    bits[1 + np.arange(128), np.arange(128)] = True
+    return bits
+
+
+def probe_q8(s: np.ndarray) -> np.ndarray:
+    """S [n_q, 129] of one-token queries against the probe corpus -> the q8 [n_q, 128] each query was quantised to."""
+    s = np.asarray(s, dtype=np.int64).reshape(-1, 129)
+    d = s[:, 1:] - s[:, :1]
+    if (d % 2).any():
+        raise ValueError("odd score differences: not the scores of one-token queries against the probe corpus")
+    return d // 2
+
+
+def tie_inputs(scale: float) -> np.ndarray:
+    """float32 x with fp32(x * scale) == k + 0.5 exactly, for every k in -64 .. 63 for which such an x exists (each the one
+    closest to (k + 0.5) / scale): the quantiser's rounding ties, the +-63.5 clamp boundary included."""
+    s = np.float32(scale)
+    out = []
+    with np.errstate(over="ignore", under="ignore", invalid="ignore"):
+        for k in range(-64, 64):
+            t = np.float32(k + 0.5)
+            x0 = np.float32(np.float64(t) / np.float64(s))
+            if not np.isfinite(x0) or x0 == 0:
+                continue
+            cand = [x0]
+            for direction in (np.float32(np.inf), np.float32(-np.inf)):
+                x = x0
+                for _ in range(4):
+                    x = np.nextafter(x, direction, dtype=np.float32)
+                    cand.append(x)
+            hits = [x for x in cand if np.float32(x * s) == t]
+            if hits:
+                out.append(min(hits, key=lambda x: abs(np.float64(x) - np.float64(t) / np.float64(s))))
+    return np.asarray(out, dtype=np.float32)
 
 
 def mask_allowed(words: Optional[np.ndarray], n_pages: int) -> Optional[np.ndarray]:

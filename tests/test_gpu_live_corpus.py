@@ -10,8 +10,9 @@
   * Shard files on both tiers, fresh and appended to an index, empty ones too: read into the index's own block, equal to
     the index they were saved from.
   * Free device memory around growth and compaction, and around a store's open / load: the block lives outside torch's
-    allocator, so the tests sample torch.cuda.mem_get_info.  Other jobs may share the card: the bounds carry a tolerance of
-    256 MiB.
+    allocator, so the tests sample the device memory this process holds, through NVML's per-process accounting, which
+    other jobs on the card do not move (torch.cuda.mem_get_info's free memory where NVML cannot tell this process apart).
+    The bounds carry a tolerance of 256 MiB.
   * One stream-order case: a search in flight on one stream, a compaction, a search after it.
 """
 import asyncio
@@ -37,7 +38,7 @@ from test_compact_plan_cpu import page_runs, patterns  # noqa: E402
 
 DEV = torch.device("cuda", 0)
 CHUNK = 32 << 20
-TOL = 256 << 20  # other jobs share the card
+TOL = 256 << 20  # scratch the handle keeps, and other jobs on the card where free_bytes cannot exclude them
 DTYPES = ("bf16", "int8", "fp8", "binary")
 
 
@@ -49,9 +50,54 @@ def cstream():
     return ctypes.c_void_p(torch.cuda.current_stream(DEV).cuda_stream)
 
 
+def _nvml_own_pid():
+    """This process's pid as NVML reports it (it may differ from os.getpid() inside a container): the one process whose
+    device memory grows by a 256 MiB block backed for the purpose.  None when NVML cannot say (no NVML, no per-process
+    accounting, or another process grew as much at the same time)."""
+    try:
+        import pynvml
+
+        pynvml.nvmlInit()
+        dev = pynvml.nvmlDeviceGetHandleByIndex(DEV.index or 0)
+
+        def used():
+            torch.cuda.synchronize(DEV)
+            return {p.pid: p.usedGpuMemory for p in pynvml.nvmlDeviceGetComputeRunningProcesses(dev)}
+
+        h = nat.Handle(DEV.index or 0)
+        try:
+            before = used()
+            probe = DeviceBlock.resized(None, h, DEV, 256 << 20)
+            after = used()
+            probe.free()
+        finally:
+            torch.cuda.synchronize(DEV)
+            h.close()
+        grown = [pid for pid, u in after.items() if u is not None and u - (before.get(pid) or 0) >= (192 << 20)]
+        return (dev, grown[0]) if len(grown) == 1 else None
+    except Exception:  # pragma: no cover - NVML missing or refused: fall back to the card's free memory
+        return None
+
+
+_OWN = []
+
+
 def free_bytes():
+    """Device memory free to this process: the card's total less what this process holds (NVML's per-process use), so
+    that other jobs on the card move none of the bounds below; torch.cuda.mem_get_info's free memory, and the bounds'
+    tolerance, where NVML cannot tell this process apart."""
+    if not _OWN:
+        _OWN.append(_nvml_own_pid())
     torch.cuda.synchronize(DEV)
-    return torch.cuda.mem_get_info(DEV)[0]
+    free, total = torch.cuda.mem_get_info(DEV)
+    if _OWN[0] is None:
+        return free
+    import pynvml
+
+    dev, pid = _OWN[0]
+    mine = [p.usedGpuMemory for p in pynvml.nvmlDeviceGetComputeRunningProcesses(dev) if p.pid == pid]
+    assert len(mine) == 1 and mine[0] is not None, "NVML lost track of this process"
+    return total - mine[0]
 
 
 @pytest.fixture(scope="module")

@@ -13,8 +13,12 @@ assert_scores / assert_ranking / assert_candidate_ranking and their tolerances:
     ranking against the reference, bit-identical to b200ms_score + masked b200ms_topk, plan = tests/scan_plan_model.py;
   * search_docs_device with 16 pages per document against tests/docs_oracle.py;
   * rerank_batch of 1000 candidates per query, most past 4 GiB, with duplicates and unused slots; explain of pages past 4 GiB;
-  * the host tier: an int8 corpus of more than 4 GiB in pinned memory reranks bit-identically to the HBM tier.
+  * the host tier: an int8 corpus of more than 4 GiB in pinned memory reranks bit-identically to the HBM tier;
+  * the sign stage (bf16, int8, fp8): b200ms_sign_rows of every row, past byte 2^32, against the header's rule in torch
+    integer ops; every page's exact S (scale_reference.sign_reference) through per-query masks of at most 4096 pages on the
+    filtered plan, and the first 4096 candidates of the unmasked batch in the oracle's order.
 """
+import ctypes
 import gc
 import time
 
@@ -28,11 +32,12 @@ if not torch.cuda.is_available():  # pragma: no cover - the gpu marker normally 
     pytest.skip("CUDA device required", allow_module_level=True)
 
 import scale_reference as sr  # noqa: E402
+import sign_oracle as so  # noqa: E402
 import scan_plan_model as spm  # noqa: E402
 import test_gpu_filtered_scan as tfs  # noqa: E402
 from docs_oracle import topk_docs_np  # noqa: E402
 from morphik_core_b200 import _native as nat  # noqa: E402
-from morphik_core_b200.index import MaxSimIndex  # noqa: E402
+from morphik_core_b200.index import MaxSimIndex, _aligned_bytes  # noqa: E402
 from oracle.scoring import TOL, assert_candidate_ranking, assert_ranking, assert_scores, slot_scores_of  # noqa: E402
 
 DEV = torch.device("cuda", 0)
@@ -272,3 +277,68 @@ def test_host_tier_rerank_is_bit_identical(scale):
         assert host.gather_stats()["unique_pages"] > 0
     finally:
         host.close()
+
+
+# ------------------------------------------------------------------------------------------------ sign stage
+def sign_candidates(idx, queries, n_cand, masks=None, index=None):
+    """b200ms_sign_candidates_device at q_scale 127 and score_scale 1 (scores are float32(S)) -> host arrays."""
+    src = torch.from_numpy(np.concatenate(queries).astype(np.float32)).to(DEV)
+    lens = [len(q) for q in queries]
+    n_q = len(lens)
+    ts = torch.empty((n_q, n_cand), dtype=torch.float32, device=DEV)
+    ti = torch.empty((n_q, n_cand), dtype=torch.int64, device=DEV)
+    tc = torch.empty((n_q,), dtype=torch.int32, device=DEV)
+    vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    idx.h.check(nat.lib.b200ms_sign_candidates_device(
+        idx.h.ptr, vp(src), nat.F32, nat.i32_array(lens), n_q, n_cand, vp(masks), 0 if masks is None else masks.shape[0],
+        vp(index), ctypes.c_float(127.0), ctypes.c_float(1.0), vp(ts), vp(ti), vp(tc),
+        ctypes.c_void_p(torch.cuda.current_stream(DEV).cuda_stream)), "b200ms_sign_candidates_device")
+    return tfs.to_np((ts, ti, tc))
+
+
+def assert_sign_order(got, S, allowed, what):
+    ts, ti, tc = got
+    want = so.topk(S, len(ti), allowed)
+    assert int(tc) == len(want) and ti[:len(want)].tolist() == want, what
+    assert np.array_equal(ts[:len(want)], S[want].astype(np.float32)), what
+    assert (ti[len(want):] == -1).all(), what
+
+
+@pytest.mark.parametrize("scale", ["bf16", "int8", "fp8"], indirect=True)
+def test_sign_stage_past_4gib(scale):
+    idx, dtype = scale.idx, scale.dtype
+    n, rows = idx.n_pages, idx.n_rows_padded
+    stream = ctypes.c_void_p(torch.cuda.current_stream(DEV).cuda_stream)
+    signs = _aligned_bytes(rows * 16, DEV, 16)
+    try:
+        idx.h.check(nat.lib.b200ms_sign_rows(idx.h.ptr, 0, n, ctypes.c_void_p(signs.data_ptr()), stream), "b200ms_sign_rows")
+        want_rows = sr.sign_rows_of(dtype, idx.packed_rows())
+        got_rows = signs.view(rows, 16)
+        past = FOUR_GIB // idx.row_bytes
+        assert torch.equal(got_rows[:past], want_rows[:past]) and torch.equal(got_rows[past:], want_rows[past:])
+        idx.h.check(nat.lib.b200ms_set_sign_rows(idx.h.ptr, ctypes.c_void_p(signs.data_ptr()), rows, stream),
+                    "b200ms_set_sign_rows")
+        S = sr.sign_reference(want_rows, scale.lens, [so.quantise_query(q, 127.0) for q in scale.qs])
+        del want_rows
+        # every page once: query 0 under disjoint masks of at most 4096 pages (more units than SMs: the filtered plan)
+        perm = np.random.default_rng(3).permutation(n)
+        parts = np.array_split(perm, -(-n // 4096))
+        allow = np.zeros((len(parts), n), bool)
+        for m, part in enumerate(parts):
+            allow[m, part] = True
+        masks = torch.from_numpy(np.stack([idx.mask_from_pages(a) for a in allow]).view(np.int32)).to(DEV)
+        index = torch.arange(len(parts), dtype=torch.int32, device=DEV)
+        ts, ti, tc = sign_candidates(idx, [scale.qs[0]] * len(parts), 4096, masks, index)
+        for m in range(len(parts)):
+            assert_sign_order((ts[m], ti[m], tc[m]), S[0], allow[m], f"{dtype} mask {m}")
+        assert np.array_equal(np.sort(np.concatenate([ti[m, :tc[m]] for m in range(len(parts))])), np.arange(n))
+        # the unmasked batch of the module's 13 queries
+        ts, ti, tc = sign_candidates(idx, scale.qs, 4096)
+        for qi in range(len(scale.qs)):
+            assert_sign_order((ts[qi], ti[qi], tc[qi]), S[qi], None, f"{dtype} q{qi}")
+        print(f"\n[scale] {dtype}: sign stage checked on {n} pages, {rows * 16 / 2**20:.0f} MiB of sign rows, {len(parts)} masks")
+    finally:
+        torch.cuda.synchronize(DEV)
+        idx._attached = False
+        idx._attach()  # set_corpus detaches the sign rows before their buffer goes
+        del signs

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import scale_reference as sr
+import sign_oracle as so
 from oracle import maxsim_oracle as orc
 from oracle import planted
 from oracle.scoring import assert_scores, oracle_scores, reference_values
@@ -150,3 +151,23 @@ def test_gpu_corpora_reach_past_four_gib(dtype, n_pages):
     rows = int(sr.padded_rows(sr.page_lens(n_pages, 0)).sum())
     assert rows * sr.ROW_BYTES[dtype] > 2 ** 32 + 2 ** 30
     assert rows < 2 ** 31  # TMA row coordinates are int32
+
+
+@pytest.mark.parametrize("dtype", ["bf16", "int8", "fp8"])
+def test_sign_reference_equals_the_sign_oracle(dtype):
+    # every packed value through the torch sign rule
+    if dtype == "bf16":
+        every = np.arange(65536, dtype=np.uint16).view(np.uint8).reshape(-1, 256)
+    else:
+        every = np.tile(np.arange(256, dtype=np.uint8), 64).reshape(-1, 128)
+    got = sr.sign_rows_of(dtype, torch.from_numpy(every), step=7).numpy()
+    assert np.array_equal(got, so.pack_bits(so.sign_bits(dtype, every)))
+    # S of planted pages, and of queries without tokens and pages without rows
+    pc = planted.planted_corpus(dtype, seed=33, n_random=12)
+    rows = pack_pages(dtype, pc.pages)
+    signs = sr.sign_rows_of(dtype, rows)
+    qs = planted.planted_queries(pc, [1, 33, 0, 130], seed=5)
+    q8s = [so.quantise_query(q, 127.0) for q in qs]
+    want = so.scores(q8s, so.sign_bits(dtype, rows.numpy()), pc.lens)
+    assert np.array_equal(sr.sign_reference(signs, pc.lens, q8s), want)
+    assert np.array_equal(sr.sign_reference(signs, pc.lens, q8s, budget=1), want)

@@ -2,6 +2,7 @@
 every dtype against the float signs of oracle/value_rules.py's packed values, every edge of the query quantiser, the
 2 q8 / c_t form of the scan against the +-1 dot product, empty pages, padding tokens and the tie order."""
 import numpy as np
+import pytest
 import torch
 
 import sign_oracle as so
@@ -103,6 +104,42 @@ def test_scores_empty_pages_padding_rows_and_empty_queries():
             if n and len(q8):
                 want = sum(max(int(q8[t] @ pm[ps[p] + r]) for r in range(n)) for t in range(len(q8)))
                 assert s[q, p] == want
+
+
+def test_probe_corpus_decodes_q8():
+    rng = np.random.default_rng(3)
+    q8 = rng.integers(-63, 64, size=(20, 128))
+    q8[0], q8[1], q8[2] = 63, -63, 0
+    bits = so.probe_bits()
+    assert bits.sum() == 128 and not bits[0].any()
+    padded = np.repeat(bits, 32, axis=0)  # single-row pages, padding rows repeat the row
+    s = so.scores(list(q8[:, None, :]), padded, [1] * 129)
+    np.testing.assert_array_equal(so.probe_q8(s), q8)
+    # brute force: page 1 + i scores -sum q8 + 2 q8_i
+    np.testing.assert_array_equal(s[:, 1:], -q8.sum(axis=1, keepdims=True) + 2 * q8)
+    s[0, 5] += 1
+    with pytest.raises(ValueError):
+        so.probe_q8(s)
+
+
+@pytest.mark.parametrize("scale", [127.0, 32.0, 512.0, 1.0, 0.75])
+def test_tie_inputs_are_ties(scale):
+    x = so.tie_inputs(scale)
+    assert x.dtype == np.float32
+    y = x * np.float32(scale)
+    assert set(y.tolist()) <= {k + 0.5 for k in range(-64, 64)} and len(set(y.tolist())) == len(x)
+    if scale in (32.0, 512.0, 1.0):  # a power of two: every k has its tie
+        assert len(x) == 128
+    # brute force over the float32 bit patterns within 4 ulps of (k + 0.5) / scale: a k without a returned x has no tie
+    found = set(y.tolist())
+    for k in range(-64, 64):
+        x0 = np.array([(k + 0.5) / scale], dtype=np.float32).view(np.int32)[0]
+        near = (x0 + np.arange(-4, 5, dtype=np.int32)).view(np.float32)
+        assert bool((near * np.float32(scale) == np.float32(k + 0.5)).any()) == ((k + 0.5) in found), k
+    # the quantiser rounds every tie to the even neighbour, then clamps
+    q = so.quantise_query(np.resize(x, (len(x) + 127) // 128 * 128).reshape(-1, 128), scale).reshape(-1)[:len(x)]
+    lo = np.floor(y)
+    np.testing.assert_array_equal(q, np.clip(np.where(lo % 2 == 0, lo, lo + 1), -63, 63).astype(np.int64))
 
 
 def test_topk_order_and_masks():
