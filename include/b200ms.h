@@ -186,10 +186,30 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
                         int dst_dtype, float i8_scale, int32_t* group_offsets_out, int* n_groups_out, void* stream);
 
 /* ---- the hot path ---------------------------------------------------------------------------- */
-/* group_scores[g, p] = sum over the (<=32) tokens of group g of max over the rows of page p of <q_t, d_r>
+/* group_scores[g, p] = sum over the (<=32) true tokens of group g of max over the rows of page p of <q_t, d_r>
  *   BF16 / F8 corpus: float32 (fp32 accumulate on wgmma);  I8: int32 exact;  B1: int32 sum_t max_r (128 - hamming).
  * q_packed: device [roundup(n_groups,4)*32, 128] of the corpus dtype; q_lens/group_offsets (HOST) as produced by
- * b200ms_pack_queries (B1 needs the true token counts; may be NULL for BF16/I8).
+ * b200ms_pack_queries.  With both given, the true tokens of each group are the query's (the zero padding rows of a group
+ * add +0).  B1 needs them; for BF16 / I8 / F8 they may be NULL, and then every row of q_packed counts as a token, the zero
+ * padding rows included (each adds max_r <0, d_r>: 0 on finite pages, NaN on a page whose rows all hold an infinity).
+ * Value rule of BF16 and F8 corpora (the "float value rule"; every entry point that scores them follows it):
+ *   - sim(q_t, d_r) is the dot product of the PACKED values (bf16, or e4m3 codes widened exactly to f16), rounded to fp32,
+ *     with IEEE non-finite arithmetic: 0 * +-inf = NaN, NaN * x = NaN, +inf + -inf = NaN.  The products are exact and
+ *     the finite sum is rounded to fp32: past its range to +-inf, into its subnormal range as IEEE rounds, below half the
+ *     least subnormal to 0.  The order of the fp32 additions is the tensor core's, so a finite result can differ from the
+ *     exactly rounded sum by a few fp32 ulps per term (oracle/scoring.py TOL).
+ *   - Measured on an NVIDIA H100 80GB HBM3 (700 W limit; wgmma m64n128k16 .bf16, fp32 accumulate), on every bf16 pattern
+ *     and on one-hot products of powers of two: subnormal bf16 inputs are used as they are, not flushed; a product that
+ *     lands in fp32's subnormal range is kept (2^-127 .. 2^-149 exact), 2^-150 and below give 0; a product of 2^128 or
+ *     more gives +-inf.  A product does not overflow on its own: 2^64 * 2^64 + (-2^64) * 2^64 inside one 16-element MMA
+ *     step gives 0, not NaN (partial sums across steps are fp32).  e4m3 products lie in [2^-18, 448^2] and are exact.
+ *   - The max over a page's TRUE rows is fmaxf's: a NaN row is ignored unless every row is NaN (then the max is NaN).
+ *   - The group score sums the query's true tokens only, so a query's score is the IEEE sum of its tokens' maxima:
+ *     NaN if some token's max is NaN or if +inf and -inf meet, else +-inf if one occurs, else finite.
+ *   - zero_pad_compat (b200ms_set_option) replaces a clamped page's token max m by fmaxf(m, 0), so a NaN max becomes 0 there;
+ *     colpali_engine's torch scorer propagates the NaN instead (torch.max over a row holding a NaN is NaN).
+ * Reranks, document searches, host-resident corpora and sharded searches score with this kernel, so the rule holds for
+ * them; b200ms_explain_device reports the same per-token values.
  * group_scores: device [n_groups_padded, ld] with ld >= n_pages, n_groups_padded = roundup(n_groups,4).
  * Pages with zero rows score 0 (COALESCE(...,0.0), multi_vector_store.py:308).
  * b200ms_score scans every page.  The search entry points below that take an allow mask (b200ms_search_host*,
@@ -248,7 +268,8 @@ int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int src_dtype, c
                                 float i8_q_scale, float score_scale, int64_t id_base, float* top_scores_dev,
                                 int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream);
 
-/* MaxSim over an explicit candidate list (the "rerank" half of a two-stage search, fast_multivector_store.py:545-557):
+/* MaxSim over an explicit candidate list (the "rerank" half of a two-stage search, fast_multivector_store.py:545-557;
+ * BF16 / F8 scores follow the float value rule of b200ms_score, so do the rerank and document calls below):
  * cand_ids_dev = device array of n_cand page ids (-1, or any id outside [0, n_pages) = unused slot; a page may appear in
  * several slots).  Only those pages are scanned; ties break towards the earlier candidate slot (= better first-stage rank),
  * for every n_cand.  Outputs as b200ms_search_device. */
@@ -280,6 +301,8 @@ int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, co
  * best row -1, map entries -inf.  Map entries at r >= page length are -inf.
  * Queries are packed exactly as b200ms_search_device packs them (same i8_q_scale, same sign rule).
  * A max over rows is fmaxf's (a NaN only when every row is NaN); a tie, +0 and -0 included, reports the lowest row.
+ * BF16 / F8 values follow the float value rule of b200ms_score: their token scores add up, NaN and +-inf included, to the
+ * rerank's score, since neither counts a query's padding tokens.
  * Host-resident corpora: the named pages are gathered like a rerank's candidates (b200ms_last_gather_stats reports the call)
  * and the outputs are bit-identical to an HBM corpus of the same rows.
  * Option "zero_pad_compat" is ignored: maps are over true rows only.
@@ -299,7 +322,8 @@ int b200ms_explain_device(b200ms_t* h, const void* q_dev, int src_dtype, const i
  * is set, if a mask is given, and its page_doc is in range).  The result is
  *   - documents in the order of their first page in L, at most k of them;
  *   - for each, its first per_doc pages in L (a document with fewer eligible pages returns fewer);
- *   - every score bit for bit the score the flat call reports for that page; a document's score is its first page's.
+ *   - every score bit for bit the score the flat call reports for that page (BF16 / F8: the float value rule of
+ *     b200ms_score); a document's score is its first page's.
  * Candidate mode: L ranks q's valid slots (id in [0, n_pages)) by score DESC then slot ASC; a page that occupies several
  * slots counts once, at its earliest slot.  With n_docs == n_pages, page_doc[p] == p and per_doc == 1 the result equals
  * the flat call's.  Outputs are device arrays:
@@ -355,7 +379,7 @@ int b200ms_allgather_topk(b200ms_t* h, void* nccl_comm, const void* xchg_local_d
 /* Pipelined sharded search.  _begin enqueues the local scan + top-k (global ids = id_base + local page) on `stream` and the
  * all-gather + merge on the handle's communication stream behind an event, then returns a ticket (>= 0; negative = error);
  * the caller's stream is NOT made to wait for the other ranks, so the next _begin may follow at once (two exchange slots: at
- * most two searches in flight).  _end makes `stream` wait for that ticket's merged result in the output buffers given to
+ * most two searches in flight).  The local scores follow the float value rule of b200ms_score.  _end makes `stream` wait for that ticket's merged result in the output buffers given to
  * _begin.  Masks as in b200ms_search_device_masked (n_masks = 0: unfiltered).  Works with world == 1 (no collective). */
 int64_t b200ms_sharded_search_begin(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
                                     const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,

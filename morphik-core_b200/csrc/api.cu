@@ -675,8 +675,8 @@ static int candidate_plan(b200ms_t* h, const CorpusView& v, const int64_t* unit_
 // Per-query candidate lists on wgmma: one launch per 128-token query tile, the tile's queries against THEIR candidate
 // lists only (a contiguous slot range).
 static int score_wgmma_per_query(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const CandSpec& cs,
-                                 const void* q_packed, int n_groups, const int32_t* goff, int n_q, void* group_scores,
-                                 int64_t ld, cudaStream_t s) {
+                                 const void* q_packed, int n_groups, const int32_t* goff, const int32_t* ntok_dev, int n_q,
+                                 void* group_scores, int64_t ld, cudaStream_t s) {
   const int n_mtiles = int(groups_padded(n_groups)) / 4;
   int q_lo = 0;
   for (int m = 0; m < n_mtiles; ++m) {
@@ -692,7 +692,7 @@ static int score_wgmma_per_query(b200ms_t* h, const CorpusView& v, const UnitPla
     sub.n_units = int(int64_t(q_hi - q_lo) * cs.stride());
     if (sub.clamp_bits) sub.clamp_bits += s0 / 32;
     void* sc = static_cast<uint8_t*>(group_scores) + size_t(s0) * 4;
-    if (int e = launch_score_wgmma(h, v, sub, q_packed, n_groups, sc, ld, s, m, m + 1)) return e;
+    if (int e = launch_score_wgmma(h, v, sub, q_packed, n_groups, ntok_dev, sc, ld, s, m, m + 1)) return e;
   }
   return B200MS_OK;
 }
@@ -743,9 +743,9 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   } else if (b1) {
     e = launch_score_b1(h, v, unit_ids, cs.n_cand, q_packed, n_groups, ntok_dev, group_scores, ld, s, 0, n_groups, scan);
   } else if (cs.per_query) {
-    e = score_wgmma_per_query(h, v, plan, cs, q_packed, n_groups, goff, n_q, group_scores, ld, s);
+    e = score_wgmma_per_query(h, v, plan, cs, q_packed, n_groups, goff, ntok_dev, n_q, group_scores, ld, s);
   } else {
-    e = launch_score_wgmma(h, v, plan, q_packed, n_groups, group_scores, ld, s);
+    e = launch_score_wgmma(h, v, plan, q_packed, n_groups, ntok_dev, group_scores, ld, s);
   }
   if (e) return e;
   if (!h->capturing) {
@@ -763,9 +763,10 @@ B200MS_API int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, con
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   StreamOrder order(h, s);
   if (int e = order.error()) return e;
-  const int32_t* ntok_dev = nullptr;
-  if (h->corpus.dtype == B200MS_B1) {
-    if (!q_lens || !group_offsets || n_q <= 0) return set_error(h, B200MS_EINVAL, "score: B1 needs q_lens and group_offsets");
+  const int32_t* ntok_dev = nullptr;  // dense corpora without q_lens / group_offsets: every packed row is a token
+  if (h->corpus.dtype == B200MS_B1 && (!q_lens || !group_offsets || n_q <= 0))
+    return set_error(h, B200MS_EINVAL, "score: B1 needs q_lens and group_offsets");
+  if (q_lens && group_offsets && n_q > 0) {
     const int64_t gp = groups_padded(n_groups);
     std::vector<int32_t> ntok(size_t(gp > 0 ? gp : 4), 0);
     group_tokens(q_lens, n_q, group_offsets, n_groups, ntok.data());

@@ -354,8 +354,10 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
                     void* ctx);
 
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
+// group_ntok (device, [n_groups_real] or NULL = 32 each): the true tokens of every group; a padding token adds +0
 int launch_score_wgmma(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const void* q_packed, int n_groups_real,
-                       void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo = 0, int m_tile_hi = -1);
+                       const int32_t* group_ntok, void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo = 0,
+                       int m_tile_hi = -1);
 // scan != NULL (full scans, cand_ids == NULL): only the pages scan->pages lists, scores still indexed by page id
 int launch_score_b1(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
                     int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,

@@ -150,7 +150,7 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
                     const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start,
                     const int32_t* __restrict__ unit_end, int slot_mode, int n_units,
                     const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,
-                    const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
+                    const int32_t* __restrict__ group_ntok, const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
                     int num_stages, int splits) {
   using K = Kind<KIND>;
   using Acc = typename K::Acc;
@@ -360,20 +360,24 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
 #pragma unroll
     for (int k = 0; k < 4; ++k) runmax[i][k] = Acc(0);
 
-  // score of page `page` (unit u in slot_mode) for the group of query tile i; page < 0: nothing accumulated yet
+  // score of page `page` (unit u in slot_mode) for the group of query tile i; page < 0: nothing accumulated yet.  Only the
+  // group's true tokens count (group_ntok; NULL: all 32): a zero padding row's max is NaN on a page whose rows all hold an
+  // infinity (0 * inf), not 0.
   auto flush = [&](int i, int u, int page) {
     const int mt = m_tile_base + wg + 2 * i;
     const int group = mt * 4 + w;
     if (group < n_groups_real && page >= 0) {
       const int o = slot_mode ? u : page;
+      const int ntok = group_ntok ? __ldg(group_ntok + group) : kGroup;
       Acc v[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         Acc cnst = Acc(0);
         // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w; read here, not held in registers
-        if constexpr (BITS)
-          cnst = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2));
-        v[k] = clamp_token_max(clamp_bits, o, quad_max(runmax[i][k])) + cnst;
+        const int tok = 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2);
+        if constexpr (BITS) cnst = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + tok);
+        const Acc m = clamp_token_max(clamp_bits, o, quad_max(runmax[i][k])) + cnst;
+        v[k] = tok < ntok ? m : Acc(0);
       }
       const Acc s = group_sum(v);
       if (lane == 0) group_scores[int64_t(group) * ld + o] = s;
@@ -488,7 +492,8 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
 // the second read hits L2 -- two back-to-back passes over the corpus would read it from HBM twice.
 template <int KIND, int NM, bool BITS>
 static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
-                      int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s, int splits = 1) {
+                      const int32_t* group_ntok, int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s,
+                      int splits = 1) {
   using K = Kind<KIND>;
   const uint32_t avail = kSmemLimit - 1024 /*align*/ - kBarrierBytes - NM * K::kTileBytes;
   int stages = int(avail / K::kTileBytes);
@@ -505,7 +510,7 @@ static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, cons
   static const CUtensorMap kNoTmap{};  // 1-bit rows: the producer expands bits and never issues TMA loads for them
   kern<<<grid, kThreads, smem, s>>>(c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
                                    c.chunk_page, up.start, up.end, up.slot_mode, up.n_units, up.n_units_dev,
-                                   m_tile_base, n_groups_real, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
+                                   m_tile_base, n_groups_real, group_ntok, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
                                    stages, splits);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch maxsim_wgmma");
@@ -516,13 +521,13 @@ static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, cons
 // the grid holds a pair of CTAs.
 template <int KIND, bool BITS>
 static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
-                        int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
+                        const int32_t* group_ntok, int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
   constexpr int kMaxNM = Kind<KIND>::kMaxNM;
   const bool pairs = (h->max_ctas > 0 ? h->max_ctas : h->num_sms) >= 2;
   for (int base = m_lo; base < m_hi;) {
     const int rem = m_hi - base;
     if (pairs && rem >= 2 * kMaxNM) {
-      if (int e = launch_one<KIND, kMaxNM, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s, 2)) return e;
+      if (int e = launch_one<KIND, kMaxNM, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, 2)) return e;
       base += 2 * kMaxNM;
       continue;
     }
@@ -530,12 +535,12 @@ static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, co
     while (nm < rem && nm < kMaxNM) nm <<= 1;
     int e;
     switch (nm) {
-      case 1: e = launch_one<KIND, 1, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
-      case 2: e = launch_one<KIND, 2, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
-      case 4: e = launch_one<KIND, 4, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s); break;
+      case 1: e = launch_one<KIND, 1, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
+      case 2: e = launch_one<KIND, 2, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
+      case 4: e = launch_one<KIND, 4, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
       default:
         if constexpr (kMaxNM >= 8) {
-          e = launch_one<KIND, 8, BITS>(h, c, up, tq, tok_const, base, n_groups_real, scores, ld, s);
+          e = launch_one<KIND, 8, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s);
         } else {
           e = set_error(h, B200MS_EINVAL, "maxsim_wgmma: bad NM");
         }
@@ -559,7 +564,7 @@ static int query_tmap(b200ms_t* h, const void* q, int dtype, int n_q_rows) {
 // m_tile_lo / m_tile_hi: score only query tiles [m_tile_lo, m_tile_hi) (hi < 0: all) -- the batched rerank walks the query
 // tiles one launch at a time, each against its own candidate units.
 int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const void* q_packed, int n_groups_real,
-                       void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
+                       const int32_t* group_ntok, void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
   if (!c.tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
   const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_mtiles = n_groups_padded / 4;
@@ -582,9 +587,9 @@ int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, con
     hi = m_tile_hi < n_mtiles ? m_tile_hi : n_mtiles;
   }
   switch (kind_of_dtype(c.dtype)) {
-    case 0: return launch_tiles<0, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
-    case 1: return launch_tiles<1, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
-    case 2: return launch_tiles<2, false>(h, c, up, h->tmap_q, nullptr, n_groups_real, lo, hi, group_scores, ld, s);
+    case 0: return launch_tiles<0, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
+    case 1: return launch_tiles<1, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
+    case 2: return launch_tiles<2, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
     default: return set_error(h, B200MS_ESTATE, "score: corpus dtype has no wgmma scorer");
   }
 }
@@ -601,7 +606,7 @@ int launch_b1_tiles(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, cons
                     int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
   const int n_groups_padded = int(groups_padded(n_groups_real));
   if (int e = query_tmap(h, q_i8, B200MS_I8, n_groups_padded * kGroup)) return e;
-  return launch_tiles<1, true>(h, v, plan, h->tmap_q, tok_const, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
+  return launch_tiles<1, true>(h, v, plan, h->tmap_q, tok_const, nullptr, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
 }
 
 // 1-bit full scan: the query bits become +-1 int8 rows (b1_q_i8) and per-token constants, then the int8 kernel with the
