@@ -349,6 +349,47 @@ int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtyp
                                     int64_t n_docs, float i8_q_scale, float score_scale, float* doc_page_scores,
                                     int64_t* doc_page_ids, int32_t* doc_page_counts, int32_t* doc_counts, void* stream);
 
+/* ---- diversifying results (new; no reference counterpart) ---------------------------------------------------------------
+ * Maximal marginal relevance (MMR) over each query's candidate list: near-copies of a page picked already (a re-uploaded
+ * deck, a repeated slide template, the same figure on two pages) give way to pages that add something.  The call needs no
+ * query rows: relevance comes from the scores a search already reported, so it follows every search path (full scan,
+ * filtered scans, both first stages of the two-stage search, host-resident corpora).
+ * Per query q (cand_ids / cand_scores device [n_q, n_cand], as every search and rerank returns them; q_lens HOST):
+ *   rel_j  = cand_scores[q, j] / q_lens[q] in fp32 (a mean per query token); q_lens[q] == 0: rel_j = cand_scores[q, j].
+ *   sim(j -> s) = fp32(fp32(S) * score_scale) / len_j, every step rounded to fp32, where S = sum over the TRUE rows r of
+ *     page j of the max over the TRUE rows r' of page s of dot(j_r, s_r') -- how much of page j page s covers (directional).
+ *     The dot is the scan's per-row value on the packed rows (BF16: fp32 wgmma of bf16; F8: e4m3 widened to f16, fp32;
+ *     I8: exact s8 dot; B1: 128 - hamming) and the float value rule of b200ms_score holds for BF16 / F8 (max by fmaxf over
+ *     true rows, IEEE non-finite arithmetic).  S is an fp32 sum for BF16 / F8 (each 64-row tile of page j summed in row
+ *     order, the tiles added in order) and an exact int64 for I8 / B1 (1041 rows at +-127 pass int32).  score_scale is the
+ *     one the search reported its scores with (BF16 1, I8 / F8 1/scale^2, B1 1/128), so sim and rel share units.  A page
+ *     without rows, on either side, gives sim = 0.
+ *   red_j  = fmaxf over the pages picked so far of sim(j -> pick) (a NaN only when every one is NaN).
+ *   Pick 1 is the best slot by rel; every later pick the best live slot by
+ *     v_j = __fsub_rn(__fmul_rn(lambda_mult, rel_j), __fmul_rn(__fsub_rn(1, lambda_mult), red_j))
+ *   in the total order of b200ms_topk (-0 == +0, NaN above every number, NaNs tied), ties to the lower slot.  With
+ *   lambda_mult == 1, v_j = rel_j and red is never read (0 * inf cannot make a NaN): the result is the candidates in rel
+ *   order, which for a search's own list is its order.
+ *   Slots: an id of -1 or outside [0, n_pages) is unused and never picked; a page in several slots counts once, at its
+ *   earliest slot (the rule of b200ms_rerank_docs_batch_device).  count = min(k, distinct valid candidates).
+ * Outputs (device): out_ids int64 [n_q, k] in pick order, out_scores float32 [n_q, k] (each pick's cand_scores entry bit
+ * for bit), out_counts int32 [n_q]; unused entries -1 / -inf.  sims (NULL or float32 [n_q, k, n_cand]): sims[q, i, j] =
+ * sim(slot j -> pick i) for every slot j still unpicked after pick i (why a page was demoted, and by which pick); -inf for
+ * unused and repeated slots, for pick i itself and the picks before it, and for i >= count.
+ * Launches on cuda_stream, without a host synchronisation on an HBM corpus: a setup kernel, then two kernels per further
+ * pick (min(k, n_cand) picks at most), and two more for the last row of sims when it is asked for; lambda_mult == 1 without
+ * sims is the setup kernel alone.  Option "zero_pad_compat" is ignored.
+ * Host-resident corpora: the call's unique candidate pages are gathered once (b200ms_last_gather_stats reports it; the call
+ * synchronises cuda_stream), and the results are bit-identical to an HBM corpus of the same rows.  Every pair must be
+ * resident together, so a call whose unique candidate pages need more than one gather round (option "host_stage_bytes")
+ * is refused with B200MS_EINVAL.
+ * B200MS_EINVAL: NULL arguments, lambda_mult NaN or outside [0, 1], score_scale not finite and > 0, k < 1, n_cand outside
+ * [1, B200MS_MAX_K], n_q < 1, a negative query length, n_q * n_cand >= 2^30, the host-tier round rule above;
+ * B200MS_ESTATE: no corpus attached.  Nothing is launched when a call is refused. */
+int b200ms_mmr_device(b200ms_t* h, const int64_t* cand_ids, const float* cand_scores, int n_cand, const int32_t* q_lens,
+                      int n_q, int k, float lambda_mult, float score_scale, int64_t* out_ids, float* out_scores,
+                      int32_t* out_counts, float* sims, void* cuda_stream);
+
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the
  * path in B200MS_NCCL_LIB); b200ms_comm_available() says whether that worked.

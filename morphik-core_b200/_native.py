@@ -126,6 +126,7 @@ _SIGNATURES = {
     "b200ms_set_sign_rows": (c_int, [vp, vp, c_int64, vp]),
     "b200ms_sign_candidates_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, vp, vp, vp,
                                               vp]),
+    "b200ms_mmr_device": (c_int, [vp, vp, vp, c_int, i32p, c_int, c_int, c_float, c_float, vp, vp, vp, vp, vp]),
 }
 
 

@@ -317,7 +317,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
                        &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
-                       &h->compact_meta, &h->compact_bounce};
+                       &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   release_blocks(h);

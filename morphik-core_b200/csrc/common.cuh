@@ -260,6 +260,8 @@ struct b200ms {
   // buffer (compact.cu)
   std::vector<b200ms_block_t*> blocks;
   bms::DeviceBuf compact_meta, compact_bounce;
+  // diversifying results (maxsim_mmr.cu): per-call state of the greedy pick and the round kernels' per-tile partial sums
+  bms::DeviceBuf mmr_state, mmr_partials;
 };
 
 namespace bms {
@@ -346,6 +348,8 @@ inline CorpusView corpus_view(const b200ms_t* h) {
 int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStream_t s,
                      int (*round_fn)(b200ms_t*, const CorpusView&, const int64_t* remap, int r, int rounds, void* ctx),
                      void* ctx);
+// Gather rounds gather_host_tier needs for unique pages of `rows` padded rows in all (0 for none)
+int host_tier_rounds(const b200ms_t* h, int64_t rows);
 // Candidate scoring of a host-resident corpus: gather_host_tier over the candidate slots, every round scored through
 // score_round.
 int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_t ld, void* group_scores, cudaStream_t s,

@@ -154,6 +154,21 @@ static int grid_of(const b200ms_t* h, int64_t n) {
   return b < 1 ? 1 : int(b);
 }
 
+// round geometry: capacity cap rows (the budget, at least the largest page), pages starting in each W-row window
+static void round_geometry(const b200ms_t* h, int64_t* cap, int64_t* W) {
+  const Corpus& c = h->corpus;
+  int64_t cp = (h->host_stage_bytes / b200ms_row_bytes(c.dtype)) & ~int64_t(kGroup - 1);
+  if (cp < c.max_page_rows) cp = c.max_page_rows;
+  *cap = cp;
+  *W = cp - c.max_page_rows + kGroup;
+}
+
+int host_tier_rounds(const b200ms_t* h, int64_t rows) {
+  int64_t cap = 0, W = 0;
+  round_geometry(h, &cap, &W);
+  return int((rows + W - 1) / W);
+}
+
 int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStream_t s,
                      int (*round_fn)(b200ms_t*, const CorpusView&, const int64_t* remap, int r, int rounds, void* ctx),
                      void* ctx) {
@@ -189,10 +204,8 @@ int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStrea
   h->ht_unique = n_uniq;
   h->ht_bytes = rows * rb;
   if (rows == 0) return B200MS_OK;  // no valid candidate, or only empty pages: nothing to gather
-  // round geometry: capacity cap rows (the budget, at least the largest page), pages starting in each W-row window
-  int64_t cap = (h->host_stage_bytes / rb) & ~int64_t(kGroup - 1);
-  if (cap < c.max_page_rows) cap = c.max_page_rows;
-  const int64_t W = cap - c.max_page_rows + kGroup;
+  int64_t cap = 0, W = 0;
+  round_geometry(h, &cap, &W);
   const int rounds = int((rows + W - 1) / W);
   const int64_t stage_rows = rounds == 1 ? rows : cap;
   if (int e = reserve(h, h->ht_stage, size_t(stage_rows) * size_t(rb) + 1024)) return e;

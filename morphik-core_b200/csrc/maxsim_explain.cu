@@ -17,13 +17,13 @@
 #include "common.cuh"
 #include "mma_tile.cuh"
 #include "ptx.cuh"
+#include "row_tiles.cuh"
 
 namespace bms {
 
-constexpr int kExplainTokens = 64;      // query tokens per work item (one wgmma M block)
-constexpr int kExplainThreads = 128;    // one warpgroup
-constexpr int kExplainB1Threads = 256;  // 1-bit kernel: 8 warps, one token each at a time
-constexpr uint32_t kABlockPanel = 64 * 128;  // one 128-byte K panel of the 64-row A block
+constexpr int kExplainTokens = kABlockRows;       // query tokens per work item (one wgmma M block)
+constexpr int kExplainThreads = kRowTileThreads;  // one warpgroup
+constexpr int kExplainB1Threads = 256;            // 1-bit kernel: 8 warps, one token each at a time
 
 struct ExplainArgs {
   const void* q = nullptr;            // packed query rows of the corpus dtype (b200ms_pack_queries layout)
@@ -126,38 +126,20 @@ __device__ __forceinline__ void write_token(const ExplainArgs& a, const ExplainI
   a.best_rows[x.slot * a.t_max + t] = ok ? bi : -1;
 }
 
-// one 128-byte-row K-major SWIZZLE_128B atom: row r, 16-byte chunk c (0..7) of a panel
-__device__ __forceinline__ uint32_t sw128_off(int r, int c) {
-  return uint32_t(r >> 3) * 1024u + uint32_t(r & 7) * 128u + ((uint32_t(c) ^ uint32_t(r & 7)) << 4);
-}
-
 // ------------------------------------------------------------------ dense dtypes on wgmma
-// KIND 0 bf16, 1 int8, 2 fp8 e4m3 (widened to f16 in shared memory on both operands)
+// KIND 0 bf16, 1 int8, 2 fp8 e4m3 (widened to f16 in shared memory on both operands); the tile loop is row_tiles.cuh's
 template <int KIND>
 __global__ void __launch_bounds__(kExplainThreads)
 maxsim_explain_wgmma(const __grid_constant__ ExplainArgs a) {
   using K = Kind<KIND>;
   using Acc = typename K::Acc;
-  constexpr int kSrcChunks = KIND == 0 ? 16 : 8;  // 16-byte pieces of one stored row
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t b_addr = smem_u32(smem);                   // [kPanels][128 rows x 128 B]
   const uint32_t a_addr = b_addr + K::kPanels * kSubtileBytes;  // [kPanels][64 rows x 128 B]
-  const int r = threadIdx.x;  // B: row r of every page tile
-  const int warp = r >> 5, lane = r & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint4* qrows = static_cast<const uint4*>(a.q);
   const uint4* prows = static_cast<const uint4*>(a.rows);
-
-  // 16-byte piece c of a stored row -> shared memory (e4m3: two f16 pieces)
-  auto put = [&](uint32_t base, uint32_t panel_bytes, int row, int c, const uint4& v) {
-    if constexpr (KIND == 2) {
-      const uint4 lo = e4m3x8_to_f16x8(v.x, v.y), hi = e4m3x8_to_f16x8(v.z, v.w);
-      st_shared_v4(base + uint32_t((2 * c) >> 3) * panel_bytes + sw128_off(row, (2 * c) & 7), lo);
-      st_shared_v4(base + uint32_t((2 * c + 1) >> 3) * panel_bytes + sw128_off(row, (2 * c + 1) & 7), hi);
-    } else {
-      st_shared_v4(base + uint32_t(c >> 3) * panel_bytes + sw128_off(row, c & 7), v);
-    }
-  };
 
   const int n_slots = a.n_q * a.n_cand;
   for (int tt = blockIdx.y; tt < a.n_ttiles; tt += gridDim.y)
@@ -170,100 +152,53 @@ maxsim_explain_wgmma(const __grid_constant__ ExplainArgs a) {
     }
     const int padded = (x.len + kGroup - 1) & ~(kGroup - 1);
     const int n_tiles = (padded + kTileN - 1) / kTileN;
-    uint4 nxt[kSrcChunks];
-    auto fetch = [&](int n) {
-      const int row = n * kTileN + r;
-#pragma unroll
-      for (int c = 0; c < kSrcChunks; ++c) nxt[c] = make_uint4(0, 0, 0, 0);
-      if (row < padded) {
-#pragma unroll
-        for (int c = 0; c < kSrcChunks; ++c) nxt[c] = __ldg(prows + (x.row0 + row) * kSrcChunks + c);
-      }
-    };
-    fetch(0);
-    __syncthreads();  // the previous item's wgmmas have read the A block
-    {
-      const int64_t qrow0 = int64_t(__ldg(a.goff + x.q)) * kGroup + x.t0;
-      constexpr int kPieces = kExplainTokens * kSrcChunks / kExplainThreads;
-#pragma unroll
-      for (int k = 0; k < kPieces; ++k) {
-        const int p = r + k * kExplainThreads;
-        const int row = p / kSrcChunks, c = p % kSrcChunks;
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (qrow0 + row < a.q_rows) v = __ldg(qrows + (qrow0 + row) * kSrcChunks + c);
-        put(a_addr, kABlockPanel, row, c, v);
-      }
-    }
     // per token (accumulator rows m0 = 16 warp + lane/4 and m0 + 8): this lane's running max and lowest row
     Acc bv0 = Acc(0), bv1 = Acc(0);
     int bi0 = -1, bi1 = -1;
     const int m0 = 16 * warp + (lane >> 2);
     const int tok0 = x.t0 + m0, tok1 = tok0 + 8;
-    for (int n = 0; n < n_tiles; ++n) {
-      if (n > 0) __syncthreads();  // the previous tile's wgmmas have read the B tile
-#pragma unroll
-      for (int c = 0; c < kSrcChunks; ++c) put(b_addr, kSubtileBytes, r, c, nxt[c]);
-      fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
-      __syncthreads();
-      Acc d[64];
-      wgmma_fence();
-      {
-        const uint64_t ad = wgmma_desc_kmajor_sw128(a_addr), bd = wgmma_desc_kmajor_sw128(b_addr);
-#pragma unroll
-        for (int ks = 0; ks < K::kKSteps; ++ks) {  // 32 B of K per step, 4 steps per 128 B panel: the scan's order
-          const uint32_t ao = ((ks >> 2) * kABlockPanel + (ks & 3) * 32) >> 4;
-          const uint32_t bo = ((ks >> 2) * kSubtileBytes + (ks & 3) * 32) >> 4;
-          if constexpr (KIND == 0) {
-            wgmma_m64n128k16_bf16(d, ad + ao, bd + bo, ks != 0);
-          } else if constexpr (KIND == 1) {
-            wgmma_m64n128k32_s8(d, ad + ao, bd + bo, ks != 0);
-          } else {
-            wgmma_m64n128k16_f16(d, ad + ao, bd + bo, ks != 0);
-          }
-        }
-        wgmma_commit();
-      }
-      if (n + 1 < n_tiles) fetch(n + 1);  // in flight while the chain runs
-      wgmma_wait<0>();
-      reg_fence_all(d);
-      const int rbase = n * kTileN + 2 * (lane & 3);
-#pragma unroll
-      for (int jb = 0; jb < 16; ++jb) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int row = rbase + 8 * jb + e;
-          if (row < x.len) {
-            if (beats(d[4 * jb + e], row, bv0, bi0)) {
-              bv0 = d[4 * jb + e];
-              bi0 = row;
-            }
-            if (beats(d[4 * jb + 2 + e], row, bv1, bi1)) {
-              bv1 = d[4 * jb + 2 + e];
-              bi1 = row;
-            }
-          }
-        }
-      }
-      if (a.sim_map) {
-        const float ninf = -__int_as_float(0x7f800000);
-#pragma unroll
-        for (int h2 = 0; h2 < 2; ++h2) {
-          const int t = h2 ? tok1 : tok0;
-          if (t >= x.t1) continue;
-          const bool live = t < x.qlen;
+    const int64_t qrow0 = int64_t(__ldg(a.goff + x.q)) * kGroup + x.t0;
+    rows_vs_page_tiles<KIND>(
+        a_addr, b_addr, prows, x.row0, padded, [&] { load_a_block<KIND>(a_addr, qrows, qrow0, a.q_rows); },
+        [&](const Acc(&d)[64], int n) {
+          const int rbase = n * kTileN + 2 * (lane & 3);
 #pragma unroll
           for (int jb = 0; jb < 16; ++jb) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int row = rbase + 8 * jb + e;
-              if (row < a.map_rows)
-                a.sim_map[map_index(a, x.slot, t, row)] =
-                    (live && row < x.len) ? float(d[4 * jb + 2 * h2 + e]) * a.scale : ninf;
+              if (row < x.len) {
+                if (beats(d[4 * jb + e], row, bv0, bi0)) {
+                  bv0 = d[4 * jb + e];
+                  bi0 = row;
+                }
+                if (beats(d[4 * jb + 2 + e], row, bv1, bi1)) {
+                  bv1 = d[4 * jb + 2 + e];
+                  bi1 = row;
+                }
+              }
             }
           }
-        }
-      }
-    }
+          if (a.sim_map) {
+            const float ninf = -__int_as_float(0x7f800000);
+#pragma unroll
+            for (int h2 = 0; h2 < 2; ++h2) {
+              const int t = h2 ? tok1 : tok0;
+              if (t >= x.t1) continue;
+              const bool live = t < x.qlen;
+#pragma unroll
+              for (int jb = 0; jb < 16; ++jb) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int row = rbase + 8 * jb + e;
+                  if (row < a.map_rows)
+                    a.sim_map[map_index(a, x.slot, t, row)] =
+                        (live && row < x.len) ? float(d[4 * jb + 2 * h2 + e]) * a.scale : ninf;
+                }
+              }
+            }
+          }
+        });
     shfl_best(bv0, bi0, 1);
     shfl_best(bv0, bi0, 2);
     shfl_best(bv1, bi1, 1);
@@ -333,11 +268,11 @@ static int launch_explain(b200ms_t* h, const ExplainArgs& a, int dtype, cudaStre
     maxsim_explain_b1<<<grid, kExplainB1Threads, 0, s>>>(a);
   } else {
     const void* kern = nullptr;
-    int smem = 1024;
+    int smem = 0;
     switch (kind_of_dtype(dtype)) {
-      case 0: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<0>); smem += 3 * Kind<0>::kPanels * kABlockPanel; break;
-      case 1: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<1>); smem += 3 * Kind<1>::kPanels * kABlockPanel; break;
-      case 2: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<2>); smem += 3 * Kind<2>::kPanels * kABlockPanel; break;
+      case 0: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<0>); smem = row_tiles_smem<0>(); break;
+      case 1: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<1>); smem = row_tiles_smem<1>(); break;
+      case 2: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<2>); smem = row_tiles_smem<2>(); break;
       default: return set_error(h, B200MS_ESTATE, "explain: corpus dtype has no scorer");
     }
     if (int e = ensure_smem(h, kern, smem, "cudaFuncSetAttribute(maxsim_explain_wgmma)")) return e;

@@ -933,6 +933,43 @@ class MaxSimIndex:
                 "b200ms_explain_device")
         return ts, br, sm
 
+    # ------------------------------------------------------------------ diversifying results
+    def mmr(self, cand_ids: torch.Tensor, cand_scores: torch.Tensor, q_lens: Sequence[int], k: int, lambda_mult: float,
+            with_sims: bool = False):
+        """Maximal marginal relevance over each query's candidate list (b200ms_mmr_device), asynchronous on torch's current
+        stream.  cand_ids int64 / cand_scores float32 [n_q, n_cand] on the device, as a search or rerank returned them (-1 =
+        unused slot); q_lens the queries' token counts (relevance is score / tokens).  Picks greedily: first the most
+        relevant page, then each time the page maximising lambda_mult * relevance - (1 - lambda_mult) * (its largest
+        page-to-page MaxSim against a page picked already, per row of its own).  k is capped at n_cand.
+
+        Returns device tensors (page ids int64 [n_q, k] in pick order, their input scores float32 [n_q, k], counts int32
+        [n_q]) and, with ``with_sims``, sims float32 [n_q, k, n_cand]: sims[q, i, j] = the similarity of slot j to pick i,
+        for the slots still unpicked after pick i (-inf elsewhere).  Works on both tiers; a host-tier call whose candidate
+        pages do not fit one staging round raises NativeError."""
+        n_q = len(q_lens)
+        if cand_ids.ndim != 2 or cand_ids.shape[0] != n_q:
+            raise ValueError(f"cand_ids must be [n_q = {n_q}, n_cand], got {tuple(cand_ids.shape)}")
+        n_cand, kk = _check_candidates(cand_ids, n_q, k, self.device, per_query=True)
+        if (cand_scores.dtype != torch.float32 or tuple(cand_scores.shape) != tuple(cand_ids.shape)
+                or not cand_scores.is_contiguous() or cand_scores.device != self.device):
+            raise ValueError(f"cand_scores must be a contiguous float32 {list(cand_ids.shape)} tensor on {self.device}")
+        if not 0.0 <= float(lambda_mult) <= 1.0:  # NaN fails too
+            raise ValueError(f"lambda_mult must be in [0, 1], got {lambda_mult}")
+        if int(k) < 1 or n_cand < 1:
+            raise ValueError("k and n_cand must be >= 1")
+        if any(int(t) < 0 for t in q_lens):
+            raise ValueError("query lengths must be >= 0")
+        ts, ti, tc = _topk_outputs(n_q, kk, self.device)
+        sims = torch.empty((n_q, kk, n_cand), dtype=torch.float32, device=self.device) if with_sims else None
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_mmr_device(self.h.ptr, _vp(cand_ids), _vp(cand_scores), n_cand, nat.i32_array(q_lens), n_q, kk,
+                                          ctypes.c_float(lambda_mult), ctypes.c_float(self.score_scale), _vp(ti), _vp(ts),
+                                          _vp(tc), _vp(sims), self._stream()),
+                "b200ms_mmr_device")
+        return (ti, ts, tc, sims) if with_sims else (ti, ts, tc)
+
     # ------------------------------------------------------------------ multi-GPU (document shards, NCCL inside libb200ms)
     @staticmethod
     def comm_unique_id() -> bytes:

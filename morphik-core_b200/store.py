@@ -452,6 +452,60 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                     out.append(chunks)
             return out
 
+    async def query_similar_mmr(self, query_embedding, k: int, fetch_k: int = 20, lambda_mult: float = 0.5,
+                                doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None) -> List[DocumentChunk]:
+        """k chunks that are relevant AND different from each other (extension; LangChain's
+        ``max_marginal_relevance_search``): the store's own search (exhaustive or two-stage) fetches the best
+        ``max(fetch_k, k)`` chunks under the ``doc_ids`` / ``app_id`` filter, then maximal marginal relevance picks k of them on
+        the GPU (MaxSimIndex.mmr): first the best chunk, then each time the chunk maximising ``lambda_mult`` * relevance -
+        (1 - ``lambda_mult``) * its page-to-page MaxSim against the chunks picked already.  ``lambda_mult`` = 1 is
+        query_similar's ranking, 0 the most diverse.  Chunks come in pick order with query_similar's scores.  Mask, search,
+        MMR and chunk construction are one critical section; ``last_query_timing["mmr_ms"]`` is the MMR call's device time."""
+        q = as_query_matrix(query_embedding)
+        if not 0.0 <= float(lambda_mult) <= 1.0:  # NaN fails too
+            raise ValueError(f"lambda_mult must be in [0, 1], got {lambda_mult}")
+        if k <= 0:
+            return []
+        return await asyncio.to_thread(self._search_mmr_locked, q, int(k), int(fetch_k), float(lambda_mult), doc_ids, app_id)
+
+    def _search_mmr_locked(self, q, k, fetch_k, lambda_mult, doc_ids, app_id):
+        import torch
+
+        t0 = time.perf_counter()
+        with self._lock:
+            n = len(self.catalog)
+            if n == 0:
+                return []
+            visible, words = self.catalog.allow_words(doc_ids, app_id)
+            if not visible:
+                return []
+            fetch = min(_capped_k(max(fetch_k, k)), n)
+            t1 = time.perf_counter()
+            ts, ti, tc = self._search_unlocked([q], fetch, words)
+            t2 = time.perf_counter()
+            count = int(tc[0])
+            if count == 0:
+                return []
+            dev = torch.device(self._index.device)
+            cand_ids = torch.from_numpy(np.ascontiguousarray(ti[:1, :count], dtype=np.int64)).to(dev)
+            cand_scores = torch.from_numpy(np.ascontiguousarray(ts[:1, :count], dtype=np.float32)).to(dev)
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if dev.type == "cuda" else None
+            if ev:
+                ev[0].record(torch.cuda.current_stream(dev))
+            mi, ms, mc = self._index.mmr(cand_ids, cand_scores, [int(q.shape[0])], min(k, count), lambda_mult)
+            if ev:
+                ev[1].record(torch.cuda.current_stream(dev))
+            mi, ms, mc = (np.asarray(t.cpu()) for t in (mi, ms, mc))  # waits for the call
+            t3 = time.perf_counter()
+            mmr_ms = ev[0].elapsed_time(ev[1]) if ev else (t3 - t2) * 1e3
+            out = self._chunks(ms[0], mi[0], int(mc[0]))
+            t4 = time.perf_counter()
+        self.last_query_timing = {"prepare_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3, "mmr_ms": float(mmr_ms),
+                                  "build_chunks_ms": (t4 - t3) * 1e3, "total_ms": (t4 - t0) * 1e3}
+        if self._two_stage is not None:
+            self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
+        return out
+
     async def get_chunks_by_id(self, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
                                skip_image_content: bool = False) -> List[DocumentChunk]:
         if not chunk_identifiers:
