@@ -188,6 +188,8 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
 /* ---- the hot path ---------------------------------------------------------------------------- */
 /* group_scores[g, p] = sum over the (<=32) true tokens of group g of max over the rows of page p of <q_t, d_r>
  *   BF16 / F8 corpus: float32 (fp32 accumulate on wgmma);  I8: int32 exact;  B1: int32 sum_t max_r (128 - hamming).
+ *   (A group holds at most 32 tokens, so its I8 score fits int32; a whole query's sum need not -- see b200ms_topk for the
+ *   I32 sum rule every selection and reported score follows.)
  * q_packed: device [roundup(n_groups,4)*32, 128] of the corpus dtype; q_lens/group_offsets (HOST) as produced by
  * b200ms_pack_queries.  With both given, the true tokens of each group are the query's (the zero padding rows of a group
  * add +0).  B1 needs them; for BF16 / I8 / F8 they may be NULL, and then every row of q_packed counts as a token, the zero
@@ -222,13 +224,17 @@ int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, const int32_t*
                  int n_q, void* group_scores, int64_t ld, void* stream);
 
 /* Per query: sum[p] = the group scores group_scores[g, p], g in [group_offsets[q], group_offsets[q+1]), added in order to
- * +0 (float32, or int32 for score_dtype I32: the caller keeps the sums in range); keep the k best pages whose bit is set
- * in allow_mask (device, bit p&31 of word p>>5; NULL = all; bits at p >= n_pages are ignored), ordered by sum DESC then
- * page id ASC (the reference leaves ties unspecified).  The order is total: -0 ties with +0, every NaN ranks above every
- * number (+inf included) and NaNs tie with each other -- as torch.topk and Postgres ORDER BY ... DESC order them.  I32
- * sums are ranked exactly, also where float32 would merge them.  Columns p >= n_pages (ld > n_pages) are never read.
- * Reported score = float32(sum) * scale in fp32 (a NaN as 0x7fffffff).  Outputs are device arrays: top_scores/top_ids
- * [n_q, k] (unused slots: -inf / -1), top_counts [n_q].  id_base is added to every page id (global ids of a shard). */
+ * +0; keep the k best pages whose bit is set in allow_mask (device, bit p&31 of word p>>5; NULL = all; bits at
+ * p >= n_pages are ignored), ordered by sum DESC then page id ASC (the reference leaves ties unspecified).  The order is
+ * total: -0 ties with +0, every NaN ranks above every number (+inf included) and NaNs tie with each other -- as torch.topk
+ * and Postgres ORDER BY ... DESC order them.  Columns p >= n_pages (ld > n_pages) are never read.
+ * Sums of score_dtype F32 are float32.  Sums of score_dtype I32 (the "I32 sum rule"): the group scores are added in int64
+ * and the sum is clamped to +-(2^31 - 1).  Pages whose clamped sums differ are ranked exactly, also where float32 would
+ * merge them; pages whose sums lie beyond the bound tie at it (lower page id first).  An int8 query of 1041 or more tokens
+ * (1033 or more against -128 codes) can get there: a token scores at most 128 * 127^2 (128 * 127 * 128).
+ * Reported score = float32(sum) * scale in fp32, of the clamped sum for I32 (a NaN as 0x7fffffff).  Outputs are device
+ * arrays: top_scores/top_ids [n_q, k] (unused slots: -inf / -1), top_counts [n_q].  id_base is added to every page id
+ * (global ids of a shard). */
 int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
                 const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, int k, float scale, int64_t id_base,
                 float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream);
@@ -268,7 +274,9 @@ int b200ms_search_device_masked(b200ms_t* h, const void* q_dev, int src_dtype, c
                                 float i8_q_scale, float score_scale, int64_t id_base, float* top_scores_dev,
                                 int64_t* top_ids_dev, int32_t* top_counts_dev, void* stream);
 
-/* MaxSim over an explicit candidate list (the "rerank" half of a two-stage search, fast_multivector_store.py:545-557;
+/* The searches above rank and report I8 / B1 pages by the I32 sum rule of b200ms_topk, and so do the reranks and document
+ * calls below.
+ * MaxSim over an explicit candidate list (the "rerank" half of a two-stage search, fast_multivector_store.py:545-557;
  * BF16 / F8 scores follow the float value rule of b200ms_score, so do the rerank and document calls below):
  * cand_ids_dev = device array of n_cand page ids (-1, or any id outside [0, n_pages) = unused slot; a page may appear in
  * several slots).  Only those pages are scanned; ties break towards the earlier candidate slot (= better first-stage rank),
@@ -292,8 +300,10 @@ int b200ms_rerank_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, co
  * sim() is the search's own per-token value, in the units of the reported score:
  *   BF16 / F8 fp32 dot (times score_scale), I8 int32 dot (times score_scale), B1 (128 - hamming) (times score_scale).
  * The dense dtypes compute it on the scan's tensor-core instructions in the scan's order, so the map holds the very values the
- * scan took its max over: sum_t token_scores[q, j, t] is the score b200ms_rerank_batch_device reports for that page (exactly
- * for I8 / B1; for BF16 / F8 up to the order of the float32 sum over tokens), and token_scores == sim_map at best_rows.
+ * scan took its max over: sum_t token_scores[q, j, t] is the score b200ms_rerank_batch_device reports for that page (for
+ * I8 / B1 exactly while the int64 sum of the integer token values lies within +-(2^31 - 1); beyond it the rerank reports
+ * the bound, by the I32 sum rule of b200ms_topk; for BF16 / F8 up to the order of the float32 sum over tokens), and
+ * token_scores == sim_map at best_rows.
  * q_dev: F32 | BF16 rows [sum q_lens, 128]; q_lens HOST; page_ids_dev device int64 [n_q, n_cand] (-1 or outside
  * [0, n_pages) = unused slot; a page may appear in several slots); t_max = max(q_lens).  Outputs are device arrays:
  *   token_scores / best_rows [n_q, n_cand, t_max], sim_map [n_q, n_cand, t_max, map_rows].
@@ -332,7 +342,7 @@ int b200ms_explain_device(b200ms_t* h, const void* q_dev, int src_dtype, const i
  * B200MS_EINVAL: NULL outputs or page_doc, k outside [1, 4096], per_doc outside [1, B200MS_MAX_PER_DOC], n_docs < 1 while
  * pages exist, n_docs > n_pages, and the per-call bounds of the flat call;  B200MS_ESTATE: as the flat call (no corpus; a
  * full scan of a host-resident corpus).  Nothing is launched when a call is refused. */
-/* over a score matrix, like b200ms_topk (group_offsets HOST, one allow mask or NULL) */
+/* over a score matrix, like b200ms_topk (group_offsets HOST, one allow mask or NULL; I32 sums by its I32 sum rule) */
 int b200ms_topk_docs(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
                      const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, const int32_t* page_doc, int64_t n_docs,
                      int k, int per_doc, float scale, int64_t id_base, float* doc_page_scores, int64_t* doc_page_ids,

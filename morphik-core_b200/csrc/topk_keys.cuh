@@ -21,13 +21,25 @@ __device__ __forceinline__ float score_of_key(uint32_t k, float) {
 }
 __device__ __forceinline__ float score_of_key(uint32_t k, int) { return float(int(k ^ 0x80000000u)); }
 
+// The type a page's group scores are added in: float32 for float scores; int64 for I32 scores, whose sum can pass int32
+// (an int8 token scores up to 128 * 127^2, so a query of 1041 tokens can).  finish_sum saturates that int64 sum to
+// +-(2^31 - 1): the order stays exact inside the range, pages beyond it tie at the bound, and no sum wraps to the other
+// sign.  The bound is symmetric, so a sum never reaches INT32_MIN, whose key is 0.
+template <typename T> struct SumOf { using type = T; };
+template <> struct SumOf<int> { using type = int64_t; };
+constexpr int64_t kI32SumBound = 2147483647;
+__device__ __forceinline__ float finish_sum(float s) { return s; }
+__device__ __forceinline__ int finish_sum(int64_t s) {
+  return int(s < -kI32SumBound ? -kI32SumBound : s > kI32SumBound ? kI32SumBound : s);
+}
+
 template <typename T>
 __device__ __forceinline__ bool page_key(const T* __restrict__ gs, int64_t ld, int g0, int g1, const uint32_t* allow,
                                          int64_t p, uint32_t* key) {
   if (allow && !((__ldg(allow + (p >> 5)) >> (p & 31)) & 1u)) return false;
-  T acc = T(0);
+  typename SumOf<T>::type acc = 0;
   for (int g = g0; g < g1; ++g) acc += __ldg(gs + int64_t(g) * ld + p);
-  *key = key_of(acc);
+  *key = key_of(finish_sum(acc));
   return true;
 }
 

@@ -21,6 +21,18 @@ TOL = {"bf16": 3e-5, "fp8": 1e-4, "int8": 0.0, "binary": 0.0}
 I8_SCALE = 127.0
 F8_SCALE = 64.0
 SCORE_QUANTUM = {"int8": 1.0 / (I8_SCALE * I8_SCALE), "binary": 1.0 / 128.0}
+I32_SUM_BOUND = (1 << 31) - 1
+
+
+def i32_sum(sums) -> np.ndarray:
+    """The I32 sum rule of b200ms_topk: a page's exact (int64) sum of I32 group scores, clamped to +-(2^31 - 1).  This is
+    what int8 and 1-bit pages are ranked by (ties at the bound break by id, or slot, like any tie)."""
+    return np.clip(np.asarray(sums, np.int64), -I32_SUM_BOUND, I32_SUM_BOUND)
+
+
+def i32_reported(sums, scale: float) -> np.ndarray:
+    """The score reported for exact (int64) sums: float32(i32_sum(sums)) * float32(scale), rounded to float32."""
+    return (i32_sum(sums).astype(np.float32) * np.float32(scale)).astype(np.float32)
 
 
 def _concat(pages: Sequence[np.ndarray]) -> np.ndarray:

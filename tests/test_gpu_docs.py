@@ -2,9 +2,9 @@
 b200ms_search_docs_device, b200ms_rerank_docs_batch_device and B200MultiVectorStore.query_similar_documents.
 
 The grouped result is a pure function of the flat ranking, so every check is exact: ids, counts and score bits.
-  - b200ms_topk_docs on crafted matrices (F32 and I32, ties, NaN, +-0, +-inf, out-of-range page_doc, an allow mask, one
-    document, k > n_docs, per_doc > pages per document, n_pages > 8192 with a k that slices) against tests/docs_oracle.py,
-    and the identity grouping against b200ms_topk;
+  - b200ms_topk_docs on crafted matrices (F32 and I32, I32 sums past +-2^31, ties, NaN, +-0, +-inf, out-of-range page_doc,
+    an allow mask, one document, k > n_docs, per_doc > pages per document, n_pages > 8192 with a k that slices) against
+    tests/docs_oracle.py, and the identity grouping against b200ms_topk;
   - full scans of every corpus dtype against host grouping of the GPU's own flat ranking, unmasked, with one mask, with
     per-query masks, with zero_pad_compat; above 8192 pages against grouping of score_groups' float32 sums;
   - per-query candidate lists with unused slots, ids past the corpus and repeated pages against grouping of
@@ -29,8 +29,10 @@ from morphik_core_b200 import _native as nat  # noqa: E402
 from morphik_core_b200.index import MaxSimIndex  # noqa: E402
 from morphik_core_b200.models import DocumentChunk  # noqa: E402
 from morphik_core_b200.store import B200MultiVectorStore  # noqa: E402
+from oracle.scoring import i32_sum  # noqa: E402
 
 F32 = np.float32
+INT_MAX = (1 << 31) - 1
 CANON_NAN = np.uint32(0x7FFFFFFF)
 EINVAL, ESTATE = -1, -3
 
@@ -105,7 +107,9 @@ def f32_values(rng, shape):
 
 
 def i32_values(rng, shape):
-    pool = np.asarray([0, 1, -1, 1 << 26, (1 << 26) + 1, -(1 << 27)], np.int64)
+    """Group scores whose sums over 2 or 3 groups pass +-2^31, land on +-(2^31 - 1), one past it and next to it."""
+    pool = np.asarray([0, 1, -1, 1 << 26, (1 << 26) + 1, -(1 << 27), INT_MAX, INT_MAX - 1, -INT_MAX, -(1 << 31), 1 << 30],
+                      np.int64)
     v = rng.integers(-(1 << 28), 1 << 28, size=shape, dtype=np.int64)
     m = rng.random(shape) < 0.6
     v[m] = rng.choice(pool, size=int(m.sum()))
@@ -194,7 +198,7 @@ def test_topk_docs_against_the_oracle(sdt, case):
                 acc = (acc + vals[g, :n_pages]).astype(F32)
             rep = (acc * F32(scale)).astype(F32)
         else:
-            acc = vals[goff[q]:goff[q + 1], :n_pages].astype(np.int64).sum(axis=0)
+            acc = i32_sum(vals[goff[q]:goff[q + 1], :n_pages].astype(np.int64).sum(axis=0))  # the I32 sum rule
             rep = (acc.astype(F32) * F32(scale)).astype(F32)
         pos, ids, pc, nd = topk_docs_np(acc, page_doc, n_docs, k, per_doc, allow=allow)
         sc = np.where(pos >= 0, rep[np.maximum(pos, 0)], F32(-np.inf)).astype(F32)

@@ -9,8 +9,8 @@ random draw.  One random ragged corpus with empty pages covers zero_pad_compat, 
 Paths: the full scan (NM = 1 / 2 / 4 / 8 resident query tiles, phantom tiles, several passes; max_ctas default / 1 / 3;
 unit_rows default / 64 / 400), top-k with and without allow-masks, the shared-list and per-query reranks (duplicate ids,
 -1 and ids past the corpus as unused slots, empty pages, queries of 1 .. 300 tokens), zero_pad_compat, and the two-level
-(sliced) top-k of a rerank with exact ties.  Exhaustive value tests: every product of two finite e4m3 codes and of two int8
-values in -127..127.
+(sliced) top-k of a rerank with exact ties.  Exhaustive value tests: every product of two finite e4m3 codes, of two int8
+values in -127..127, and of an int8 query value with every packed code -128..127.
 """
 import ctypes
 import functools
@@ -284,7 +284,9 @@ def test_fp8_every_product_of_two_finite_codes_is_exact():
 
 
 def test_int8_every_product_of_two_values_is_exact():
-    """The same construction over int8 values -127 .. 127: score = a * b exactly."""
+    """The same construction over int8 values -127 .. 127: score = a * b exactly.  The quantiser never writes -128, but
+    packed rows may hold it: a second corpus of every code -128 .. 127, loaded through append_packed, must give every
+    product of a query value and a code exactly too."""
     vals = np.arange(-127, 128)
     qs = []
     for a in vals:
@@ -303,3 +305,14 @@ def test_int8_every_product_of_two_values_is_exact():
     want = np.outer(vals, vals)
     bad = np.argwhere(raw != want)
     assert not len(bad), [(int(vals[a]), int(vals[b]), raw[a, b], want[a, b]) for a, b in bad[:5]]
+    codes = np.arange(-128, 128)
+    rows = np.repeat(np.repeat(codes[:, None], 128, axis=1), 32, axis=0).astype(np.int8)  # page c: 32 rows of code c
+    every = MaxSimIndex(dtype="int8")
+    every.append_packed(torch.from_numpy(rows.view(np.uint8)).cuda(), [1] * len(codes))
+    assert np.array_equal(every.packed_rows().cpu().numpy().view(np.int8)[::32, 0], codes.astype(np.int8))
+    scores, goff, n_pages, _ = every.score_groups(qs)
+    torch.cuda.synchronize()
+    raw = scores[: len(vals), :n_pages].cpu().numpy().astype(np.int64)
+    want = np.outer(vals, codes)
+    bad = np.argwhere(raw != want)
+    assert not len(bad), [(int(vals[a]), int(codes[b]), raw[a, b], want[a, b]) for a, b in bad[:5]]

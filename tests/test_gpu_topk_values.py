@@ -2,8 +2,10 @@
 
 Score matrices are built on the host and handed to the C-ABI directly.  The oracle (oracle/maxsim_oracle.rank_desc_np) is
 the documented total order: score DESC then id ASC, -0 == +0, every NaN above every number and NaNs tied.  Sums are formed
-as the header says (groups in order from +0.0f in float32, int32 for I32 scores), and a reported score is
-float32(sum) * scale in fp32 -- compared bit for bit, a NaN as 0x7fffffff.
+as the header says (groups in order from +0.0f in float32; for I32 scores in int64, clamped to +-(2^31 - 1)), and a
+reported score is float32(sum) * scale in fp32 -- compared bit for bit, a NaN as 0x7fffffff.  The I32 class "overflow"
+has sums past +-2^31: every group at INT32_MAX or INT32_MIN, alternating signs, sums exactly at +-(2^31 - 1), one past
+it and 2^31 - 2, so that a wrapped, truncated or misplaced bound changes the order.
 
 Boundaries: n_pages 1024 / 1025 (counting kernel vs radix select), multiples of 8192 (slice count), k at and around the
 slice cap 8192 / k, k above the number of allowed pages; columns past n_pages (ld > n_pages) hold sentinels that would
@@ -23,6 +25,7 @@ if not torch.cuda.is_available():  # pragma: no cover - the gpu marker normally 
 
 from morphik_core_b200 import _native as nat  # noqa: E402
 from oracle import maxsim_oracle as orc  # noqa: E402
+from oracle.scoring import i32_sum  # noqa: E402
 
 F32 = np.float32
 INT_MAX = (1 << 31) - 1
@@ -87,7 +90,16 @@ def f32_class(name, rng, shape):
 
 
 F32_CLASSES = ["equal", "two", "zeros", "inf", "subnormal", "nan", "gauss"]
-I32_CLASSES = ["equal", "two", "extremes", "large"]
+I32_CLASSES = ["equal", "two", "extremes", "large", "overflow"]
+GROUPS = {"overflow": 4}  # groups of a class's query (default (i % 4) + 1)
+INT_MIN = -(1 << 31)
+# group scores of the "overflow" class (4 groups): sums beyond +-(2^31 - 1), at it, one past it and next to it
+OVERFLOW_ROWS = np.asarray([
+    [INT_MAX, INT_MAX, INT_MAX, INT_MAX], [INT_MIN, INT_MIN, INT_MIN, INT_MIN], [INT_MAX, 0, 0, 0], [INT_MAX - 1, 0, 0, 0],
+    [INT_MAX - 3, 1, 1, 1], [INT_MAX - 3, 1, 1, 2], [INT_MAX, 1, 0, 0], [1 << 30, 1 << 30, 0, 0], [1 << 30, 1 << 30, -1, 0],
+    [INT_MIN, 0, 0, 0], [-INT_MAX, 0, 0, 0], [-INT_MAX + 1, 0, 0, 0], [INT_MIN, 1, 0, 0], [INT_MIN, -1, 0, 0],
+    [INT_MAX, -INT_MAX, INT_MAX, -INT_MAX], [INT_MAX, INT_MAX, INT_MIN, INT_MIN], [INT_MAX, INT_MAX, INT_MAX, INT_MIN],
+    [INT_MIN, INT_MIN, INT_MAX, 5], [(1 << 24) + 1, 0, 0, 0], [1 << 24, 0, 0, 0], [12345, 0, 0, 0]], np.int64)
 
 
 def split_sum(rng, total, parts):
@@ -101,6 +113,10 @@ def split_sum(rng, total, parts):
 
 
 def i32_class(name, rng, groups, n):
+    if name == "overflow":  # summands that pass int32 on their own
+        parts = OVERFLOW_ROWS[rng.integers(0, len(OVERFLOW_ROWS), size=n)].T
+        assert parts.shape[0] == groups
+        return parts.astype(np.int32), parts.sum(axis=0)
     if name == "equal":
         tot = np.full(n, 12345, np.int64)
     elif name == "two":
@@ -124,7 +140,7 @@ class Case:
         self.dtype, self.n_pages = dtype, n_pages
         self.ld = n_pages + 37
         classes = F32_CLASSES if dtype == "f32" else I32_CLASSES
-        self.ngroups = [(i % 4) + 1 for i in range(len(classes))]
+        self.ngroups = [GROUPS.get(name, (i % 4) + 1) for i, name in enumerate(classes)]
         self.goff = np.concatenate([[0], np.cumsum(self.ngroups)]).astype(np.int32)
         G = int(self.goff[-1])
         if dtype == "f32":
@@ -146,7 +162,7 @@ class Case:
                 parts, tot = i32_class(name, rng, g1 - g0, n_pages)
                 gs[g0:g1, :n_pages] = parts
                 assert np.array_equal(parts.astype(np.int64).sum(axis=0), tot)
-                self.sums.append(tot)
+                self.sums.append(i32_sum(tot))  # the I32 sum rule: int64, clamped to +-(2^31 - 1)
         self.scale = F32(1.0) if dtype == "f32" else F32(1.0 / (127.0 * 127.0))
         self.gs = torch.from_numpy(gs).cuda()
         self.classes = classes
