@@ -238,6 +238,13 @@ int b200ms_score(b200ms_t* h, const void* q_packed, int n_groups, const int32_t*
 int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
                 const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, int k, float scale, int64_t id_base,
                 float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream);
+/* b200ms_topk with one allow-mask PER QUERY (the FDE first stage of a search whose queries carry different filters):
+ * allow_masks_dev [n_masks, ceil(n_pages/32)] and mask_index_dev [n_q] (-1 = unfiltered) are DEVICE arrays, as in
+ * b200ms_search_device_masked; n_masks = 0: unfiltered.  Everything else as b200ms_topk. */
+int b200ms_topk_masked(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                       const int32_t* group_offsets, int n_q, const uint32_t* allow_masks_dev, int n_masks,
+                       const int32_t* mask_index_dev, int k, float scale, int64_t id_base, float* top_scores,
+                       int64_t* top_ids, int32_t* top_counts, void* cuda_stream);
 
 /* Merge candidate lists (e.g. the all-gathered per-shard top-k): cand_scores/cand_ids device [n_q, m]
  * (entries with id < 0 are ignored) -> best k by (score DESC, id ASC) in the total order of b200ms_topk (-0 == +0, NaN
@@ -399,6 +406,48 @@ int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtyp
 int b200ms_mmr_device(b200ms_t* h, const int64_t* cand_ids, const float* cand_scores, int n_cand, const int32_t* q_lens,
                       int n_q, int k, float lambda_mult, float score_scale, int64_t* out_ids, float* out_scores,
                       int32_t* out_counts, float* sims, void* cuda_stream);
+
+/* ---- searching with stored pages as the queries (new; no reference counterpart) -------------------------------------------
+ * "Pages like this one": DocumentService.retrieve_chunks(query_image=...) (core/services/document_service.py:193, 278-286)
+ * embeds a query image as a page-length query; a page that is already stored is the same kind of query, and its packed rows
+ * are already here.  These calls take source page ids (HOST int64 [n_src], each in [0, n_pages); anything else is
+ * B200MS_EINVAL) and use each page's packed rows as one query, copied as stored -- BF16 rows, I8 codes at the corpus scale,
+ * F8 e4m3 codes, B1 sign rows -- with no dequantise / requantise round trip: query q has the page's TRUE row count as its
+ * length, padding rows never count, and the value rule of b200ms_score holds unchanged.  A host-resident corpus's source
+ * rows are read through the mapping (one PCIe read of the named pages, as b200ms_fde_encode_corpus).
+ *   search_pages_device: the full scan of b200ms_search_device_masked for these queries -- the same packing layout, work
+ *     units (filtered scans included), b200ms_topk selection, I32 sum rule, tie and NaN order -- with one allow-mask row per
+ *     source (allow_masks_dev [n_masks, ceil(n_pages/32)], mask_index_dev [n_src], -1 = unfiltered; n_masks = 0: none).
+ *     Masks are the only filter: excluding the source itself, or its document, is a mask bit the caller clears.  Host-resident
+ *     corpora: B200MS_ESTATE (use a first stage and rerank_pages_batch_device).
+ *   rerank_pages_batch_device: b200ms_rerank_batch_device for these queries over cand_ids_dev [n_src, n_cand] (-1 = unused
+ *     slot), tie order by slot as there; a candidate whose page the source's mask row forbids is an unused slot.  Works on
+ *     host-resident corpora: the candidates are gathered exactly as b200ms_rerank_batch_device gathers them
+ *     (b200ms_last_gather_stats reports them; the source rows are not part of the gather).
+ *   Reported score (both): the normalised page-to-page MaxSim on the scale of b200ms_mmr_device's sim(source -> page),
+ *     __fdiv_rn(float32(sum) * score_scale, len) with len the source's true row count: the score b200ms_search_device would
+ *     report for the source's rows (dequantised: bf16 values, e4m3 values / scale, int8 codes / scale, +-1 for sign bits) divided by
+ *     len, so that one number means the same across sources of different lengths.  A NaN stays as reported (0x7fffffff).
+ *     score_scale as for the search (BF16 1, I8 / F8 1/scale^2, B1 1/128): the library does not know a quantised corpus's
+ *     scale.  I8: the sum follows the I32 sum rule of b200ms_topk -- a row scores at most 128 * 128 * 128 = 2^21 (-128 codes
+ *     against -128 rows), so a source of 1024 rows can pass 2^31 - 1 (1033 rows of +-127 codes against -128 rows, 1041
+ *     against +-127 rows); such pages are clamped to the bound and tie there, lower page id (slot) first.
+ *     A source page with zero rows gets count 0 (every slot -inf / -1).
+ *   page_rows_device: the true rows of the source pages back to back into out (device float32 [sum of their lengths, 128]),
+ *     each element the packed value widened exactly (bf16; int8 code; e4m3 value; sign bit as +1 / -1) times scale in fp32 --
+ *     the float query a first stage (b200ms_fde_encode, b200ms_sign_candidates_device) takes, with scale = 1/corpus scale for
+ *     I8 / F8 corpora.
+ * B200MS_EINVAL: n_src < 1, a source id outside [0, n_pages) (a page compacted away no longer exists), k outside [1, 4096],
+ * NULL outputs, n_masks > 0 without masks and index, n_cand < 1 or n_src * n_cand >= 2^30;  B200MS_ESTATE: no corpus, a
+ * full search_pages_device of a host-resident corpus.  Nothing is launched when a call is refused. */
+int b200ms_search_pages_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, int k, const uint32_t* allow_masks_dev,
+                               int n_masks, const int32_t* mask_index_dev, float score_scale, int64_t id_base,
+                               float* top_scores_dev, int64_t* top_ids_dev, int32_t* top_counts_dev, void* cuda_stream);
+int b200ms_rerank_pages_batch_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, const int64_t* cand_ids_dev,
+                                     int n_cand, int k, const uint32_t* allow_masks_dev, int n_masks,
+                                     const int32_t* mask_index_dev, float score_scale, float* top_scores_dev,
+                                     int64_t* top_ids_dev, int32_t* top_counts_dev, void* cuda_stream);
+int b200ms_page_rows_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, float scale, float* out, void* cuda_stream);
 
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the

@@ -66,6 +66,8 @@ _SIGNATURES = {
     "b200ms_pack_queries": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_float, i32p, POINTER(c_int), vp]),
     "b200ms_score": (c_int, [vp, vp, c_int, i32p, i32p, c_int, vp, c_int64, vp]),
     "b200ms_topk": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, c_int, c_float, c_int64, vp, vp, vp, vp]),
+    "b200ms_topk_masked": (c_int, [vp, vp, c_int, c_int64, c_int64, i32p, c_int, vp, c_int, vp, c_int, c_float, c_int64, vp, vp,
+                                   vp, vp]),
     "b200ms_merge_topk": (c_int, [vp, vp, vp, c_int, c_int, c_int, vp, vp, vp, vp]),
     "b200ms_search_host": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_float, c_float, c_int64, vp, vp, vp]),
     "b200ms_search_host_masked": (c_int, [vp, vp, i32p, c_int, c_int, vp, c_int, i32p, c_float, c_float, c_int64, vp, vp, vp]),
@@ -127,6 +129,9 @@ _SIGNATURES = {
     "b200ms_sign_candidates_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, vp, c_int, vp, c_float, c_float, vp, vp, vp,
                                               vp]),
     "b200ms_mmr_device": (c_int, [vp, vp, vp, c_int, i32p, c_int, c_int, c_float, c_float, vp, vp, vp, vp, vp]),
+    "b200ms_search_pages_device": (c_int, [vp, i64p, c_int, c_int, vp, c_int, vp, c_float, c_int64, vp, vp, vp, vp]),
+    "b200ms_rerank_pages_batch_device": (c_int, [vp, i64p, c_int, vp, c_int, c_int, vp, c_int, vp, c_float, vp, vp, vp, vp]),
+    "b200ms_page_rows_device": (c_int, [vp, i64p, c_int, c_float, vp, vp]),
 }
 
 
@@ -146,6 +151,10 @@ MAX_PER_DOC = 64
 def i32_array(values):
     arr = (c_int32 * len(values))(*[int(v) for v in values])
     return arr
+
+
+def i64_array(values):
+    return (c_int64 * len(values))(*[int(v) for v in values])
 
 
 class Handle:

@@ -317,7 +317,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
                        &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
-                       &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials};
+                       &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials, &h->src_pages};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   release_blocks(h);
@@ -804,10 +804,10 @@ B200MS_API int b200ms_score_times_ms(b200ms_t* h, float* out_ms, int n) {
   return n;
 }
 
-B200MS_API int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
-                           const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, int k, float scale,
-                           int64_t id_base, float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream) {
-  if (!h) return B200MS_EINVAL;
+// b200ms_topk / b200ms_topk_masked: allow = one mask (mask_index NULL) or a [n_masks, words] matrix with a row per query
+static int topk_impl(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                     const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, const int32_t* mask_index, int k,
+                     float scale, int64_t id_base, float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream) {
   if ((score_dtype != B200MS_F32 && score_dtype != B200MS_I32) || n_pages < 0 || ld < n_pages || n_q < 0 || k < 1 ||
       k > B200MS_MAX_K || (n_q > 0 && (!group_offsets || !top_scores || !top_ids || !top_counts)) ||
       (n_q > 0 && n_pages > 0 && !group_scores))
@@ -819,7 +819,26 @@ B200MS_API int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtyp
   if (int e = order.error()) return e;
   if (int e = upload(h, h->meta, group_offsets, size_t(n_q + 1) * 4, s)) return e;
   return launch_topk(h, group_scores, score_dtype, n_pages, ld, static_cast<const int32_t*>(h->meta.p), n_q, allow_mask,
-                     k, scale, id_base, nullptr, top_scores, top_ids, top_counts, s);
+                     k, scale, id_base, nullptr, top_scores, top_ids, top_counts, s, mask_index, (n_pages + 31) / 32);
+}
+
+B200MS_API int b200ms_topk(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                           const int32_t* group_offsets, int n_q, const uint32_t* allow_mask, int k, float scale,
+                           int64_t id_base, float* top_scores, int64_t* top_ids, int32_t* top_counts, void* stream) {
+  if (!h) return B200MS_EINVAL;
+  return topk_impl(h, group_scores, score_dtype, n_pages, ld, group_offsets, n_q, allow_mask, nullptr, k, scale, id_base,
+                   top_scores, top_ids, top_counts, stream);
+}
+
+B200MS_API int b200ms_topk_masked(b200ms_t* h, const void* group_scores, int score_dtype, int64_t n_pages, int64_t ld,
+                                  const int32_t* group_offsets, int n_q, const uint32_t* allow_masks_dev, int n_masks,
+                                  const int32_t* mask_index_dev, int k, float scale, int64_t id_base, float* top_scores,
+                                  int64_t* top_ids, int32_t* top_counts, void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  if (n_masks < 0 || (n_masks > 0 && (!allow_masks_dev || !mask_index_dev)))
+    return set_error(h, B200MS_EINVAL, "topk_masked: n_masks > 0 needs the mask matrix and one index per query");
+  return topk_impl(h, group_scores, score_dtype, n_pages, ld, group_offsets, n_q, n_masks > 0 ? allow_masks_dev : nullptr,
+                   n_masks > 0 ? mask_index_dev : nullptr, k, scale, id_base, top_scores, top_ids, top_counts, cuda_stream);
 }
 
 B200MS_API int b200ms_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand_ids, int n_q, int m, int k,
@@ -857,7 +876,7 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   if (c.host && !r.cand.ids) return set_error(h, B200MS_ESTATE, kHostFullScan);
   if (c.host && h->capturing) return set_error(h, B200MS_ESTATE, "search: a host-resident corpus cannot be graph-captured");
   const int n_q = r.n_q;
-  if (n_q < 1 || !r.q_lens || !r.q || r.k < 1 || r.k > B200MS_MAX_K || !r.top_scores || !r.top_ids || !r.top_counts)
+  if (n_q < 1 || !r.q_lens || (!r.q && !r.src_pages) || r.k < 1 || r.k > B200MS_MAX_K || !r.top_scores || !r.top_ids || !r.top_counts)
     return set_error(h, B200MS_EINVAL, "search: bad arguments (n_q >= 1, 1 <= k <= 4096)");
   if (r.docs) {
     const DocSpec& d = *r.docs;
@@ -884,10 +903,12 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   const int64_t* ds_dev = reinterpret_cast<const int64_t*>(md + m.off_ds);
   const int32_t* goff_dev = reinterpret_cast<const int32_t*>(md + m.off_goff);
   const int32_t* ntok_dev = reinterpret_cast<const int32_t*>(md + m.off_ntok);
-  if (m.groups_padded > 0)
-    if (int e = launch_pack_rows(h, r.q, r.q_dtype, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, 1, h->q_packed.p, c.dtype,
-                                 r.i8_q_scale, s))
-      return e;
+  if (m.groups_padded > 0) {
+    const int e = r.src_pages ? launch_pack_src_pages(h, r.src_pages, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, h->q_packed.p, s)
+                              : launch_pack_rows(h, r.q, r.q_dtype, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, 1, h->q_packed.p,
+                                                 c.dtype, r.i8_q_scale, s);
+    if (e) return e;
+  }
   const int ng = int(m.groups);
   if (!c.host) {
     UnitPlan scan;
@@ -931,6 +952,10 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   if (int e = reserve(h, h->cand_mask, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
   if (int e = launch_cand_units(h, corpus_view(h), cs.ids, n_slots, nullptr, nullptr, static_cast<uint32_t*>(h->cand_mask.p), s))
     return e;
+  if (r.allow && cs.per_query)
+    if (int e = launch_mask_cand_slots(h, cs.ids, n_slots, cs.stride(), r.allow, r.mask_index,
+                                       static_cast<uint32_t*>(h->cand_mask.p), s))
+      return e;
   return launch_topk(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, static_cast<const uint32_t*>(h->cand_mask.p), r.k,
                      r.score_scale, 0, cs.ids, r.top_scores, r.top_ids, r.top_counts, s, nullptr, 0, cs.stride());
 }
@@ -1053,6 +1078,105 @@ B200MS_API int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, i
   const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
   r.docs = &d;
   return search_ordered(h, r, static_cast<cudaStream_t>(stream));
+}
+
+// ---- searching with stored pages as the queries
+// The source pages of a call: every id names a page of the attached corpus; their true lengths into *lens
+static int check_src_pages(b200ms_t* h, const int64_t* src, int n_src, const char* what, std::vector<int32_t>* lens) {
+  const Corpus& c = h->corpus;
+  if (c.dtype < 0) return set_error(h, B200MS_ESTATE, std::string(what) + ": no corpus attached");
+  if (!src || n_src < 1) return set_error(h, B200MS_EINVAL, std::string(what) + ": bad arguments (n_src >= 1 source pages)");
+  lens->resize(size_t(n_src));
+  for (int i = 0; i < n_src; ++i) {
+    if (src[i] < 0 || src[i] >= c.n_pages)
+      return set_error(h, B200MS_EINVAL, std::string(what) + ": source page " + std::to_string(src[i]) + " is not a page of the corpus (" +
+                                             std::to_string(c.n_pages) + " pages)");
+    (*lens)[size_t(i)] = h->page_len_host[size_t(src[i])];
+  }
+  return B200MS_OK;
+}
+
+static int check_masks(b200ms_t* h, const uint32_t* masks, int n_masks, const int32_t* index, const char* what) {
+  if (n_masks < 0 || (n_masks > 0 && (!masks || !index)))
+    return set_error(h, B200MS_EINVAL, std::string(what) + ": n_masks > 0 needs the mask matrix and one index per source");
+  return B200MS_OK;
+}
+
+// pack the sources' rows -> score -> top-k (search_core) -> divide every source's scores by its length
+static int search_pages_ordered(b200ms_t* h, const int64_t* src_host, SearchRequest& r, cudaStream_t s) {
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  if (int e = upload(h, h->src_pages, src_host, size_t(r.n_q) * 8, s)) return e;
+  r.src_pages = static_cast<const int64_t*>(h->src_pages.p);
+  if (int e = search_core(h, r, build_search_meta(r.q_lens, r.n_q), s)) return e;
+  return launch_normalise_pages(h, r.src_pages, r.n_q, r.k, r.top_scores, r.top_ids, r.top_counts, s);
+}
+
+B200MS_API int b200ms_search_pages_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, int k,
+                                          const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
+                                          float score_scale, int64_t id_base, float* top_scores_dev, int64_t* top_ids_dev,
+                                          int32_t* top_counts_dev, void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kHostFullScan);
+  std::vector<int32_t> lens;
+  if (int e = check_src_pages(h, src_pages_host, n_src, "search_pages_device", &lens)) return e;
+  if (int e = check_masks(h, allow_masks_dev, n_masks, mask_index_dev, "search_pages_device")) return e;
+  if (k < 1 || k > B200MS_MAX_K || !top_scores_dev || !top_ids_dev || !top_counts_dev)
+    return set_error(h, B200MS_EINVAL, "search_pages_device: bad arguments (1 <= k <= 4096, outputs)");
+  DeviceGuard g(h->device);
+  SearchRequest r{nullptr, h->corpus.dtype, lens.data(), n_src, k, 1.f, score_scale, top_scores_dev, top_ids_dev, top_counts_dev,
+                  id_base};
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
+  return search_pages_ordered(h, src_pages_host, r, static_cast<cudaStream_t>(cuda_stream));
+}
+
+B200MS_API int b200ms_rerank_pages_batch_device(b200ms_t* h, const int64_t* src_pages_host, int n_src,
+                                                const int64_t* cand_ids_dev, int n_cand, int k,
+                                                const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
+                                                float score_scale, float* top_scores_dev, int64_t* top_ids_dev,
+                                                int32_t* top_counts_dev, void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  std::vector<int32_t> lens;
+  if (int e = check_src_pages(h, src_pages_host, n_src, "rerank_pages_batch_device", &lens)) return e;
+  if (int e = check_masks(h, allow_masks_dev, n_masks, mask_index_dev, "rerank_pages_batch_device")) return e;
+  const CandSpec cand{cand_ids_dev, n_cand, 1};
+  if (!cand_ids_dev || n_cand < 1 || cand.n_slots(n_src) >= (int64_t(1) << 30) || k < 1 || k > B200MS_MAX_K || !top_scores_dev ||
+      !top_ids_dev || !top_counts_dev)
+    return set_error(h, B200MS_EINVAL, "rerank_pages_batch_device: bad arguments (n_cand >= 1, n_src*n_cand < 2^30, 1 <= k <= 4096)");
+  DeviceGuard g(h->device);
+  SearchRequest r{nullptr, h->corpus.dtype, lens.data(), n_src, k, 1.f, score_scale, top_scores_dev, top_ids_dev, top_counts_dev};
+  r.cand = cand;
+  if (n_masks > 0) {
+    r.allow = allow_masks_dev;
+    r.mask_index = mask_index_dev;
+  }
+  return search_pages_ordered(h, src_pages_host, r, static_cast<cudaStream_t>(cuda_stream));
+}
+
+B200MS_API int b200ms_page_rows_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, float scale, float* out,
+                                       void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  std::vector<int32_t> lens;
+  if (int e = check_src_pages(h, src_pages_host, n_src, "page_rows_device", &lens)) return e;
+  // [src ids | true-row offsets], one upload
+  std::vector<int64_t> meta(size_t(2 * n_src + 1), 0);
+  for (int i = 0; i < n_src; ++i) {
+    meta[size_t(i)] = src_pages_host[i];
+    meta[size_t(n_src + i + 1)] = meta[size_t(n_src + i)] + lens[size_t(i)];
+  }
+  const int64_t n_rows = meta.back();
+  if (n_rows > 0 && !out) return set_error(h, B200MS_EINVAL, "page_rows_device: out is NULL");
+  if (n_rows == 0) return B200MS_OK;
+  DeviceGuard g(h->device);
+  cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  if (int e = upload(h, h->src_pages, meta.data(), meta.size() * 8, s)) return e;
+  const int64_t* d = static_cast<const int64_t*>(h->src_pages.p);
+  return launch_page_rows(h, d, d + n_src, n_src, n_rows, scale, out, s);
 }
 
 // Small unmasked zero-copy calls repeat with the same shapes (interactive queries): the second call of a shape is captured

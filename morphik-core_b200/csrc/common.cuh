@@ -96,6 +96,8 @@ struct SearchRequest {
   const int32_t* mask_index = nullptr;   // per query: row of `allow` (-1 = no mask); NULL = the one mask for every query
   CandSpec cand;                         // ids == NULL: full scan
   const DocSpec* docs = nullptr;         // != NULL: the top k documents (per-query candidate lists only) instead of pages
+  const int64_t* src_pages = nullptr;    // != NULL (device, [n_q]): query q is corpus page src_pages[q], its packed rows taken
+                                         // as they are stored (q and q_dtype unused; q_lens = the pages' true lengths)
 };
 
 // Results of a search as one block: [n_q*k int64 ids | n_q*k f32 scores | n_q int32 counts], padded to 16 bytes, so that
@@ -262,6 +264,8 @@ struct b200ms {
   bms::DeviceBuf compact_meta, compact_bounce;
   // diversifying results (maxsim_mmr.cu): per-call state of the greedy pick and the round kernels' per-tile partial sums
   bms::DeviceBuf mmr_state, mmr_partials;
+  // searching with stored pages as the queries (search_pages.cu): the call's source page ids [, their true-row offsets]
+  bms::DeviceBuf src_pages;
 };
 
 namespace bms {
@@ -416,5 +420,19 @@ int launch_fde_scan(b200ms_t* h, const void* F, const float* inv_norm, int64_t n
                     float* scores, int64_t ld, cudaStream_t s);
 int launch_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand_ids, int n_q, int m, int k,
                       float* top_scores, int64_t* top_ids, int32_t* top_counts, cudaStream_t s);
+// search_pages.cu.  src_dev: device page ids of the attached corpus (checked by the caller); ss_dev / ds_dev: [n_src+1] true /
+// padded row offsets of the sources (build_search_meta of their lengths).
+// The sources' packed rows in the query layout of b200ms_pack_queries (dst_rows rows, zero past each source's true rows)
+int launch_pack_src_pages(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, const int64_t* ds_dev, int64_t n_src,
+                          int64_t dst_rows, void* dst, cudaStream_t s);
+// The sources' true rows back to back as float32 [n_rows, 128]: packed value (a sign bit as +-1) times scale
+int launch_page_rows(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, int64_t n_src, int64_t n_rows, float scale,
+                     float* out, cudaStream_t s);
+// Candidate mode: clear the valid bit of every slot whose page its list's allow-mask row (as SearchRequest) forbids
+int launch_mask_cand_slots(b200ms_t* h, const int64_t* cand, int64_t n_slots, int64_t stride, const uint32_t* allow,
+                           const int32_t* mask_index, uint32_t* slot_mask, cudaStream_t s);
+// Reported scores of source q divided by its true length; a source without rows gets count 0
+int launch_normalise_pages(b200ms_t* h, const int64_t* src_dev, int n_src, int k, float* scores, int64_t* ids,
+                           int32_t* counts, cudaStream_t s);
 
 }  // namespace bms

@@ -355,14 +355,23 @@ class TwoStageIndex(TwoStageSearch):
             return encode_items(self.index, list(queries), False, self.fde_dim)
         return encode_rows(self.index, *staged, False, self.fde_dim)
 
-    def _scan(self, q_fde: torch.Tensor, lens: Sequence[int], kc: int, mask: Optional[torch.Tensor]):
+    def _scan(self, q_fde: torch.Tensor, lens: Sequence[int], kc: int, mask: Optional[torch.Tensor],
+              mask_index: Optional[torch.Tensor] = None):
         """Scan of the FDE matrix for query FDEs [n_q, fde_dim] -> top kc pages per query among those `mask` (already
-        checked) allows: (scores, page ids, counts) on the device."""
+        checked) allows: (scores, page ids, counts) on the device.  With ``mask_index`` (int32 [n_q], -1 = unfiltered),
+        `mask` is a [n_masks, words] matrix and query q keeps to its row (b200ms_topk_masked)."""
         n_q = q_fde.shape[0]
         scores = self.fde_scores(q_fde)
         ts, ti, tc = _topk_outputs(n_q, kc, self.device)
         goff = nat.i32_array(list(range(n_q + 1)))
         with torch.cuda.device(self.device):
+            if mask_index is not None:
+                self.index.h.check(
+                    nat.lib.b200ms_topk_masked(self.index.h.ptr, _vp(scores), nat.F32, self._n, scores.shape[1], goff, n_q,
+                                               _vp(mask), int(mask.shape[0]), _vp(mask_index), kc, ctypes.c_float(1.0), 0,
+                                               _vp(ts), _vp(ti), _vp(tc), self.index._stream()),
+                    "b200ms_topk_masked(fde)")
+                return ts, ti, tc
             self.index.h.check(
                 nat.lib.b200ms_topk(self.index.h.ptr, _vp(scores), nat.F32, self._n, scores.shape[1], goff, n_q, _vp(mask), kc,
                                     ctypes.c_float(1.0), 0, _vp(ts), _vp(ti), _vp(tc), self.index._stream()),

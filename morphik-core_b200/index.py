@@ -830,6 +830,71 @@ class MaxSimIndex:
                 "b200ms_rerank_batch_device")
         return ts, ti, tc
 
+    # ------------------------------------------------------------------ stored pages as the queries
+    def _src_pages(self, src_pages) -> List[int]:
+        """Source page ids -> a non-empty list of ints in [0, n_pages) (ValueError otherwise, before any launch)."""
+        ids = [int(p) for p in (src_pages.tolist() if isinstance(src_pages, (np.ndarray, torch.Tensor)) else src_pages)]
+        if not ids or any(not 0 <= p < self.n_pages for p in ids):
+            raise ValueError(f"src_pages must be one or more page ids in [0, {self.n_pages}), got {ids}")
+        return ids
+
+    def search_pages(self, src_pages, k: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                     mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0,
+                     out: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
+        """Pages like stored pages (b200ms_search_pages_device), asynchronous on torch's current stream: source page i's own
+        packed rows are query i of a full scan, and a page's score is the page-to-page MaxSim per source row -- the score
+        search_device would give the source's rows, over the source's row count.  Masks as search_device, one row per source
+        (the only filter: the source itself is returned unless its mask bit is clear).  A source without rows gets count 0.
+        Returns device tensors (scores float32 [n_src,k], page ids + id_base int64 [n_src,k], counts int32 [n_src])."""
+        ids = self._src_pages(src_pages)
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, len(ids), self.n_pages, self.device)
+        if masks is not None and index is None:  # one mask for every source: a one-row matrix
+            index = torch.zeros((len(ids),), dtype=torch.int32, device=self.device)
+        ts, ti, tc = _topk_outputs(len(ids), int(k), self.device, out)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_search_pages_device(
+                    self.h.ptr, nat.i64_array(ids), len(ids), int(k), _vp(masks), n_masks, _vp(index),
+                    ctypes.c_float(self.score_scale), int(id_base), _vp(ts), _vp(ti), _vp(tc), self._stream()),
+                "b200ms_search_pages_device")
+        return ts, ti, tc
+
+    def rerank_pages_batch(self, src_pages, cand_ids: torch.Tensor, k: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                           mask_index_dev: Optional[torch.Tensor] = None,
+                           out: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
+        """rerank_batch with stored pages as the queries (b200ms_rerank_pages_batch_device): source i's packed rows against
+        its own candidate list cand_ids int64 [n_src, n_cand] (-1 = unused slot), scores as search_pages; a candidate its
+        source's mask row forbids is an unused slot.  k is capped at n_cand.  Works on both tiers."""
+        ids = self._src_pages(src_pages)
+        n_cand, kk = _check_candidates(cand_ids, len(ids), k, self.device, per_query=True)
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, len(ids), self.n_pages, self.device)
+        if masks is not None and index is None:
+            index = torch.zeros((len(ids),), dtype=torch.int32, device=self.device)
+        ts, ti, tc = _topk_outputs(len(ids), kk, self.device, out)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_rerank_pages_batch_device(
+                    self.h.ptr, nat.i64_array(ids), len(ids), _vp(cand_ids), n_cand, kk, _vp(masks), n_masks, _vp(index),
+                    ctypes.c_float(self.score_scale), _vp(ts), _vp(ti), _vp(tc), self._stream()),
+                "b200ms_rerank_pages_batch_device")
+        return ts, ti, tc
+
+    def page_rows(self, src_pages) -> Tuple[torch.Tensor, List[int]]:
+        """The true rows of the source pages back to back as float32 [sum len, 128] on the device, dequantised
+        (b200ms_page_rows_device: int8 codes and e4m3 values over the corpus scale, sign bits as +-1), and their lengths --
+        the float query of a first stage."""
+        ids = self._src_pages(src_pages)
+        lens = [int(self._page_lens[p]) for p in ids]
+        out = torch.empty((max(sum(lens), 1), nat.DIM), dtype=torch.float32, device=self.device)
+        scale = 1.0 / self.i8_scale if self.dtype in (nat.I8, nat.F8) else 1.0
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(nat.lib.b200ms_page_rows_device(self.h.ptr, nat.i64_array(ids), len(ids), ctypes.c_float(scale),
+                                                         _vp(out), self._stream()), "b200ms_page_rows_device")
+        return out, lens
+
     # ------------------------------------------------------------------ grouping results by document
     def _check_docs_args(self, per_doc: int, page_doc_dev: torch.Tensor):
         if not 1 <= int(per_doc) <= nat.MAX_PER_DOC:

@@ -506,6 +506,63 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
         return out
 
+    async def query_similar_to_chunks(self, chunk_identifiers: List[Tuple[str, int]], k: int,
+                                      doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None,
+                                      include_same_document: bool = False,
+                                      min_score: Optional[float] = None) -> List[List[DocumentChunk]]:
+        """Chunks like stored chunks (extension; "query by id"): each named chunk's stored embedding is the query, as
+        ``retrieve_chunks(query_image=...)`` would send a page-length query, without fetching or re-sending the embedding.
+        One list per visible source chunk, in first-mention order, under the rules of ``get_chunks_by_id`` (unknown or
+        deleted chunks and chunks of another ``app_id`` are skipped, duplicates collapsed).  ``doc_ids`` / ``app_id`` filter
+        the results as in query_similar; the source chunk is never returned, and its document's other chunks only with
+        ``include_same_document``.  Scores are page-to-page MaxSim per source row (query_similar's score for the source's
+        rows over their count), so they compare across sources; ``min_score`` drops hits below it.  Every source of a call
+        shares one pass over the corpus; masks, GPU search and chunk construction are one critical section."""
+        if k <= 0 or not chunk_identifiers:
+            return []
+        return await asyncio.to_thread(self._similar_to_chunks_locked, list(chunk_identifiers), int(k), doc_ids, app_id,
+                                       bool(include_same_document), min_score)
+
+    def _similar_to_chunks_locked(self, chunk_identifiers, k, doc_ids, app_id, include_same_document, min_score):
+        import torch
+
+        t0 = time.perf_counter()
+        with self._lock:
+            recs = self._visible_records(chunk_identifiers, app_id)
+            if not recs:
+                return []
+            n = len(self.catalog)
+            base = self.catalog.allow_mask(doc_ids, app_id)
+            base = self.catalog.alive[:n].copy() if base is None else base
+            masks = []
+            for pid, rec in recs:  # one row per source: the filter, minus the source (and, by default, its document)
+                m = base.copy()
+                m[pid] = False
+                if not include_same_document:
+                    m[self.catalog.pages_of(rec.document_id)] = False
+                masks.append(m)
+            if not any(m.any() for m in masks):
+                return [[] for _ in recs]
+            words = np.stack([PageCatalog.mask_words(m) for m in masks])
+            kk = min(_capped_k(k), n)
+            pids = [pid for pid, _ in recs]
+            t1 = time.perf_counter()
+            if self._two_stage is not None:  # each source's row filters its candidates too: no slot goes to an excluded page
+                ts, ti, tc = self._two_stage.search_pages(pids, kk, n_candidates=max(self._n_candidates, kk), allow_masks=words)
+            else:
+                dev = torch.device(self._index.device)
+                mat = torch.from_numpy(words.view(np.int32)).to(dev)
+                index = torch.arange(len(pids), dtype=torch.int32, device=dev)
+                ts, ti, tc = (np.asarray(t.cpu()) for t in self._index.search_pages(pids, kk, mat, index))
+            t2 = time.perf_counter()
+            out = [self._chunks(ts[i], ti[i], int(tc[i]), min_score) for i in range(len(pids))]
+            t3 = time.perf_counter()
+        self.last_query_timing = {"prepare_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3,
+                                  "build_chunks_ms": (t3 - t2) * 1e3, "total_ms": (t3 - t0) * 1e3}
+        if self._two_stage is not None:
+            self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
+        return out
+
     async def get_chunks_by_id(self, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
                                skip_image_content: bool = False) -> List[DocumentChunk]:
         if not chunk_identifiers:

@@ -38,9 +38,11 @@ class TwoStageSearch:
         (rows, dtype code, lengths) when the caller staged them already for the rerank, else None."""
         return staged[0] if staged else self.index._stage_rows(list(queries))[0]
 
-    def _scan(self, q, lens: Sequence[int], n_cand: int, mask: Optional[torch.Tensor]):
-        """Top n_cand pages per query among those `mask` (checked, one row for every query) allows: device tensors (scores
-        float32 [n_q, n_cand], page ids int64 [n_q, n_cand] (-1 padded), counts int32 [n_q])."""
+    def _scan(self, q, lens: Sequence[int], n_cand: int, mask: Optional[torch.Tensor],
+              mask_index: Optional[torch.Tensor] = None):
+        """Top n_cand pages per query among those `mask` (checked, one row for every query; with ``mask_index`` int32
+        [n_q], a [n_masks, words] matrix and each query's row, -1 = unfiltered) allows: device tensors (scores float32
+        [n_q, n_cand], page ids int64 [n_q, n_cand] (-1 padded), counts int32 [n_q])."""
         raise NotImplementedError
 
     def journal_rows(self, first: int, n: int):
@@ -118,6 +120,50 @@ class TwoStageSearch:
         ts, ti, tc, ev = self.search_device(queries, k, n_candidates, mask_dev)
         torch.cuda.synchronize(self.device)
         out = _host(ts, (n_q, k), -np.inf), _host(ti, (n_q, k), -1), tc.cpu().numpy().astype(np.int32)
+        self.last_timing_ms = self.stage_timing_ms(ev)
+        return out
+
+    def search_pages_device(self, src_pages, k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
+                            mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0):
+        """search_device with stored pages as the queries: the first stage runs on each source page's rows, dequantised on
+        the device (MaxSimIndex.page_rows), and MaxSimIndex.rerank_pages_batch reranks its candidates with the packed page
+        query, so scores are MaxSimIndex.search_pages's.  Masks as search_pages, one row per source, in BOTH stages: a page
+        a source may not return (the source itself, its document) never takes one of its candidate slots.  Returns as
+        search_device."""
+        ids = self.index._src_pages(src_pages)
+        masks, _, index = _check_device_masks(allow_mask_dev, mask_index_dev, len(ids), self.n_pages, self.device)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        ev[0].record()
+        rows, lens = self.index.page_rows(ids)
+        q = self._encode(None, (rows, nat.F32, lens))
+        ev[1].record()
+        if index is None:
+            _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k)), masks)
+        else:
+            _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k)), masks, index)
+        ev[2].record()
+        ts, ti, tc = self.index.rerank_pages_batch(ids, ci, k, allow_mask_dev, mask_index_dev)
+        if id_base:
+            ti = torch.where(ti >= 0, ti + int(id_base), ti)
+        ev[3].record()
+        return ts, ti, tc, ev
+
+    def search_pages(self, src_pages, k: int, n_candidates: int = 1000, allow_masks: Optional[np.ndarray] = None):
+        """search_pages_device with host masks: ``allow_masks`` uint32 [n_src, words], one row per source, or None;
+        synchronous.  Returns host arrays (scores [n_src,k], page ids [n_src,k], counts [n_src]) and fills last_timing_ms with
+        search's stage names."""
+        n_src = len(self.index._src_pages(src_pages))
+        words = (self.n_pages + 31) // 32
+        masks = index = None
+        if allow_masks is not None:
+            m = np.ascontiguousarray(allow_masks, dtype=np.uint32)
+            if m.shape != (n_src, words):
+                raise ValueError(f"allow_masks must be uint32 [{n_src}, {words}], got {m.shape}")
+            masks = torch.from_numpy(m.view(np.int32)).to(self.device)
+            index = torch.arange(n_src, dtype=torch.int32, device=self.device)
+        ts, ti, tc, ev = self.search_pages_device(src_pages, k, n_candidates, masks, index)
+        torch.cuda.synchronize(self.device)
+        out = _host(ts, (n_src, k), -np.inf), _host(ti, (n_src, k), -1), tc.cpu().numpy().astype(np.int32)
         self.last_timing_ms = self.stage_timing_ms(ev)
         return out
 
