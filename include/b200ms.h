@@ -449,6 +449,56 @@ int b200ms_rerank_pages_batch_device(b200ms_t* h, const int64_t* src_pages_host,
                                      int64_t* top_ids_dev, int32_t* top_counts_dev, void* cuda_stream);
 int b200ms_page_rows_device(b200ms_t* h, const int64_t* src_pages_host, int n_src, float scale, float* out, void* cuda_stream);
 
+/* ---- relevance feedback: liked and disliked examples, one fused score (new; no reference counterpart) ---------------------
+ * "More like these, less like that": a REQUEST has one or more weighted EXAMPLES, and pages rank by the weighted sum of their
+ * scores against every example, all examples of all requests scored in ONE pass over the corpus (or the candidates).
+ *   Examples (HOST arrays): n_qe query embeddings first -- rows of q_dev (F32 or BF16, [sum q_lens, 128], as
+ *   b200ms_search_device_masked) of q_lens[i] tokens -- then n_src stored pages src_pages_host[j] in [0, n_pages), packed as
+ *   b200ms_search_pages_device packs them.  Example i (query examples first, then pages) belongs to request ex_req_host[i] in
+ *   [0, n_req) and carries the weight ex_weight_host[i]: finite and != 0, > 0 for "like", < 0 for "unlike".  Every request
+ *   needs at least one example of positive weight.
+ *   Example score s_e(p): __fdiv_rn(float32(finish_sum(sum of its group scores)) * score_scale, len) -- for a page example
+ *     exactly what b200ms_search_pages_device reports (len = its true rows), for a query example b200ms_search_device's score
+ *     over its token count (len = T): the mean MaxSim per query row.  I8 / B1: each example's sum follows the I32 sum rule of
+ *     b200ms_topk on its own (an int64 sum clamped to +-(2^31 - 1)); the fusion happens after that clamp.  An example of zero
+ *     rows or tokens adds no term (a request whose examples all have none scores 0 on every page).
+ *   Fused score: acc = 0.0f; for each example e of the request, in example order: acc = __fadd_rn(acc, __fmul_rn(w_e,
+ *     s_e(p))) -- no FMA contraction, so numpy float32 reproduces it bit for bit.  The fused rows go through the selection of
+ *     b200ms_topk (one group per request, F32, scale 1): its keys, ties towards the lower page (candidate mode: the lower
+ *     slot), its NaN order, id_base.  One allow-mask row per REQUEST (allow_masks_dev [n_masks, ceil(n_pages/32)],
+ *     mask_index_dev [n_req], -1 = unfiltered; n_masks = 0: none).  Example pages are returned like any other page: a caller
+ *     who does not want them clears their bits in the request's mask row.  zero_pad_compat does not apply.
+ *   search_examples_device: the full scan (filtered scans included: the pages some request's mask row allows).  Host-resident
+ *     corpora: B200MS_ESTATE (use a first stage, union_candidates_device and rerank_examples_batch_device).
+ *   rerank_examples_batch_device: over one candidate list per request, cand_ids_dev [n_req, n_cand] (-1 = unused slot);
+ *     every example of request r scores r's list, a candidate r's mask row forbids is an unused slot, and the outputs are
+ *     [n_req, k] as b200ms_rerank_batch_device's.  Works on host-resident corpora: the candidates are gathered once per
+ *     distinct page, exactly as b200ms_rerank_batch_device gathers them (b200ms_last_gather_stats).
+ * B200MS_EINVAL: no example, n_req < 1, a request without a positive example, a zero or non-finite weight, ex_req outside
+ * [0, n_req), a page id outside [0, n_pages), a negative query length, a query example without F32 / BF16 rows, k outside
+ * [1, 4096], NULL outputs, n_masks > 0 without masks and index, n_cand < 1 or (n_req + examples) * n_cand >= 2^30;
+ * B200MS_ESTATE: no corpus, a full search_examples_device of a host-resident corpus.  Nothing is launched when a call is
+ * refused.
+ *   union_candidates_device: the union of first-stage lists, for the rerank above.  Request r owns rows list_off_host[r] ..
+ *     list_off_host[r+1] of cand_ids_dev [n_lists, n_cand] (list_off_host [n_req+1] rising from 0 to n_lists); out_dev
+ *     [n_req, width] gets r's distinct ids (>= 0; negative ids are unused slots) in first-occurrence order, row-major over
+ *     its lists, then -1.  A union of more than width ids keeps the first width.  One CTA per request, deterministic, no
+ *     host synchronisation.  B200MS_EINVAL: n_req < 1, n_cand < 1, width < 1, n_lists * n_cand >= 2^30, a bad list_off, NULL
+ *     arrays. */
+int b200ms_search_examples_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_qe,
+                                  const int64_t* src_pages_host, int n_src, const int32_t* ex_req_host,
+                                  const float* ex_weight_host, int n_req, int k, const uint32_t* allow_masks_dev, int n_masks,
+                                  const int32_t* mask_index_dev, float i8_q_scale, float score_scale, int64_t id_base,
+                                  float* top_scores_dev, int64_t* top_ids_dev, int32_t* top_counts_dev, void* cuda_stream);
+int b200ms_rerank_examples_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_qe,
+                                        const int64_t* src_pages_host, int n_src, const int32_t* ex_req_host,
+                                        const float* ex_weight_host, int n_req, const int64_t* cand_ids_dev, int n_cand,
+                                        int k, const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
+                                        float i8_q_scale, float score_scale, float* top_scores_dev, int64_t* top_ids_dev,
+                                        int32_t* top_counts_dev, void* cuda_stream);
+int b200ms_union_candidates_device(b200ms_t* h, const int64_t* cand_ids_dev, int n_lists, int n_cand,
+                                   const int32_t* list_off_host, int n_req, int64_t* out_dev, int width, void* cuda_stream);
+
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the
  * path in B200MS_NCCL_LIB); b200ms_comm_available() says whether that worked.

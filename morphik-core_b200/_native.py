@@ -132,6 +132,11 @@ _SIGNATURES = {
     "b200ms_search_pages_device": (c_int, [vp, i64p, c_int, c_int, vp, c_int, vp, c_float, c_int64, vp, vp, vp, vp]),
     "b200ms_rerank_pages_batch_device": (c_int, [vp, i64p, c_int, vp, c_int, c_int, vp, c_int, vp, c_float, vp, vp, vp, vp]),
     "b200ms_page_rows_device": (c_int, [vp, i64p, c_int, c_float, vp, vp]),
+    "b200ms_search_examples_device": (c_int, [vp, vp, c_int, i32p, c_int, i64p, c_int, i32p, f32p, c_int, c_int, vp, c_int, vp,
+                                              c_float, c_float, c_int64, vp, vp, vp, vp]),
+    "b200ms_rerank_examples_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, i64p, c_int, i32p, f32p, c_int, vp, c_int, c_int,
+                                                    vp, c_int, vp, c_float, c_float, vp, vp, vp, vp]),
+    "b200ms_union_candidates_device": (c_int, [vp, vp, c_int, c_int, i32p, c_int, vp, c_int, vp]),
 }
 
 
@@ -155,6 +160,10 @@ def i32_array(values):
 
 def i64_array(values):
     return (c_int64 * len(values))(*[int(v) for v in values])
+
+
+def f32_array(values):
+    return (c_float * len(values))(*[float(v) for v in values])
 
 
 class Handle:

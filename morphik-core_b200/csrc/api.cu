@@ -2,6 +2,8 @@
 // (chunk table, work-unit plan, TMA descriptor), query packing and the fused search entry points.
 // Host-side C++ only orchestrates; all arithmetic on embeddings happens in the CUDA kernels.
 // (Multi-GPU entry points -- NCCL communicator, all-gather of top-k lists, pipelined sharded search -- live in comm.cu.)
+#include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -317,7 +319,8 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->fde_final_sign, &h->ht_bitmap, &h->ht_wpre, &h->ht_uniq, &h->ht_stage_off, &h->ht_hdr,
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
                        &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
-                       &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials, &h->src_pages};
+                       &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials, &h->src_pages,
+                       &h->ex_meta, &h->ex_lists, &h->ex_fused, &h->ex_union};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   release_blocks(h);
@@ -870,7 +873,7 @@ int plan_full_scan(b200ms_t* h, const uint32_t* allow, const int32_t* mask_index
   return h->scan_planned ? launch_scan_plan(h, allow, mask_index, n_q, s, plan) : B200MS_OK;
 }
 
-int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev) {
+int search_scan(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev, ScanResult* out) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "search: no corpus attached (call b200ms_set_corpus first)");
   if (c.host && !r.cand.ids) return set_error(h, B200MS_ESTATE, kHostFullScan);
@@ -903,11 +906,17 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   const int64_t* ds_dev = reinterpret_cast<const int64_t*>(md + m.off_ds);
   const int32_t* goff_dev = reinterpret_cast<const int32_t*>(md + m.off_goff);
   const int32_t* ntok_dev = reinterpret_cast<const int32_t*>(md + m.off_ntok);
-  if (m.groups_padded > 0) {
-    const int e = r.src_pages ? launch_pack_src_pages(h, r.src_pages, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, h->q_packed.p, s)
-                              : launch_pack_rows(h, r.q, r.q_dtype, ss_dev, ds_dev, n_q, m.groups_padded * kGroup, 1, h->q_packed.p,
-                                                 c.dtype, r.i8_q_scale, s);
-    if (e) return e;
+  if (m.groups_padded > 0) {  // query rows [0, ds[n_rows_q]), then the stored pages' rows; the last packer zeroes the tail
+    const int64_t rows = m.groups_padded * kGroup;
+    const int n_rows_q = r.src_pages ? r.src_first : n_q;
+    const int64_t q_end = n_rows_q == n_q ? rows : reinterpret_cast<const int64_t*>(m.host.data() + m.off_ds)[n_rows_q];
+    if (n_rows_q > 0)
+      if (int e = launch_pack_rows(h, r.q, r.q_dtype, ss_dev, ds_dev, n_rows_q, q_end, 1, h->q_packed.p, c.dtype, r.i8_q_scale, s))
+        return e;
+    if (n_rows_q < n_q)
+      if (int e = launch_pack_src_pages(h, r.src_pages, ss_dev + n_rows_q, ds_dev + n_rows_q, n_q - n_rows_q, q_end, rows,
+                                        h->q_packed.p, s))
+        return e;
   }
   const int ng = int(m.groups);
   if (!c.host) {
@@ -937,7 +946,22 @@ int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
   }
   if (ng == 0 || n_items == 0)
     if (int e = zero_scores(h, h->scores.p, gp, ld, s, "search: memset")) return e;
-  const int sdt = (c.dtype == B200MS_BF16 || c.dtype == B200MS_F8) ? B200MS_F32 : B200MS_I32;
+  out->cs = cs;
+  out->ld = ld;
+  out->goff_dev = goff_dev;
+  out->sdt = (c.dtype == B200MS_BF16 || c.dtype == B200MS_F8) ? B200MS_F32 : B200MS_I32;
+  return B200MS_OK;
+}
+
+int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev) {
+  ScanResult sr;
+  if (int e = search_scan(h, r, m, s, meta_dev, &sr)) return e;
+  const Corpus& c = h->corpus;
+  const int n_q = r.n_q;
+  const CandSpec& cs = sr.cs;
+  const int64_t ld = sr.ld;
+  const int32_t* goff_dev = sr.goff_dev;
+  const int sdt = sr.sdt;
   if (r.docs)
     return cs.ids ? launch_topk_docs(h, h->scores.p, sdt, cs.n_cand, ld, goff_dev, n_q, nullptr, nullptr, cs.ids, cs.stride(),
                                      c.n_pages, *r.docs, r.k, r.score_scale, 0, s)
@@ -1177,6 +1201,215 @@ B200MS_API int b200ms_page_rows_device(b200ms_t* h, const int64_t* src_pages_hos
   if (int e = upload(h, h->src_pages, meta.data(), meta.size() * 8, s)) return e;
   const int64_t* d = static_cast<const int64_t*>(h->src_pages.p);
   return launch_page_rows(h, d, d + n_src, n_src, n_rows, scale, out, s);
+}
+
+// ---- relevance feedback: weighted examples, one fused score per request
+// The examples of a call: n_qe query embeddings (rows of q_dev, lengths q_lens) then n_src stored pages; example i belongs to
+// request ex_req[i] and carries weight ex_w[i].  Their true lengths (tokens, rows) into *lens, in example order.
+static int check_examples(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_qe, const int64_t* src,
+                          int n_src, const int32_t* ex_req, const float* ex_w, int n_req, const char* what,
+                          std::vector<int32_t>* lens) {
+  const Corpus& c = h->corpus;
+  const std::string w(what);
+  if (c.dtype < 0) return set_error(h, B200MS_ESTATE, w + ": no corpus attached");
+  if (n_qe < 0 || n_src < 0 || n_qe + n_src < 1 || n_req < 1 || !ex_req || !ex_w ||
+      (n_qe > 0 && (!q_dev || !q_lens || !src_dtype_ok(src_dtype))) || (n_src > 0 && !src))
+    return set_error(h, B200MS_EINVAL, w + ": bad arguments (one or more examples, n_req >= 1, F32/BF16 query rows)");
+  lens->clear();
+  for (int i = 0; i < n_qe; ++i) {
+    if (q_lens[i] < 0) return set_error(h, B200MS_EINVAL, w + ": a query example has a negative length");
+    lens->push_back(q_lens[i]);
+  }
+  for (int i = 0; i < n_src; ++i) {
+    if (src[i] < 0 || src[i] >= c.n_pages)
+      return set_error(h, B200MS_EINVAL, w + ": example page " + std::to_string(src[i]) + " is not a page of the corpus (" +
+                                             std::to_string(c.n_pages) + " pages)");
+    lens->push_back(h->page_len_host[size_t(src[i])]);
+  }
+  std::vector<char> positive(size_t(n_req), 0);
+  for (int i = 0; i < n_qe + n_src; ++i) {
+    if (ex_req[i] < 0 || ex_req[i] >= n_req)
+      return set_error(h, B200MS_EINVAL, w + ": example " + std::to_string(i) + " names request " + std::to_string(ex_req[i]) +
+                                             " outside [0, " + std::to_string(n_req) + ")");
+    if (!std::isfinite(ex_w[i]) || ex_w[i] == 0.f)
+      return set_error(h, B200MS_EINVAL, w + ": example " + std::to_string(i) + " has a zero or non-finite weight");
+    if (ex_w[i] > 0.f) positive[size_t(ex_req[i])] = 1;
+  }
+  for (int q = 0; q < n_req; ++q)
+    if (!positive[size_t(q)])
+      return set_error(h, B200MS_EINVAL, w + ": request " + std::to_string(q) + " has no example of positive weight");
+  return B200MS_OK;
+}
+
+struct ExampleCall {
+  const int64_t* src_host;
+  int n_src, n_qe;
+  const int32_t* ex_req;
+  const float* ex_w;
+  int n_req;
+  const int64_t* cand;  // NULL: full scan; else the requests' lists [n_req, n_cand]
+  int n_cand;
+  const uint32_t* masks;  // n_masks > 0: one row per request through mask_index
+  int n_masks;
+  const int32_t* mask_index;
+};
+
+// Every example of every request scored in ONE search_scan (each example a query of it: query embeddings packed from q,
+// pages from their packed rows; in candidate mode every example scores its request's list), then one fused score row per
+// request (launch_fuse_examples) and one selection over those rows (launch_topk: one group per request, F32, scale 1).
+static int search_examples_ordered(b200ms_t* h, SearchRequest& r, const ExampleCall& x, cudaStream_t s) {
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  const Corpus& c = h->corpus;
+  const int n_ex = r.n_q, n_req = x.n_req;
+  const SearchMeta m = build_search_meta(r.q_lens, n_ex);
+  const int32_t* goff = m.goff();
+  const int64_t stride = x.cand ? CandSpec{x.cand, x.n_cand, 1}.stride() : 0;
+  // one upload: [source page ids int64 | the examples by request | req_off int32 [n_req+1] | 0..n_req int32 | ex_req int32]
+  const size_t off_items = size_t(x.n_src) * 8, off_req = off_items + size_t(n_ex) * sizeof(ExampleItem);
+  const size_t off_iota = off_req + size_t(n_req + 1) * 4, off_exreq = off_iota + size_t(n_req + 1) * 4;
+  std::vector<uint8_t> blk(off_exreq + size_t(n_ex) * 4);
+  if (x.n_src > 0) memcpy(blk.data(), x.src_host, off_items);
+  ExampleItem* items = reinterpret_cast<ExampleItem*>(blk.data() + off_items);
+  int32_t* req_off = reinterpret_cast<int32_t*>(blk.data() + off_req);
+  int32_t* iota = reinterpret_cast<int32_t*>(blk.data() + off_iota);
+  memcpy(blk.data() + off_exreq, x.ex_req, size_t(n_ex) * 4);
+  for (int q = 0; q <= n_req; ++q) req_off[q] = 0, iota[q] = q;
+  for (int i = 0; i < n_ex; ++i) req_off[x.ex_req[i] + 1]++;
+  for (int q = 0; q < n_req; ++q) req_off[q + 1] += req_off[q];
+  std::vector<int32_t> fill(req_off, req_off + n_req);
+  for (int i = 0; i < n_ex; ++i)  // stable: a request's examples stay in example order
+    items[fill[size_t(x.ex_req[i])]++] = ExampleItem{goff[i], goff[i + 1], float(r.q_lens[i]), x.ex_w[i], int64_t(i) * stride};
+  if (int e = upload(h, h->ex_meta, blk.data(), blk.size(), s)) return e;
+  const uint8_t* md = static_cast<const uint8_t*>(h->ex_meta.p);
+  const ExampleItem* items_dev = reinterpret_cast<const ExampleItem*>(md + off_items);
+  const int32_t* req_off_dev = reinterpret_cast<const int32_t*>(md + off_req);
+  const int32_t* iota_dev = reinterpret_cast<const int32_t*>(md + off_iota);
+  const int32_t* ex_req_dev = reinterpret_cast<const int32_t*>(md + off_exreq);
+  if (x.n_src > 0) {
+    r.src_pages = reinterpret_cast<const int64_t*>(md);
+    r.src_first = x.n_qe;
+  }
+  const uint32_t* allow = x.n_masks > 0 ? x.masks : nullptr;
+  const int32_t* mask_index = x.n_masks > 0 ? x.mask_index : nullptr;
+  int64_t* req_lists = nullptr;
+  if (x.cand) {  // [n_req + n_ex, stride]: the requests' lists padded to 32-slot strides, then every example's request's list
+    if (int e = reserve(h, h->ex_lists, size_t(n_req + n_ex) * size_t(stride) * 8)) return e;
+    req_lists = static_cast<int64_t*>(h->ex_lists.p);
+    int64_t* ex_lists = req_lists + int64_t(n_req) * stride;
+    if (int e = launch_pad_cands(h, x.cand, x.n_cand, n_req, stride, req_lists, s)) return e;
+    if (int e = launch_gather_rows<int64_t>(h, req_lists, stride, ex_req_dev, n_ex, ex_lists, s)) return e;
+    r.cand = CandSpec{ex_lists, int(stride), 1};
+  } else if (allow) {  // the filtered scan reads the pages any example's request may return
+    if (int e = reserve(h, h->ex_lists, size_t(n_ex) * 4)) return e;
+    int32_t* ex_mask_index = static_cast<int32_t*>(h->ex_lists.p);
+    if (int e = launch_gather_rows<int32_t>(h, mask_index, 1, ex_req_dev, n_ex, ex_mask_index, s)) return e;
+    r.allow = allow;
+    r.mask_index = ex_mask_index;
+  }
+  ScanResult sr;
+  if (int e = search_scan(h, r, m, s, nullptr, &sr)) return e;
+  if (!x.cand) {
+    const int64_t words = (c.n_pages + 31) / 32, fld = words * 32 > 32 ? words * 32 : 32;
+    if (int e = reserve(h, h->ex_fused, size_t(n_req) * size_t(fld) * 4)) return e;
+    float* fused = static_cast<float*>(h->ex_fused.p);
+    if (int e = launch_fuse_examples(h, h->scores.p, sr.sdt, sr.ld, items_dev, req_off_dev, n_req, c.n_pages, allow, mask_index,
+                                     words, r.score_scale, fused, fld, s))
+      return e;
+    return launch_topk(h, fused, B200MS_F32, c.n_pages, fld, iota_dev, n_req, allow, r.k, 1.f, r.id_base, nullptr, r.top_scores,
+                       r.top_ids, r.top_counts, s, mask_index, words);
+  }
+  // candidate mode: request r's slots are r * stride + j; its valid-slot bits (unused slots and pages its mask row forbids
+  // cleared) filter both the fusion and the selection
+  const int64_t n_slots = int64_t(n_req) * stride;
+  uint32_t* slot_mask = nullptr;
+  if (int e = reserve(h, h->cand_mask, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
+  slot_mask = static_cast<uint32_t*>(h->cand_mask.p);
+  if (int e = launch_cand_units(h, corpus_view(h), req_lists, int(n_slots), nullptr, nullptr, slot_mask, s)) return e;
+  if (allow)
+    if (int e = launch_mask_cand_slots(h, req_lists, n_slots, stride, allow, mask_index, slot_mask, s)) return e;
+  if (int e = reserve(h, h->ex_fused, size_t(n_slots) * 4)) return e;
+  float* fused = static_cast<float*>(h->ex_fused.p);
+  if (int e = launch_fuse_examples(h, h->scores.p, sr.sdt, sr.ld, items_dev, req_off_dev, n_req, x.n_cand, slot_mask, nullptr,
+                                   stride / 32, r.score_scale, fused, stride, s))
+    return e;
+  // all requests' fused slots form ONE row (request r's at r * stride, where the selection looks for them); with ld 0 that
+  // row is every request's one group
+  return launch_topk(h, fused, B200MS_F32, x.n_cand, 0, iota_dev, n_req, slot_mask, r.k, 1.f, 0, req_lists, r.top_scores,
+                     r.top_ids, r.top_counts, s, nullptr, 0, stride);
+}
+
+B200MS_API int b200ms_search_examples_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_qe,
+                                             const int64_t* src_pages_host, int n_src, const int32_t* ex_req_host,
+                                             const float* ex_weight_host, int n_req, int k, const uint32_t* allow_masks_dev,
+                                             int n_masks, const int32_t* mask_index_dev, float i8_q_scale, float score_scale,
+                                             int64_t id_base, float* top_scores_dev, int64_t* top_ids_dev,
+                                             int32_t* top_counts_dev, void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  if (h->corpus.host) return set_error(h, B200MS_ESTATE, kHostFullScan);
+  std::vector<int32_t> lens;
+  if (int e = check_examples(h, q_dev, src_dtype, q_lens, n_qe, src_pages_host, n_src, ex_req_host, ex_weight_host, n_req,
+                             "search_examples_device", &lens))
+    return e;
+  if (int e = check_masks(h, allow_masks_dev, n_masks, mask_index_dev, "search_examples_device")) return e;
+  if (k < 1 || k > B200MS_MAX_K || !top_scores_dev || !top_ids_dev || !top_counts_dev)
+    return set_error(h, B200MS_EINVAL, "search_examples_device: bad arguments (1 <= k <= 4096, outputs)");
+  DeviceGuard g(h->device);
+  SearchRequest r{q_dev, src_dtype, lens.data(), n_qe + n_src, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev,
+                  top_counts_dev, id_base};
+  const ExampleCall x{src_pages_host, n_src, n_qe, ex_req_host, ex_weight_host, n_req, nullptr, 0, allow_masks_dev, n_masks,
+                      mask_index_dev};
+  return search_examples_ordered(h, r, x, static_cast<cudaStream_t>(cuda_stream));
+}
+
+B200MS_API int b200ms_rerank_examples_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens,
+                                                   int n_qe, const int64_t* src_pages_host, int n_src,
+                                                   const int32_t* ex_req_host, const float* ex_weight_host, int n_req,
+                                                   const int64_t* cand_ids_dev, int n_cand, int k,
+                                                   const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
+                                                   float i8_q_scale, float score_scale, float* top_scores_dev,
+                                                   int64_t* top_ids_dev, int32_t* top_counts_dev, void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  std::vector<int32_t> lens;
+  if (int e = check_examples(h, q_dev, src_dtype, q_lens, n_qe, src_pages_host, n_src, ex_req_host, ex_weight_host, n_req,
+                             "rerank_examples_batch_device", &lens))
+    return e;
+  if (int e = check_masks(h, allow_masks_dev, n_masks, mask_index_dev, "rerank_examples_batch_device")) return e;
+  const CandSpec cand{cand_ids_dev, n_cand, 1};
+  if (!cand_ids_dev || n_cand < 1 || cand.n_slots(n_req + n_qe + n_src) >= (int64_t(1) << 30) || k < 1 || k > B200MS_MAX_K ||
+      !top_scores_dev || !top_ids_dev || !top_counts_dev)
+    return set_error(h, B200MS_EINVAL,
+                     "rerank_examples_batch_device: bad arguments (n_cand >= 1, (n_req + examples)*n_cand < 2^30, 1 <= k <= 4096)");
+  DeviceGuard g(h->device);
+  SearchRequest r{q_dev, src_dtype, lens.data(), n_qe + n_src, k, i8_q_scale, score_scale, top_scores_dev, top_ids_dev,
+                  top_counts_dev};
+  const ExampleCall x{src_pages_host, n_src, n_qe, ex_req_host, ex_weight_host, n_req, cand_ids_dev, n_cand, allow_masks_dev,
+                      n_masks, mask_index_dev};
+  return search_examples_ordered(h, r, x, static_cast<cudaStream_t>(cuda_stream));
+}
+
+B200MS_API int b200ms_union_candidates_device(b200ms_t* h, const int64_t* cand_ids_dev, int n_lists, int n_cand,
+                                              const int32_t* list_off_host, int n_req, int64_t* out_dev, int width,
+                                              void* cuda_stream) {
+  if (!h) return B200MS_EINVAL;
+  if (n_req < 1 || n_lists < 0 || n_cand < 1 || width < 1 || !list_off_host || !out_dev || (n_lists > 0 && !cand_ids_dev) ||
+      int64_t(n_lists) * n_cand >= (int64_t(1) << 30))
+    return set_error(h, B200MS_EINVAL, "union_candidates_device: bad arguments (n_req >= 1, n_cand >= 1, width >= 1, n_lists*n_cand < 2^30)");
+  int64_t most = 0;
+  bool ok = list_off_host[0] == 0 && list_off_host[n_req] == n_lists;
+  for (int q = 0; q < n_req && ok; ++q) {
+    ok = list_off_host[q + 1] >= list_off_host[q];
+    most = std::max(most, int64_t(list_off_host[q + 1] - list_off_host[q]) * n_cand);
+  }
+  if (!ok)
+    return set_error(h, B200MS_EINVAL, "union_candidates_device: list_off must rise from 0 to n_lists");
+  DeviceGuard g(h->device);
+  cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  if (int e = upload(h, h->ex_meta, list_off_host, size_t(n_req + 1) * 4, s)) return e;
+  return launch_union_candidates(h, cand_ids_dev, n_cand, static_cast<const int32_t*>(h->ex_meta.p), n_req, most, out_dev,
+                                 width, s);
 }
 
 // Small unmasked zero-copy calls repeat with the same shapes (interactive queries): the second call of a shape is captured

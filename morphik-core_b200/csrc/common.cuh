@@ -96,8 +96,19 @@ struct SearchRequest {
   const int32_t* mask_index = nullptr;   // per query: row of `allow` (-1 = no mask); NULL = the one mask for every query
   CandSpec cand;                         // ids == NULL: full scan
   const DocSpec* docs = nullptr;         // != NULL: the top k documents (per-query candidate lists only) instead of pages
-  const int64_t* src_pages = nullptr;    // != NULL (device, [n_q]): query q is corpus page src_pages[q], its packed rows taken
-                                         // as they are stored (q and q_dtype unused; q_lens = the pages' true lengths)
+  const int64_t* src_pages = nullptr;    // != NULL (device, [n_q - src_first]): query q >= src_first is corpus page
+                                         // src_pages[q - src_first], its packed rows taken as they are stored (q_lens = the
+                                         // pages' true lengths); queries before src_first are rows of q (q_dtype) as usual
+  int src_first = 0;
+};
+
+// What the scan part of a search (search_scan) leaves for its selection: the candidate lists it scored (cs.ids == NULL: a
+// full scan), the score matrix's row stride, its group offsets on the device and its score dtype (F32 | I32)
+struct ScanResult {
+  CandSpec cs;
+  int64_t ld = 0;
+  const int32_t* goff_dev = nullptr;
+  int sdt = 0;
 };
 
 // Results of a search as one block: [n_q*k int64 ids | n_q*k f32 scores | n_q int32 counts], padded to 16 bytes, so that
@@ -266,6 +277,9 @@ struct b200ms {
   bms::DeviceBuf mmr_state, mmr_partials;
   // searching with stored pages as the queries (search_pages.cu): the call's source page ids [, their true-row offsets]
   bms::DeviceBuf src_pages;
+  // relevance feedback (search_examples.cu): the call's example table, the requests' and examples' candidate lists (or the
+  // examples' mask rows), the fused score rows, and the hash tables of a candidate union
+  bms::DeviceBuf ex_meta, ex_lists, ex_fused, ex_union;
 };
 
 namespace bms {
@@ -306,6 +320,8 @@ void release_blocks(b200ms_t* h);  // block.cu: unmap, release and free every bl
 // pack -> score -> top-k of r on stream s (api.cu); m = build_search_meta(r.q_lens, r.n_q).  meta_dev != NULL: m's block
 // already sits in device-readable memory at this address (mapped pinned staging) -- no upload; else ONE cudaMemcpyAsync.
 int search_core(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev = nullptr);
+// search_core without the selection: pack -> score, the group scores left in h->scores as *out describes them
+int search_scan(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaStream_t s, const void* meta_dev, ScanResult* out);
 
 // Full scan: unit u = chunks [unit_start[u], unit_start[u+1]) of the attached corpus, scores indexed by page id
 inline UnitPlan full_scan_plan(const b200ms_t* h) {
@@ -422,9 +438,10 @@ int launch_merge_topk(b200ms_t* h, const float* cand_scores, const int64_t* cand
                       float* top_scores, int64_t* top_ids, int32_t* top_counts, cudaStream_t s);
 // search_pages.cu.  src_dev: device page ids of the attached corpus (checked by the caller); ss_dev / ds_dev: [n_src+1] true /
 // padded row offsets of the sources (build_search_meta of their lengths).
-// The sources' packed rows in the query layout of b200ms_pack_queries (dst_rows rows, zero past each source's true rows)
+// The sources' packed rows in the query layout of b200ms_pack_queries: rows [row0, dst_rows) of dst, zero past each source's
+// true rows.  ss_dev / ds_dev may be the tail of a longer layout (the sources after some query rows): row0 = ds_dev[0].
 int launch_pack_src_pages(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, const int64_t* ds_dev, int64_t n_src,
-                          int64_t dst_rows, void* dst, cudaStream_t s);
+                          int64_t row0, int64_t dst_rows, void* dst, cudaStream_t s);
 // The sources' true rows back to back as float32 [n_rows, 128]: packed value (a sign bit as +-1) times scale
 int launch_page_rows(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, int64_t n_src, int64_t n_rows, float scale,
                      float* out, cudaStream_t s);
@@ -434,5 +451,26 @@ int launch_mask_cand_slots(b200ms_t* h, const int64_t* cand, int64_t n_slots, in
 // Reported scores of source q divided by its true length; a source without rows gets count 0
 int launch_normalise_pages(b200ms_t* h, const int64_t* src_dev, int n_src, int k, float* scores, int64_t* ids,
                            int32_t* counts, cudaStream_t s);
+// search_examples.cu.  One example of a request: its group rows [g0, g1) of the score matrix (g0 == g1: no rows, no term),
+// its true rows or tokens, its weight, and the score column of its item 0 (candidate mode: its list's first slot).
+struct ExampleItem {
+  int32_t g0, g1;
+  float len, w;
+  int64_t col0;
+};
+// dst row i = src row idx[i] (row_len elements each); T = int32_t or int64_t
+template <typename T>
+int launch_gather_rows(b200ms_t* h, const T* src, int64_t row_len, const int32_t* idx, int n_rows, T* dst, cudaStream_t s);
+// fused[r * fused_ld + p], p < n_items: sum over request r's examples (items[req_off[r] .. req_off[r+1]), in order) of
+// w * (float(finish_sum(its groups' scores at col0 + p)) * score_scale / len), with _rn arithmetic; items whose bit in r's
+// allow row (mask_index ? allow row mask_index[r] : allow row r, rows mask_stride words apart; -1 / NULL = all) is clear
+// are not read or written.
+int launch_fuse_examples(b200ms_t* h, const void* gs, int score_dtype, int64_t ld, const ExampleItem* items,
+                         const int32_t* req_off, int n_req, int64_t n_items, const uint32_t* allow, const int32_t* mask_index,
+                         int64_t mask_stride, float score_scale, float* fused, int64_t fused_ld, cudaStream_t s);
+// out [n_req, width]: request r's distinct page ids (>= 0) over lists list_off[r] .. list_off[r+1] of cand [*, n_cand], in
+// first-occurrence order, -1 padded; tables: h->ex_union scratch
+int launch_union_candidates(b200ms_t* h, const int64_t* cand, int n_cand, const int32_t* list_off_dev, int n_req,
+                            int64_t max_entries, int64_t* out, int width, cudaStream_t s);
 
 }  // namespace bms

@@ -19,8 +19,8 @@ __device__ __forceinline__ int64_t item_of(const int64_t* __restrict__ start, in
 }
 
 // Query layout from corpus pages: destination row r of source i (rows ds[i] .. ds[i+1]) is row r - ds[i] of page src[i]
-// while that is below the page's true length (ss[i+1] - ss[i]), else zero; rows from ds[n] to dst_rows are zero.  One
-// thread per 16-byte piece; the bytes are copied as stored.  rows may be mapped host memory (a host-resident corpus): only
+// while that is below the page's true length (ss[i+1] - ss[i]), else zero; rows from ds[n] to dst_rows are zero, and rows
+// before ds[0] (another packer's) are not touched.  One thread per 16-byte piece; the bytes are copied as stored.  rows may be mapped host memory (a host-resident corpus): only
 // the source pages' true rows are read.
 __global__ void __launch_bounds__(256)
 pack_src_pages_kernel(const uint4* __restrict__ rows, int64_t pieces_per_row, const int64_t* __restrict__ page_start,
@@ -28,7 +28,8 @@ pack_src_pages_kernel(const uint4* __restrict__ rows, int64_t pieces_per_row, co
                       int64_t n_src, int64_t dst_rows, uint4* __restrict__ dst) {
   const int64_t total = dst_rows * pieces_per_row;
   const int64_t used = __ldg(ds + n_src) * pieces_per_row;
-  for (int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < total; t += int64_t(gridDim.x) * blockDim.x) {
+  for (int64_t t = __ldg(ds) * pieces_per_row + int64_t(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+       t += int64_t(gridDim.x) * blockDim.x) {
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
     if (t < used) {
       const int64_t r = t / pieces_per_row, piece = t - r * pieces_per_row;
@@ -119,11 +120,11 @@ static int blocks_for(b200ms_t* h, int64_t threads) {
 }
 
 int launch_pack_src_pages(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, const int64_t* ds_dev, int64_t n_src,
-                          int64_t dst_rows, void* dst, cudaStream_t s) {
-  if (dst_rows <= 0) return B200MS_OK;
+                          int64_t row0, int64_t dst_rows, void* dst, cudaStream_t s) {
+  if (dst_rows <= row0) return B200MS_OK;
   const Corpus& c = h->corpus;
   const int64_t ppr = b200ms_row_bytes(c.dtype) / 16;
-  pack_src_pages_kernel<<<blocks_for(h, dst_rows * ppr), 256, 0, s>>>(
+  pack_src_pages_kernel<<<blocks_for(h, (dst_rows - row0) * ppr), 256, 0, s>>>(
       static_cast<const uint4*>(c.rows), ppr, static_cast<const int64_t*>(h->page_start.p), src_dev, ss_dev, ds_dev, n_src,
       dst_rows, static_cast<uint4*>(dst));
   h->launches++;

@@ -895,6 +895,113 @@ class MaxSimIndex:
                                                          _vp(out), self._stream()), "b200ms_page_rows_device")
         return out, lens
 
+    # ------------------------------------------------------------------ relevance feedback: weighted examples
+    def _examples(self, q_dev: Optional[torch.Tensor], q_lens: Sequence[int], ex_pages, ex_req: Sequence[int],
+                  ex_weights: Sequence[float], n_req: int):
+        """Checked examples of a request batch (ValueError before any launch): n_qe query embeddings (rows of q_dev, lengths
+        q_lens), then stored pages ex_pages; example i belongs to request ex_req[i] and weighs ex_weights[i] (finite and
+        non-zero in float32), and every request has an example of positive weight.  Returns (q dtype code, q_lens, page
+        ids, ex_req, float32 weights)."""
+        q_lens = [int(n) for n in q_lens]
+        pages = [int(p) for p in (ex_pages.tolist() if isinstance(ex_pages, (np.ndarray, torch.Tensor)) else ex_pages)]
+        req = [int(r) for r in ex_req]
+        w = np.asarray(list(ex_weights), dtype=np.float32)
+        n_ex, n_req = len(q_lens) + len(pages), int(n_req)
+        if n_ex < 1 or n_req < 1 or len(req) != n_ex or w.shape != (n_ex,):
+            raise ValueError(f"examples: {len(q_lens)} query + {len(pages)} page examples need one request and one weight "
+                             f"each (got {len(req)} and {w.size}), n_req >= 1")
+        if any(n < 0 for n in q_lens):
+            raise ValueError(f"q_lens must be >= 0, got {q_lens}")
+        if q_lens and q_dev is None:
+            raise ValueError("query examples need their rows: q_dev is None")
+        q_dtype = _check_queries(q_dev, q_lens, self.device) if q_lens else nat.F32
+        if any(not 0 <= p < self.n_pages for p in pages):
+            raise ValueError(f"example pages must be page ids in [0, {self.n_pages}), got {pages}")
+        if any(not 0 <= r < n_req for r in req):
+            raise ValueError(f"ex_req must name requests in [0, {n_req}), got {req}")
+        if not np.all(np.isfinite(w)) or np.any(w == 0):
+            raise ValueError(f"example weights must be finite and non-zero in float32, got {w.tolist()}")
+        if len({r for r, x in zip(req, w) if x > 0}) != n_req:
+            raise ValueError("every request needs an example of positive weight")
+        return q_dtype, q_lens, pages, req, w
+
+    def _request_masks(self, allow_mask_dev, mask_index_dev, n_req: int):
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, n_req, self.n_pages, self.device)
+        if masks is not None and index is None:  # one mask for every request: a one-row matrix
+            index = torch.zeros((n_req,), dtype=torch.int32, device=self.device)
+        return masks, n_masks, index
+
+    def search_examples(self, q_dev: Optional[torch.Tensor], q_lens: Sequence[int], ex_pages, ex_req: Sequence[int],
+                        ex_weights: Sequence[float], n_req: int, k: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                        mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0,
+                        out: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
+        """Relevance feedback (b200ms_search_examples_device), asynchronous on torch's current stream: each of n_req requests
+        ranks pages by the weighted sum of their scores against its examples, all examples scored in one full scan.
+        Examples: query embeddings (q_dev [sum q_lens, 128] float32 | bfloat16, or None without query examples), then stored
+        page ids ``ex_pages``; ``ex_req`` / ``ex_weights`` give each one's request and weight (> 0 like, < 0 unlike).  An
+        example's score is the page-to-page scale of search_pages: the MaxSim per example row (or token).  Masks as
+        search_device, one row per REQUEST; example pages are returned unless their bits are clear.  Returns device tensors
+        (scores float32 [n_req,k], page ids + id_base int64 [n_req,k], counts int32 [n_req])."""
+        q_dtype, q_lens, pages, req, w = self._examples(q_dev, q_lens, ex_pages, ex_req, ex_weights, n_req)
+        masks, n_masks, index = self._request_masks(allow_mask_dev, mask_index_dev, int(n_req))
+        ts, ti, tc = _topk_outputs(int(n_req), int(k), self.device, out)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_search_examples_device(
+                    self.h.ptr, _vp(q_dev) if q_lens else None, q_dtype, nat.i32_array(q_lens), len(q_lens),
+                    nat.i64_array(pages), len(pages), nat.i32_array(req), nat.f32_array(w), int(n_req), int(k), _vp(masks),
+                    n_masks, _vp(index), ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base),
+                    _vp(ts), _vp(ti), _vp(tc), self._stream()),
+                "b200ms_search_examples_device")
+        return ts, ti, tc
+
+    def rerank_examples_batch(self, q_dev: Optional[torch.Tensor], q_lens: Sequence[int], ex_pages, ex_req: Sequence[int],
+                              ex_weights: Sequence[float], n_req: int, cand_ids: torch.Tensor, k: int,
+                              allow_mask_dev: Optional[torch.Tensor] = None, mask_index_dev: Optional[torch.Tensor] = None,
+                              out: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
+        """search_examples over one candidate list per request, cand_ids int64 [n_req, n_cand] (-1 = unused slot;
+        b200ms_rerank_examples_batch_device): every example of request r scores r's list, ties go to the lower slot, and a
+        candidate r's mask row forbids is an unused slot.  k is capped at n_cand.  Works on both tiers."""
+        q_dtype, q_lens, pages, req, w = self._examples(q_dev, q_lens, ex_pages, ex_req, ex_weights, n_req)
+        n_cand, kk = _check_candidates(cand_ids, int(n_req), k, self.device, per_query=True)
+        masks, n_masks, index = self._request_masks(allow_mask_dev, mask_index_dev, int(n_req))
+        ts, ti, tc = _topk_outputs(int(n_req), kk, self.device, out)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_rerank_examples_batch_device(
+                    self.h.ptr, _vp(q_dev) if q_lens else None, q_dtype, nat.i32_array(q_lens), len(q_lens),
+                    nat.i64_array(pages), len(pages), nat.i32_array(req), nat.f32_array(w), int(n_req), _vp(cand_ids),
+                    n_cand, kk, _vp(masks), n_masks, _vp(index), ctypes.c_float(self.i8_scale),
+                    ctypes.c_float(self.score_scale), _vp(ts), _vp(ti), _vp(tc), self._stream()),
+                "b200ms_rerank_examples_batch_device")
+        return ts, ti, tc
+
+    def union_candidates(self, cand_ids: torch.Tensor, list_off: Sequence[int], width: Optional[int] = None) -> torch.Tensor:
+        """Union of first-stage lists on the device (b200ms_union_candidates_device), asynchronous: request r owns rows
+        list_off[r] .. list_off[r+1] of cand_ids int64 [n_lists, n_cand]; returns int64 [n_req, width] with r's distinct page
+        ids (negative ids are unused slots) in first-occurrence order, row-major over its lists, -1 padded.  ``width``
+        defaults to the most slots any request owns (nothing is cut)."""
+        off = [int(o) for o in list_off]
+        n_lists = int(cand_ids.shape[0]) if cand_ids.ndim == 2 else -1
+        if (cand_ids.dtype != torch.int64 or cand_ids.ndim != 2 or not cand_ids.is_contiguous() or cand_ids.device != self.device
+                or cand_ids.shape[1] < 1):
+            raise ValueError(f"cand_ids must be a contiguous int64 [n_lists, n_cand >= 1] tensor on {self.device}")
+        if len(off) < 2 or off[0] != 0 or off[-1] != n_lists or any(b < a for a, b in zip(off, off[1:])):
+            raise ValueError(f"list_off must rise from 0 to n_lists = {n_lists}, got {off}")
+        n_cand = int(cand_ids.shape[1])
+        width = int(width) if width is not None else max(1, max(b - a for a, b in zip(off, off[1:])) * n_cand)
+        if width < 1:
+            raise ValueError(f"width must be >= 1, got {width}")
+        out = torch.empty((len(off) - 1, width), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_union_candidates_device(self.h.ptr, _vp(cand_ids), n_lists, n_cand, nat.i32_array(off),
+                                                       len(off) - 1, _vp(out), width, self._stream()),
+                "b200ms_union_candidates_device")
+        return out
+
     # ------------------------------------------------------------------ grouping results by document
     def _check_docs_args(self, per_doc: int, page_doc_dev: torch.Tensor):
         if not 1 <= int(per_doc) <= nat.MAX_PER_DOC:

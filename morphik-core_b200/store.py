@@ -563,6 +563,73 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
         return out
 
+    async def query_similar_with_feedback(self, query_embedding=None, k: int = 10,
+                                          positive_chunks: Sequence[Tuple[str, int]] = (),
+                                          negative_chunks: Sequence[Tuple[str, int]] = (),
+                                          doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None,
+                                          min_score: Optional[float] = None) -> List[DocumentChunk]:
+        """Relevance feedback (extension; the "recommend" call of vector databases): chunks like the query and the chunks
+        marked good, unlike the chunks marked wrong.  Chunk ids follow ``get_chunks_by_id``'s rules (unknown or deleted
+        chunks and chunks of another ``app_id`` are skipped, duplicates collapsed); a chunk in both lists is a ValueError.
+        The query (if given) and each positive chunk weigh +1/n_pos, each negative chunk -1/n_neg, so a chunk's score is
+        its mean similarity to the positives minus its mean similarity to the negatives, each on the page-to-page scale of
+        query_similar_to_chunks (MaxSim per example row or query token: about 1 for an exact copy of unit-norm positives).
+        ``doc_ids`` / ``app_id`` filter the results as in query_similar and the example chunks are never returned;
+        ``min_score`` drops hits below it.  Every example shares one pass over the corpus (with a first stage, the
+        positives' candidates); masks, GPU search and chunk construction are one critical section.  No query and no
+        visible positive chunk: []."""
+        q = None if query_embedding is None else as_query_matrix(query_embedding)
+        pos_ids = list(dict.fromkeys((d, int(n)) for d, n in positive_chunks))
+        neg_ids = list(dict.fromkeys((d, int(n)) for d, n in negative_chunks))
+        both = set(pos_ids) & set(neg_ids)
+        if both:
+            raise ValueError(f"chunks named as both positive and negative examples: {sorted(both)}")
+        if k <= 0 or (q is None and not pos_ids):
+            return []
+        return await asyncio.to_thread(self._feedback_locked, q, int(k), pos_ids, neg_ids, doc_ids, app_id, min_score)
+
+    def _feedback_locked(self, q, k, pos_ids, neg_ids, doc_ids, app_id, min_score):
+        import torch
+
+        t0 = time.perf_counter()
+        with self._lock:
+            pos = [pid for pid, _ in self._visible_records(pos_ids, app_id)] if pos_ids else []
+            neg = [pid for pid, _ in self._visible_records(neg_ids, app_id)] if neg_ids else []
+            n_pos = len(pos) + (q is not None)
+            if n_pos == 0:
+                return []
+            n = len(self.catalog)
+            mask = self.catalog.allow_mask(doc_ids, app_id)
+            mask = self.catalog.alive[:n].copy() if mask is None else mask
+            mask[pos + neg] = False  # the examples themselves are never results
+            if not mask.any():
+                return []
+            words = PageCatalog.mask_words(mask)[None]
+            kk = min(_capped_k(k), n)
+            queries = [] if q is None else [q]
+            pages = pos + neg
+            weights = [1.0 / n_pos] * n_pos + ([-1.0 / len(neg)] * len(neg) if neg else [])
+            ex_req = [0] * len(weights)
+            t1 = time.perf_counter()
+            if self._two_stage is not None:  # the positives' first-stage candidates, under the same mask
+                ts, ti, tc = self._two_stage.search_examples(queries, pages, ex_req, weights, 1, kk,
+                                                             n_candidates=max(self._n_candidates, kk), allow_masks=words)
+            else:
+                dev = torch.device(self._index.device)
+                q_dev = None if q is None else torch.from_numpy(np.ascontiguousarray(q, np.float32)).to(dev)
+                mat = torch.from_numpy(words.view(np.int32)).to(dev)
+                index = torch.zeros((1,), dtype=torch.int32, device=dev)
+                ts, ti, tc = (np.asarray(t.cpu()) for t in self._index.search_examples(
+                    q_dev, [int(q.shape[0])] if q is not None else [], pages, ex_req, weights, 1, kk, mat, index))
+            t2 = time.perf_counter()
+            out = self._chunks(ts[0], ti[0], int(tc[0]), min_score)
+            t3 = time.perf_counter()
+        self.last_query_timing = {"prepare_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3,
+                                  "build_chunks_ms": (t3 - t2) * 1e3, "total_ms": (t3 - t0) * 1e3}
+        if self._two_stage is not None:
+            self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
+        return out
+
     async def get_chunks_by_id(self, chunk_identifiers: List[Tuple[str, int]], app_id: Optional[str] = None,
                                skip_image_content: bool = False) -> List[DocumentChunk]:
         if not chunk_identifiers:

@@ -167,6 +167,76 @@ class TwoStageSearch:
         self.last_timing_ms = self.stage_timing_ms(ev)
         return out
 
+    def search_examples_device(self, queries: Sequence, pages, ex_req: Sequence[int], ex_weights: Sequence[float], n_req: int,
+                               k: int, n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None,
+                               mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0):
+        """MaxSimIndex.search_examples through the first stage: the query embeddings ``queries`` (host [T,128] arrays) and
+        stored ``pages`` are the examples, in that order, with ``ex_req`` / ``ex_weights`` as there.  Only the POSITIVE
+        examples pick candidates -- query embeddings through _encode, pages through their dequantised rows
+        (MaxSimIndex.page_rows) -- each under its request's mask row, in one first-stage scan; a request's lists are joined
+        by MaxSimIndex.union_candidates, and MaxSimIndex.rerank_examples_batch scores every example, negatives included,
+        against that union.  Returns as search_device."""
+        queries = list(queries)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        ev[0].record()
+        src = self.index._stage_rows(queries)[0] if queries else None
+        _, q_lens, pages, req, w = self.index._examples(src, [int(q.shape[0]) for q in queries], pages, ex_req, ex_weights,
+                                                        n_req)
+        masks, _, index = self.index._request_masks(allow_mask_dev, mask_index_dev, int(n_req))
+        if masks is not None and masks.ndim == 1:
+            masks = masks.view(1, -1)
+        n_qe = len(q_lens)
+        pos = sorted((r, i) for i, (r, x) in enumerate(zip(req, w)) if x > 0)  # by request, then in example order
+        q_off = np.concatenate([[0], np.cumsum(q_lens, dtype=np.int64)]) if n_qe else None
+        pos_pages = [i - n_qe for _, i in pos if i >= n_qe]
+        p_rows, p_lens = self.index.page_rows([pages[j] for j in pos_pages]) if pos_pages else (None, [])
+        p_off = np.concatenate([[0], np.cumsum(p_lens, dtype=np.int64)])
+        rows, lens, j = [], [], 0
+        for _, i in pos:
+            if i < n_qe:
+                rows.append(src[int(q_off[i]):int(q_off[i + 1])].float())
+                lens.append(q_lens[i])
+            else:
+                rows.append(p_rows[int(p_off[j]):int(p_off[j + 1])])
+                lens.append(int(p_lens[j]))
+                j += 1
+        q = self._encode(None, (torch.cat(rows).contiguous(), nat.F32, lens))
+        ev[1].record()
+        n_cand = self._n_cand(max(n_candidates, k))
+        if index is None:
+            _, ci, _ = self._scan(q, lens, n_cand, masks)
+        else:
+            pos_index = index[torch.tensor([r for r, _ in pos], dtype=torch.int64, device=self.device)].contiguous()
+            _, ci, _ = self._scan(q, lens, n_cand, masks, pos_index)
+        counts = np.bincount([r for r, _ in pos], minlength=int(n_req))
+        union = self.index.union_candidates(ci.contiguous(), np.concatenate([[0], np.cumsum(counts)]).tolist())
+        ev[2].record()
+        ts, ti, tc = self.index.rerank_examples_batch(src, q_lens, pages, req, w, n_req, union, k, masks, index)
+        if id_base:
+            ti = torch.where(ti >= 0, ti + int(id_base), ti)
+        ev[3].record()
+        return ts, ti, tc, ev
+
+    def search_examples(self, queries: Sequence, pages, ex_req: Sequence[int], ex_weights: Sequence[float], n_req: int, k: int,
+                        n_candidates: int = 1000, allow_masks: Optional[np.ndarray] = None):
+        """search_examples_device with host masks: ``allow_masks`` uint32 [n_req, words], one row per request, or None;
+        synchronous.  Returns host arrays (scores [n_req,k], page ids [n_req,k], counts [n_req]) and fills last_timing_ms
+        with search's stage names."""
+        n_req = int(n_req)
+        words = (self.n_pages + 31) // 32
+        masks = index = None
+        if allow_masks is not None:
+            m = np.ascontiguousarray(allow_masks, dtype=np.uint32)
+            if m.shape != (n_req, words):
+                raise ValueError(f"allow_masks must be uint32 [{n_req}, {words}], got {m.shape}")
+            masks = torch.from_numpy(m.view(np.int32)).to(self.device)
+            index = torch.arange(n_req, dtype=torch.int32, device=self.device)
+        ts, ti, tc, ev = self.search_examples_device(queries, pages, ex_req, ex_weights, n_req, k, n_candidates, masks, index)
+        torch.cuda.synchronize(self.device)
+        out = _host(ts, (n_req, k), -np.inf), _host(ti, (n_req, k), -1), tc.cpu().numpy().astype(np.int32)
+        self.last_timing_ms = self.stage_timing_ms(ev)
+        return out
+
     def search_docs_device(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
                            n_candidates: int = 1000, allow_mask_dev: Optional[torch.Tensor] = None):
         """Two-stage search grouped by document: max(n_candidates, k * per_doc) candidates per query (at most MAX_K), then
