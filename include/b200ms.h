@@ -197,13 +197,14 @@ int b200ms_pack_queries(b200ms_t* h, const void* q, int src_dtype, const int32_t
  * Value rule of BF16 and F8 corpora (the "float value rule"; every entry point that scores them follows it):
  *   - sim(q_t, d_r) is the dot product of the PACKED values (bf16, or e4m3 codes widened exactly to f16), rounded to fp32,
  *     with IEEE non-finite arithmetic: 0 * +-inf = NaN, NaN * x = NaN, +inf + -inf = NaN.  The products are exact and
- *     the finite sum is rounded to fp32: past its range to +-inf, into its subnormal range as IEEE rounds, below half the
- *     least subnormal to 0.  The order of the fp32 additions is the tensor core's, so a finite result can differ from the
+ *     the finite sum is rounded to fp32: to nearest even in its normal range, past it to +-inf, and into its subnormal
+ *     range (below 2^-126) toward zero, to a multiple of 2^-149, as the tensor core rounds there.  The order of the fp32 additions is the tensor core's, so a finite result can differ from the
  *     exactly rounded sum by a few fp32 ulps per term (oracle/scoring.py TOL).
  *   - Measured on an NVIDIA H100 80GB HBM3 (700 W limit; wgmma m64n128k16 .bf16, fp32 accumulate), on every bf16 pattern
- *     and on one-hot products of powers of two: subnormal bf16 inputs are used as they are, not flushed; a product that
- *     lands in fp32's subnormal range is kept (2^-127 .. 2^-149 exact), 2^-150 and below give 0; a product of 2^128 or
- *     more gives +-inf.  A product does not overflow on its own: 2^64 * 2^64 + (-2^64) * 2^64 inside one 16-element MMA
+ *     and on one-hot products of bf16 patterns and powers of two: subnormal bf16 inputs are used as they are, not flushed;
+ *     a product that lands in fp32's subnormal range is kept where it is a multiple of 2^-149 (2^-127 .. 2^-149 exact) and
+ *     truncated toward zero otherwise (1.0078 * 2^-150 gives 0, 1.5 * 2^-149 gives 2^-149, where round-to-nearest would
+ *     give 2^-149 and 2^-148); a product of 2^128 or more gives +-inf.  A product does not overflow on its own: 2^64 * 2^64 + (-2^64) * 2^64 inside one 16-element MMA
  *     step gives 0, not NaN (partial sums across steps are fp32).  e4m3 products lie in [2^-18, 448^2] and are exact.
  *   - The max over a page's TRUE rows is fmaxf's: a NaN row is ignored unless every row is NaN (then the max is NaN).
  *   - The group score sums the query's true tokens only, so a query's score is the IEEE sum of its tokens' maxima:
@@ -432,7 +433,8 @@ int b200ms_mmr_device(b200ms_t* h, const int64_t* cand_ids, const float* cand_sc
  *     scale.  I8: the sum follows the I32 sum rule of b200ms_topk -- a row scores at most 128 * 128 * 128 = 2^21 (-128 codes
  *     against -128 rows), so a source of 1024 rows can pass 2^31 - 1 (1033 rows of +-127 codes against -128 rows, 1041
  *     against +-127 rows); such pages are clamped to the bound and tie there, lower page id (slot) first.
- *     A source page with zero rows gets count 0 (every slot -inf / -1).
+ *     A source page with zero rows gets count 0 (every slot -inf / -1).  zero_pad_compat does not apply: its clamp belongs
+ *     to the reference's query-vs-page batching, and b200ms_mmr_device's sim has none either.
  *   page_rows_device: the true rows of the source pages back to back into out (device float32 [sum of their lengths, 128]),
  *     each element the packed value widened exactly (bf16; int8 code; e4m3 value; sign bit as +1 / -1) times scale in fp32 --
  *     the float query a first stage (b200ms_fde_encode, b200ms_sign_candidates_device) takes, with scale = 1/corpus scale for

@@ -654,7 +654,7 @@ static int ensure_clamp_pages(b200ms_t* h, cudaStream_t s, const uint32_t** out)
 // from unit_ids, page ids of v (cs.ids, or their staging-block remap for a host-resident corpus); the zero_pad_compat
 // clamp bits always come from cs.ids, the corpus page ids.
 static int candidate_plan(b200ms_t* h, const CorpusView& v, const int64_t* unit_ids, const CandSpec& cs, int n_q,
-                          cudaStream_t s, UnitPlan* plan) {
+                          bool zero_pad, cudaStream_t s, UnitPlan* plan) {
   const int n_slots = int(cs.n_slots(n_q));
   if (int e = reserve(h, h->cand_start, size_t(n_slots) * 4)) return e;
   if (int e = reserve(h, h->cand_end, size_t(n_slots) * 4)) return e;
@@ -665,7 +665,7 @@ static int candidate_plan(b200ms_t* h, const CorpusView& v, const int64_t* unit_
   plan->end = static_cast<const int32_t*>(h->cand_end.p);
   plan->n_units = n_slots;
   plan->slot_mode = 1;
-  if (h->zero_pad_batch > 0) {  // the reference's quirk, exactly: batches of zero_pad_batch candidates in first-stage order
+  if (zero_pad && h->zero_pad_batch > 0) {  // the reference's quirk, exactly: batches of zero_pad_batch candidates in first-stage order
     if (int e = reserve(h, h->clamp_slots, size_t((n_slots + 31) / 32 + 1) * 4)) return e;
     if (int e = launch_clamp_slots(h, cs.ids, cs.n_cand, cs.per_query ? n_q : 1, cs.stride(), h->zero_pad_batch,
                                    static_cast<uint32_t*>(h->clamp_slots.p), s))
@@ -703,9 +703,10 @@ static int score_wgmma_per_query(b200ms_t* h, const CorpusView& v, const UnitPla
 // Scores the rows of v.  unit_ids: the candidate slots as page ids of v (cs.ids unless v is a staging block); fill = false
 // skips the zero-fill (a later gather round of a host-resident corpus adds its slots to the same matrix).  scan (full scans
 // only): the filtered plan to walk in place of the corpus' own; the scores of the pages it leaves out are not written.
+// zero_pad = false: no zero_pad_compat clamp whatever the option says (page and example searches).
 static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int32_t* goff, int n_q, const int32_t* ntok_dev,
                       void* group_scores, int64_t ld, const CandSpec& cs, cudaStream_t s, const CorpusView& v,
-                      const int64_t* unit_ids, bool fill = true, const UnitPlan* scan = nullptr) {
+                      const int64_t* unit_ids, bool fill = true, const UnitPlan* scan = nullptr, bool zero_pad = true) {
   const Corpus& c = h->corpus;
   if (c.dtype < 0) return set_error(h, B200MS_ESTATE, "score: no corpus attached (call b200ms_set_corpus first)");
   const int64_t n_items = cs.ids ? cs.n_slots(n_q) : c.n_pages;
@@ -728,7 +729,10 @@ static int score_impl(b200ms_t* h, const void* q_packed, int n_groups, const int
   UnitPlan plan = scan ? *scan : full_scan_plan(h);
   if (!cs.ids) h->scan_planned = scan != nullptr;
   if (!b1) {
-    if (int e = cs.ids ? candidate_plan(h, v, unit_ids, cs, n_q, s, &plan) : ensure_clamp_pages(h, s, &plan.clamp_bits)) return e;
+    if (int e = cs.ids    ? candidate_plan(h, v, unit_ids, cs, n_q, zero_pad, s, &plan)
+                : zero_pad ? ensure_clamp_pages(h, s, &plan.clamp_bits)
+                           : B200MS_OK)
+      return e;
   }
   // ev0 / ev1 bracket the scoring launches only (b200ms_score_times_ms): bench.py derives the roofline's achieved figure
   // from this time
@@ -925,7 +929,7 @@ int search_scan(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
     if (full_scan)
       if (int e = plan_full_scan(h, r.allow, r.mask_index, n_q, s, &scan)) return e;
     if (int e = score_impl(h, h->q_packed.p, ng, m.goff(), n_q, ntok_dev, h->scores.p, ld, cs, s, corpus_view(h), cs.ids, true,
-                           full_scan && h->scan_planned ? &scan : nullptr))
+                           full_scan && h->scan_planned ? &scan : nullptr, !r.page_scale))
       return e;
   } else if (ng > 0 && n_items > 0) {
     struct Ctx {
@@ -937,10 +941,11 @@ int search_scan(b200ms_t* h, const SearchRequest& r, const SearchMeta& m, cudaSt
       int64_t ld;
       const CandSpec* cs;
       cudaStream_t s;
-    } ctx{h->q_packed.p, ng, m.goff(), n_q, ntok_dev, ld, &cs, s};
+      bool zero_pad;
+    } ctx{h->q_packed.p, ng, m.goff(), n_q, ntok_dev, ld, &cs, s, !r.page_scale};
     auto round = [](b200ms_t* hh, const CorpusView& v, const int64_t* unit_ids, void* scores, bool fill, void* p) {
       const Ctx& x = *static_cast<const Ctx*>(p);
-      return score_impl(hh, x.q, x.ng, x.goff, x.n_q, x.ntok, scores, x.ld, *x.cs, x.s, v, unit_ids, fill);
+      return score_impl(hh, x.q, x.ng, x.goff, x.n_q, x.ntok, scores, x.ld, *x.cs, x.s, v, unit_ids, fill, nullptr, x.zero_pad);
     };
     if (int e = score_host_tier(h, cs, n_q, gp, ld, h->scores.p, s, round, &ctx)) return e;
   }
@@ -1132,6 +1137,7 @@ static int search_pages_ordered(b200ms_t* h, const int64_t* src_host, SearchRequ
   if (int e = order.error()) return e;
   if (int e = upload(h, h->src_pages, src_host, size_t(r.n_q) * 8, s)) return e;
   r.src_pages = static_cast<const int64_t*>(h->src_pages.p);
+  r.page_scale = true;
   if (int e = search_core(h, r, build_search_meta(r.q_lens, r.n_q), s)) return e;
   return launch_normalise_pages(h, r.src_pages, r.n_q, r.k, r.top_scores, r.top_ids, r.top_counts, s);
 }
@@ -1290,6 +1296,7 @@ static int search_examples_ordered(b200ms_t* h, SearchRequest& r, const ExampleC
     r.src_pages = reinterpret_cast<const int64_t*>(md);
     r.src_first = x.n_qe;
   }
+  r.page_scale = true;
   const uint32_t* allow = x.n_masks > 0 ? x.masks : nullptr;
   const int32_t* mask_index = x.n_masks > 0 ? x.mask_index : nullptr;
   int64_t* req_lists = nullptr;

@@ -100,6 +100,8 @@ struct SearchRequest {
                                          // src_pages[q - src_first], its packed rows taken as they are stored (q_lens = the
                                          // pages' true lengths); queries before src_first are rows of q (q_dtype) as usual
   int src_first = 0;
+  bool page_scale = false;  // a page or example search: scores on b200ms_mmr_device's sim scale, so zero_pad_compat does
+                            // not apply to any of its queries
 };
 
 // What the scan part of a search (search_scan) leaves for its selection: the candidate lists it scored (cs.ids == NULL: a

@@ -5,12 +5,14 @@ Inputs are PACKED values: bf16 bit patterns (uint16) or e4m3 codes (uint8), exac
     exponents in [-266, 256]; e4m3 x e4m3 8 bits), and a product does not overflow or flush on its own (measured on an
     H100: 2^64 * 2^64 + (-2^64) * 2^64 in one MMA step is 0).  The products are summed with IEEE non-finite arithmetic
     (NaN if a NaN occurs or +inf meets -inf, else +-inf if one occurs); a finite sum is taken in float64 and rounded to
-    fp32 once: past fp32's range to +-inf, into its subnormal range as IEEE rounds, below half the least subnormal to 0.
+    fp32 once: to nearest even in fp32's normal range, past it to +-inf, and into its subnormal range (below 2^-126) toward
+    zero, to a multiple of 2^-149, as the H100's tensor core does (measured on single bf16 products: 1.0078 * 2^-150 gives
+    0, 1.5 * 2^-149 gives 2^-149, where round-to-nearest would give 2^-149 and 2^-148).
   * The max over a page's rows is fmaxf's: NaN only when every row is NaN.
   * A query's score is the IEEE sum of its true tokens' maxima, rounded to fp32; a page without rows scores 0.
   * zero_pad_compat: a clamped page's token max m becomes fmaxf(m, 0).
 The tensor core adds in fp32 in an order of its own, so a finite result may differ from this one by rounding (TOL of
-oracle/scoring.py); a single nonzero product, the probes' case, has no rounding to differ in.
+oracle/scoring.py); a single nonzero product, the probes' case, has no rounding order to differ in.
 """
 from __future__ import annotations
 
@@ -59,10 +61,16 @@ def pack_values(dtype: str, x: np.ndarray) -> np.ndarray:
     raise ValueError(dtype)
 
 
+LEAST_SUBNORMAL = 2.0 ** -149
+
+
 def fp32(x) -> np.ndarray:
-    """float64 -> the nearest fp32 (round to nearest even; past the fp32 range +-inf; subnormals as IEEE), as float64."""
-    with np.errstate(over="ignore"):
-        return np.asarray(x, dtype=np.float64).astype(np.float32).astype(np.float64)
+    """float64 -> fp32 under the value rule, as float64: round to nearest even in the normal range, +-inf past it, and
+    toward zero to a multiple of 2^-149 below 2^-126 (the tensor core's subnormal results)."""
+    x = np.asarray(x, dtype=np.float64)
+    with np.errstate(over="ignore", invalid="ignore"):
+        rn = x.astype(np.float32).astype(np.float64)
+        return np.where(np.abs(x) < 2.0 ** -126, np.trunc(x / LEAST_SUBNORMAL) * LEAST_SUBNORMAL, rn)
 
 
 def ieee_sum(terms: np.ndarray, axis: int = -1) -> np.ndarray:
