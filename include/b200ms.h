@@ -367,6 +367,47 @@ int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, int src_dtyp
                                     int64_t n_docs, float i8_q_scale, float score_scale, float* doc_page_scores,
                                     int64_t* doc_page_ids, int32_t* doc_page_counts, int32_t* doc_counts, void* stream);
 
+/* ---- documents ranked by document-level MaxSim (new; extends the document grouping above) ------------------------------
+ * DocumentService.retrieve_docs (_create_document_results, core/services/document_service.py:1759-1763) and
+ * b200ms_search_docs_device rank a document by its best page, so a query whose tokens are answered on different pages of
+ * one document scores as a partial match everywhere.  These calls score a document as one bag of patch vectors:
+ *   S(q, D) = sum over q's true tokens t of M[t, D],   M[t, D] = max over D's counted pages p of m[t, p],
+ * m[t, p] being the per-token maximum the scan computes (b200ms_explain_device's token score; 1-bit: with the token's
+ * constant).  Float maxima follow fmaxf (a NaN token max loses to any number; -0 ranks below +0), integers the integer
+ * max; B[t, D], the page holding M[t, D], is the lower page on a tie.  The M[t, D] are added exactly as a page's token
+ * maxima are (the group tree of b200ms_score, then the groups in order; I32 by the I32 sum rule), so a one-page document
+ * scores bit for bit its page's b200ms_search_device score.  A page counts when its allow bit is set (masks as
+ * b200ms_search_device_masked), its page_doc is in [0, n_docs) and it has rows; a document without a counted page is not
+ * returned, so a query may find fewer than k.  Documents are ranked in b200ms_topk's order of S (ties: lower document
+ * ordinal).  S only grows with a document's pages: long documents are favoured by definition, and nothing normalises it.
+ * zero_pad_compat does not apply.  A query without tokens finds no document.
+ * Evidence: for each returned document, its distinct pages B[t, D], each with its share (the M[t, D] it holds, added in
+ * token order), largest share first (the order of b200ms_topk's keys; ties: lower page), at most per_doc of them.  I32
+ * shares add up to S exactly, float shares within rounding.
+ * Outputs (device; unused entries -inf / -1 / 0): doc_scores float32 [n_q, k] (S * score_scale), doc_ids int64 [n_q, k]
+ * (document ordinals), page_ids int64 [n_q, k, per_doc] (page id + id_base), page_shares float32 [n_q, k, per_doc] (share *
+ * score_scale), page_counts int32 [n_q, k], doc_counts int32 [n_q].
+ * Cost: one scan of the counted pages, plus a token table of 8 B x padded query tokens x n_docs in the handle's scratch.  A
+ * batch whose table passes 1 GiB runs as several passes of whole queries; a query that alone passes it, or has more than
+ * 8192 tokens, is refused with B200MS_EINVAL.  B200MS_EINVAL also for bad arguments as b200ms_search_docs_device;
+ * B200MS_ESTATE without a corpus or for a host-resident corpus (every page of a document is read).  Nothing is launched
+ * when a call is refused.  Asynchronous on cuda_stream, in the handle's call order (a call on another stream waits
+ * for the handle's previous call). */
+/* full scan */
+int b200ms_search_doc_maxsim_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q, int k,
+                                    int per_doc, const int32_t* page_doc, int64_t n_docs, const uint32_t* allow_masks_dev,
+                                    int n_masks, const int32_t* mask_index_dev, float i8_q_scale, float score_scale,
+                                    int64_t id_base, float* doc_scores, int64_t* doc_ids, int64_t* page_ids,
+                                    float* page_shares, int32_t* page_counts, int32_t* doc_counts, void* cuda_stream);
+/* two-stage: cand_ids_dev int64 [n_q, n_cand] (-1 = unused slot) are query q's first-stage pages; q is scored over every
+ * counted page of their documents (the masks still apply) */
+int b200ms_rerank_doc_maxsim_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
+                                          const int64_t* cand_ids_dev, int n_cand, int k, int per_doc, const int32_t* page_doc,
+                                          int64_t n_docs, const uint32_t* allow_masks_dev, int n_masks,
+                                          const int32_t* mask_index_dev, float i8_q_scale, float score_scale, int64_t id_base,
+                                          float* doc_scores, int64_t* doc_ids, int64_t* page_ids, float* page_shares,
+                                          int32_t* page_counts, int32_t* doc_counts, void* cuda_stream);
+
 /* ---- diversifying results (new; no reference counterpart) ---------------------------------------------------------------
  * Maximal marginal relevance (MMR) over each query's candidate list: near-copies of a page picked already (a re-uploaded
  * deck, a repeated slide template, the same figure on two pages) give way to pages that add something.  The call needs no

@@ -137,6 +137,10 @@ _SIGNATURES = {
     "b200ms_rerank_examples_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, i64p, c_int, i32p, f32p, c_int, vp, c_int, c_int,
                                                     vp, c_int, vp, c_float, c_float, vp, vp, vp, vp]),
     "b200ms_union_candidates_device": (c_int, [vp, vp, c_int, c_int, i32p, c_int, vp, c_int, vp]),
+    "b200ms_search_doc_maxsim_device": (c_int, [vp, vp, c_int, i32p, c_int, c_int, c_int, vp, c_int64, vp, c_int, vp, c_float,
+                                                c_float, c_int64, vp, vp, vp, vp, vp, vp, vp]),
+    "b200ms_rerank_doc_maxsim_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, vp,
+                                                      c_int, vp, c_float, c_float, c_int64, vp, vp, vp, vp, vp, vp, vp]),
 }
 
 

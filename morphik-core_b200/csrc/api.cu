@@ -320,7 +320,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
                        &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
                        &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials, &h->src_pages,
-                       &h->ex_meta, &h->ex_lists, &h->ex_fused, &h->ex_union};
+                       &h->ex_meta, &h->ex_lists, &h->ex_fused, &h->ex_union, &h->dm_table, &h->dm_scores, &h->dm_allow};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   release_blocks(h);
@@ -1107,6 +1107,43 @@ B200MS_API int b200ms_rerank_docs_batch_device(b200ms_t* h, const void* q_dev, i
   const DocSpec d{page_doc, n_docs, per_doc, doc_page_scores, doc_page_ids, doc_page_counts, doc_counts};
   r.docs = &d;
   return search_ordered(h, r, static_cast<cudaStream_t>(stream));
+}
+
+// ---- documents ranked by document-level MaxSim
+static int doc_maxsim_ordered(b200ms_t* h, const bms::DocMaxSimCall& x, int src_dtype, cudaStream_t s) {
+  if (!h) return B200MS_EINVAL;
+  if (!src_dtype_ok(src_dtype)) return set_error(h, B200MS_EINVAL, "doc_maxsim: src dtype must be F32 or BF16");
+  DeviceGuard g(h->device);
+  StreamOrder order(h, s);
+  if (int e = order.error()) return e;
+  return doc_maxsim(h, x, s);
+}
+
+B200MS_API int b200ms_search_doc_maxsim_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens, int n_q,
+                                               int k, int per_doc, const int32_t* page_doc, int64_t n_docs,
+                                               const uint32_t* allow_masks_dev, int n_masks, const int32_t* mask_index_dev,
+                                               float i8_q_scale, float score_scale, int64_t id_base, float* doc_scores,
+                                               int64_t* doc_ids, int64_t* page_ids, float* page_shares,
+                                               int32_t* page_counts, int32_t* doc_counts, void* cuda_stream) {
+  bms::DocMaxSimCall x{q_dev, src_dtype, q_lens, n_q, k, per_doc, page_doc, n_docs, allow_masks_dev, n_masks, mask_index_dev,
+                       nullptr, 0, i8_q_scale, score_scale, id_base, doc_scores, doc_ids, page_shares, page_ids, page_counts,
+                       doc_counts};
+  return doc_maxsim_ordered(h, x, src_dtype, static_cast<cudaStream_t>(cuda_stream));
+}
+
+B200MS_API int b200ms_rerank_doc_maxsim_batch_device(b200ms_t* h, const void* q_dev, int src_dtype, const int32_t* q_lens,
+                                                     int n_q, const int64_t* cand_ids_dev, int n_cand, int k, int per_doc,
+                                                     const int32_t* page_doc, int64_t n_docs, const uint32_t* allow_masks_dev,
+                                                     int n_masks, const int32_t* mask_index_dev, float i8_q_scale,
+                                                     float score_scale, int64_t id_base, float* doc_scores, int64_t* doc_ids,
+                                                     int64_t* page_ids, float* page_shares, int32_t* page_counts,
+                                                     int32_t* doc_counts, void* cuda_stream) {
+  if (h && !cand_ids_dev)
+    return set_error(h, B200MS_EINVAL, "rerank_doc_maxsim_batch_device: bad arguments (candidate lists [n_q, n_cand >= 1])");
+  bms::DocMaxSimCall x{q_dev, src_dtype, q_lens, n_q, k, per_doc, page_doc, n_docs, allow_masks_dev, n_masks, mask_index_dev,
+                       cand_ids_dev, n_cand, i8_q_scale, score_scale, id_base, doc_scores, doc_ids, page_shares, page_ids,
+                       page_counts, doc_counts};
+  return doc_maxsim_ordered(h, x, src_dtype, static_cast<cudaStream_t>(cuda_stream));
 }
 
 // ---- searching with stored pages as the queries

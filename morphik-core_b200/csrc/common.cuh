@@ -79,6 +79,50 @@ struct DocSpec {
   int32_t* doc_counts = nullptr;
 };
 
+// Document mode of the wgmma scan (doc_maxsim.cu): instead of group scores, every true token row t (32 * group + token) of
+// the call keeps table[t, d] = max over the scanned pages p of document d of (token max key << 32 | ~p).  A page counts
+// when page_doc[p] is in [0, n_docs) and allow (NULL = all; else row mask_index[group_query[group]], -1 = all, rows
+// mask_stride words apart) has its bit.
+struct DocScan {
+  unsigned long long* table = nullptr;
+  int64_t n_docs = 0;
+  const int32_t* page_doc = nullptr;
+  const int32_t* group_query = nullptr;
+  const uint32_t* allow = nullptr;
+  const int32_t* mask_index = nullptr;
+  int64_t mask_stride = 0;
+};
+
+// A document-level MaxSim call (doc_maxsim.cu).  q / q_lens / masks as SearchRequest (n_masks rows; mask_index per query);
+// cand != NULL: per-query candidate page lists [n_q, n_cand] whose documents are scored.  Outputs (device): doc_scores /
+// doc_ids [n_q, k], ev_scores / ev_ids [n_q, k, per_doc], ev_counts [n_q, k], doc_counts [n_q].
+struct DocMaxSimCall {
+  const void* q = nullptr;
+  int q_dtype = B200MS_F32;
+  const int32_t* q_lens = nullptr;  // HOST
+  int n_q = 0, k = 0, per_doc = 1;
+  const int32_t* page_doc = nullptr;
+  int64_t n_docs = 0;
+  const uint32_t* allow = nullptr;
+  int n_masks = 0;
+  const int32_t* mask_index = nullptr;
+  const int64_t* cand = nullptr;
+  int n_cand = 0;
+  float i8_q_scale = 1.f, score_scale = 1.f;
+  int64_t id_base = 0;
+  float* doc_scores = nullptr;
+  int64_t* doc_ids = nullptr;
+  float* ev_scores = nullptr;
+  int64_t* ev_ids = nullptr;
+  int32_t* ev_counts = nullptr;
+  int32_t* doc_counts = nullptr;
+};
+// Largest token table (8 B x padded query tokens x n_docs) one pass of a document-level call builds, and the longest query
+// it takes (the evidence kernel holds a query's token maxima in shared memory)
+constexpr int64_t kDocTableBytes = int64_t(1) << 30;
+constexpr int kDocMaxTokens = 8192;
+int doc_maxsim(b200ms_t* h, const DocMaxSimCall& x, cudaStream_t s);
+
 // One search: pack queries -> score -> top-k.  Device pointers, except that q and the outputs may be mapped pinned memory.
 struct SearchRequest {
   const void* q = nullptr;  // rows [sum q_lens,128] of q_dtype (F32 | BF16)
@@ -282,6 +326,9 @@ struct b200ms {
   // relevance feedback (search_examples.cu): the call's example table, the requests' and examples' candidate lists (or the
   // examples' mask rows), the fused score rows, and the hash tables of a candidate union
   bms::DeviceBuf ex_meta, ex_lists, ex_fused, ex_union;
+  // document-level MaxSim (doc_maxsim.cu): the token table, the document scores and found mask, the candidate calls'
+  // document marks and allow rows
+  bms::DeviceBuf dm_table, dm_scores, dm_allow;
 };
 
 namespace bms {
@@ -381,9 +428,10 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
 
 // kernel launchers (each returns a b200ms error code and bumps h->launches)
 // group_ntok (device, [n_groups_real] or NULL = 32 each): the true tokens of every group; a padding token adds +0
+// doc != NULL: document mode (DocScan) -- group_scores and plan.clamp_bits are not used, plan.slot_mode must be 0
 int launch_score_wgmma(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const void* q_packed, int n_groups_real,
                        const int32_t* group_ntok, void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo = 0,
-                       int m_tile_hi = -1);
+                       int m_tile_hi = -1, const DocScan* doc = nullptr);
 // scan != NULL (full scans, cand_ids == NULL): only the pages scan->pages lists, scores still indexed by page id
 int launch_score_b1(b200ms_t* h, const CorpusView& v, const int64_t* cand_ids, int64_t n_cand, const void* q_packed,
                     int n_groups, const int32_t* group_ntok_dev, void* group_scores, int64_t ld, cudaStream_t s, int g_lo,
@@ -392,14 +440,15 @@ int launch_pad_cands(b200ms_t* h, const int64_t* src, int n_cand, int n_lists, i
 int launch_clamp_slots(b200ms_t* h, const int64_t* cand_ids, int n_cand, int n_lists, int64_t list_stride, int batch,
                        uint32_t* clamp_bits, cudaStream_t s);
 int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
-                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s);
+                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s, const DocScan* doc = nullptr);
 // The A operand of the 1-bit wgmma scan: int8 rows q_i8 [n_rows,128] (1024-byte aligned) and one int32 constant per row,
 // in the handle's scratch
 int reserve_b1_query(b200ms_t* h, int64_t n_rows, int8_t** q_i8, int32_t** tok_const);
 // The 1-bit wgmma scan of the sign rows of v (v.rows: 16 B per row) for prepared A rows: group_scores[g, p] = sum over the
 // group's rows t of (tok_const[t] + max over the page's rows r of <q_i8[t], bits(r) as {0,1}>)
 int launch_b1_tiles(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const int8_t* q_i8, const int32_t* tok_const,
-                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s);
+                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s, const int32_t* group_ntok = nullptr,
+                    const DocScan* doc = nullptr);
 // Corpus tables a full scan needs (unit_start, chunk_page, scan-plan scratch), enqueued on s; c.n_units is set
 int build_scan_tables(b200ms_t* h, Corpus& c, const int64_t* ps_host, cudaStream_t s);
 // Scratch of launch_scan_plan for the corpus c (set_corpus reserves it, so that no search grows it)

@@ -32,6 +32,7 @@
 #include "common.cuh"
 #include "mma_tile.cuh"
 #include "ptx.cuh"
+#include "topk_keys.cuh"
 
 namespace bms {
 
@@ -141,17 +142,25 @@ f8_query_widen_kernel(const uint2* __restrict__ q, int64_t n_words, uint4* __res
   }
 }
 
+// Document mode (DOC): a page's per-token maxima m go to the document table instead of a group score.  Each true token t
+// of the group takes atomicMax(table[32 * group + t, doc], doc_token_key(m) << 32 | ~page) when the page's document is in
+// [0, n_docs) and the group's query may see the page; the key orders numbers like key_of and puts NaN between "unset" (0)
+// and every number, as fmaxf lets any number beat NaN, and a tie goes to the lower page.  The atomics commute, so the table
+// does not depend on the order the CTAs reach the pages.
+__device__ __forceinline__ uint32_t doc_token_key(float m) { return m != m ? 1u : key_of(m); }
+__device__ __forceinline__ uint32_t doc_token_key(int m) { return key_of(m); }  // m > INT32_MIN: the key is never 0
+
 // KIND 0 bf16, 1 int8 (BITS: 1-bit corpus expanded to int8), 2 fp8 e4m3 (widened to f16 by the producer warpgroup);
-// NM = resident query tiles (1, 2, 4 or 8).
-template <int KIND, int NM, bool BITS>
-__global__ void __launch_bounds__(kThreads, 1)
-maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_constant__ CUtensorMap tmap_q,
-                    const uint4* __restrict__ bit_rows, int64_t n_rows, const int32_t* __restrict__ tok_const,
-                    const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start,
-                    const int32_t* __restrict__ unit_end, int slot_mode, int n_units,
-                    const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,
-                    const int32_t* __restrict__ group_ntok, const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
-                    int num_stages, int splits) {
+// NM = resident query tiles (1, 2, 4 or 8).  The body of maxsim_wgmma_kernel (DOC = false) and maxsim_wgmma_doc_kernel.
+template <int KIND, int NM, bool BITS, bool DOC>
+__device__ __forceinline__ void
+maxsim_wgmma_body(const CUtensorMap& tmap_rows, const CUtensorMap& tmap_q,
+                  const uint4* __restrict__ bit_rows, int64_t n_rows, const int32_t* __restrict__ tok_const,
+                  const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start,
+                  const int32_t* __restrict__ unit_end, int slot_mode, int n_units,
+                  const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,
+                  const int32_t* __restrict__ group_ntok, const uint32_t* __restrict__ clamp_bits, typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld,
+                  int num_stages, int splits, const DocScan& doc) {
   using K = Kind<KIND>;
   using Acc = typename K::Acc;
   static_assert(!BITS || KIND == 1, "1-bit corpora run on the int8 MMA");
@@ -369,18 +378,41 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
     if (group < n_groups_real && page >= 0) {
       const int o = slot_mode ? u : page;
       const int ntok = group_ntok ? __ldg(group_ntok + group) : kGroup;
-      Acc v[4];
+      if constexpr (DOC) {
+        // the page's document and whether the group's query may see the page; then one atomic per true token, from the
+        // quad's first lane.  A 1-bit token's constant c_t is left out: it moves neither the max nor the arg-max, and
+        // doc_maxsim.cu adds it when it reads the table.
+        const int d = __ldg(doc.page_doc + page);
+        bool ok = d >= 0 && d < doc.n_docs;
+        if (ok && doc.allow) {
+          const int mi = doc.mask_index ? __ldg(doc.mask_index + __ldg(doc.group_query + group)) : 0;
+          ok = mi < 0 || ((__ldg(doc.allow + int64_t(mi) * doc.mask_stride + (page >> 5)) >> (page & 31)) & 1u);
+        }
+        // 32-bit entry index: a table holds at most kDocTableBytes / 8 = 2^27 entries
+        const uint32_t nd = uint32_t(doc.n_docs);
+        const uint32_t row = uint32_t(group * kGroup + (lane >> 2)) * nd + uint32_t(d);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        Acc cnst = Acc(0);
-        // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w; read here, not held in registers
-        const int tok = 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2);
-        if constexpr (BITS) cnst = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + tok);
-        const Acc m = clamp_token_max(clamp_bits, o, quad_max(runmax[i][k])) + cnst;
-        v[k] = tok < ntok ? m : Acc(0);
+        for (int k = 0; k < 4; ++k) {
+          const int tok = 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2);
+          const Acc m = quad_max(runmax[i][k]);
+          if (ok && (lane & 3) == 0 && tok < ntok)
+            atomicMax(doc.table + (row + uint32_t(tok - (lane >> 2)) * nd),
+                      (uint64_t(doc_token_key(m)) << 32) | uint64_t(~uint32_t(page)));
+        }
+      } else {
+        Acc v[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          Acc cnst = Acc(0);
+          // token k of this thread: 16 * (k >> 1) + 8 * (k & 1) + lane / 4 of group w; read here, not held in registers
+          const int tok = 16 * (k >> 1) + 8 * (k & 1) + (lane >> 2);
+          if constexpr (BITS) cnst = __ldg(tok_const + int64_t(mt) * kTileM + 32 * w + tok);
+          const Acc m = clamp_token_max(clamp_bits, o, quad_max(runmax[i][k])) + cnst;
+          v[k] = tok < ntok ? m : Acc(0);
+        }
+        const Acc s = group_sum(v);
+        if (lane == 0) group_scores[int64_t(group) * ld + o] = s;
       }
-      const Acc s = group_sum(v);
-      if (lane == 0) group_scores[int64_t(group) * ld + o] = s;
     }
   };
 
@@ -486,6 +518,28 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
   for (int i = 0; i < MPW; ++i) flush(i, last_u, cur_page);
 }
 
+#define MAXSIM_WGMMA_PARAMS                                                                                                  \
+  const __grid_constant__ CUtensorMap tmap_rows, const __grid_constant__ CUtensorMap tmap_q,                              \
+      const uint4* __restrict__ bit_rows, int64_t n_rows, const int32_t* __restrict__ tok_const,                             \
+      const int32_t* __restrict__ chunk_page, const int32_t* __restrict__ unit_start, const int32_t* __restrict__ unit_end, \
+      int slot_mode, int n_units, const int32_t* __restrict__ n_units_dev, int m_tile_base, int n_groups_real,              \
+      const int32_t* __restrict__ group_ntok, const uint32_t* __restrict__ clamp_bits,                                     \
+      typename Kind<KIND>::Acc* __restrict__ group_scores, int64_t ld, int num_stages, int splits
+#define MAXSIM_WGMMA_ARGS                                                                                                   \
+  tmap_rows, tmap_q, bit_rows, n_rows, tok_const, chunk_page, unit_start, unit_end, slot_mode, n_units, n_units_dev,      \
+      m_tile_base, n_groups_real, group_ntok, clamp_bits, group_scores, ld, num_stages, splits
+
+template <int KIND, int NM, bool BITS>
+__global__ void __launch_bounds__(kThreads, 1) maxsim_wgmma_kernel(MAXSIM_WGMMA_PARAMS) {
+  maxsim_wgmma_body<KIND, NM, BITS, false>(MAXSIM_WGMMA_ARGS, DocScan{});
+}
+
+// document mode: no group_scores (NULL), no clamp (clamp_bits NULL), full-scan units (slot_mode 0)
+template <int KIND, int NM, bool BITS>
+__global__ void __launch_bounds__(kThreads, 1) maxsim_wgmma_doc_kernel(MAXSIM_WGMMA_PARAMS, const DocScan doc) {
+  maxsim_wgmma_body<KIND, NM, BITS, true>(MAXSIM_WGMMA_ARGS, doc);
+}
+
 // ---------------------------------------------------------------------------------------------- host side
 // Query tiles [m_tile_base, m_tile_base + splits * NM) in one launch.  splits = 2: CTAs 2k and 2k + 1 walk the same units,
 // CTA 2k with the first NM tiles and CTA 2k + 1 with the next NM, so the pair reads every patch tile from HBM once and
@@ -493,25 +547,30 @@ maxsim_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid_
 template <int KIND, int NM, bool BITS>
 static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
                       const int32_t* group_ntok, int m_tile_base, int n_groups_real, void* scores, int64_t ld, cudaStream_t s,
-                      int splits = 1) {
+                      const DocScan* doc, int splits = 1) {
   using K = Kind<KIND>;
   const uint32_t avail = kSmemLimit - 1024 /*align*/ - kBarrierBytes - NM * K::kTileBytes;
   int stages = int(avail / K::kTileBytes);
   if (stages > 8) stages = 8;
   if (stages < 2) return set_error(h, B200MS_EINVAL, "maxsim_wgmma: not enough shared memory for 2 stages");
   const uint32_t smem = 1024 + NM * K::kTileBytes + uint32_t(stages) * K::kTileBytes + kBarrierBytes;
-  auto kern = maxsim_wgmma_kernel<KIND, NM, BITS>;
-  if (int e = ensure_smem(h, reinterpret_cast<const void*>(kern), int(smem), "cudaFuncSetAttribute(maxsim_wgmma)"))
-    return e;
+  const void* fn = doc ? reinterpret_cast<const void*>(maxsim_wgmma_doc_kernel<KIND, NM, BITS>)
+                       : reinterpret_cast<const void*>(maxsim_wgmma_kernel<KIND, NM, BITS>);
+  if (int e = ensure_smem(h, fn, int(smem), "cudaFuncSetAttribute(maxsim_wgmma)")) return e;
   int grid = h->max_ctas > 0 ? h->max_ctas : h->num_sms;
   if (grid > splits * up.n_units) grid = splits * up.n_units;  // with n_units_dev an upper bound: the count is not known here
   grid -= grid % splits;
   if (grid < 1) return B200MS_OK;
   static const CUtensorMap kNoTmap{};  // 1-bit rows: the producer expands bits and never issues TMA loads for them
-  kern<<<grid, kThreads, smem, s>>>(c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const,
-                                   c.chunk_page, up.start, up.end, up.slot_mode, up.n_units, up.n_units_dev,
-                                   m_tile_base, n_groups_real, group_ntok, up.clamp_bits, static_cast<typename K::Acc*>(scores), ld,
-                                   stages, splits);
+  if (doc)
+    maxsim_wgmma_doc_kernel<KIND, NM, BITS><<<grid, kThreads, smem, s>>>(
+        c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const, c.chunk_page, up.start, up.end,
+        0, up.n_units, up.n_units_dev, m_tile_base, n_groups_real, group_ntok, nullptr, nullptr, 0, stages, splits, *doc);
+  else
+    maxsim_wgmma_kernel<KIND, NM, BITS><<<grid, kThreads, smem, s>>>(
+        c.tmap ? *c.tmap : kNoTmap, tq, static_cast<const uint4*>(c.rows), c.n_rows, tok_const, c.chunk_page, up.start, up.end,
+        up.slot_mode, up.n_units, up.n_units_dev, m_tile_base, n_groups_real, group_ntok, up.clamp_bits,
+        static_cast<typename K::Acc*>(scores), ld, stages, splits);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch maxsim_wgmma");
 }
@@ -521,13 +580,14 @@ static int launch_one(b200ms_t* h, const CorpusView& c, const UnitPlan& up, cons
 // the grid holds a pair of CTAs.
 template <int KIND, bool BITS>
 static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const CUtensorMap& tq, const int32_t* tok_const,
-                        const int32_t* group_ntok, int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s) {
+                        const int32_t* group_ntok, int n_groups_real, int m_lo, int m_hi, void* scores, int64_t ld, cudaStream_t s,
+                        const DocScan* doc = nullptr) {
   constexpr int kMaxNM = Kind<KIND>::kMaxNM;
   const bool pairs = (h->max_ctas > 0 ? h->max_ctas : h->num_sms) >= 2;
   for (int base = m_lo; base < m_hi;) {
     const int rem = m_hi - base;
     if (pairs && rem >= 2 * kMaxNM) {
-      if (int e = launch_one<KIND, kMaxNM, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, 2)) return e;
+      if (int e = launch_one<KIND, kMaxNM, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, doc, 2)) return e;
       base += 2 * kMaxNM;
       continue;
     }
@@ -535,12 +595,12 @@ static int launch_tiles(b200ms_t* h, const CorpusView& c, const UnitPlan& up, co
     while (nm < rem && nm < kMaxNM) nm <<= 1;
     int e;
     switch (nm) {
-      case 1: e = launch_one<KIND, 1, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
-      case 2: e = launch_one<KIND, 2, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
-      case 4: e = launch_one<KIND, 4, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s); break;
+      case 1: e = launch_one<KIND, 1, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, doc); break;
+      case 2: e = launch_one<KIND, 2, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, doc); break;
+      case 4: e = launch_one<KIND, 4, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, doc); break;
       default:
         if constexpr (kMaxNM >= 8) {
-          e = launch_one<KIND, 8, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s);
+          e = launch_one<KIND, 8, BITS>(h, c, up, tq, tok_const, group_ntok, base, n_groups_real, scores, ld, s, doc);
         } else {
           e = set_error(h, B200MS_EINVAL, "maxsim_wgmma: bad NM");
         }
@@ -564,7 +624,8 @@ static int query_tmap(b200ms_t* h, const void* q, int dtype, int n_q_rows) {
 // m_tile_lo / m_tile_hi: score only query tiles [m_tile_lo, m_tile_hi) (hi < 0: all) -- the batched rerank walks the query
 // tiles one launch at a time, each against its own candidate units.
 int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, const void* q_packed, int n_groups_real,
-                       const int32_t* group_ntok, void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi) {
+                       const int32_t* group_ntok, void* group_scores, int64_t ld, cudaStream_t s, int m_tile_lo, int m_tile_hi,
+                       const DocScan* doc) {
   if (!c.tmap) return set_error(h, B200MS_ESTATE, "score: corpus has no TMA descriptor");
   const int n_groups_padded = int(groups_padded(n_groups_real));
   const int n_mtiles = n_groups_padded / 4;
@@ -587,9 +648,9 @@ int launch_score_wgmma(b200ms_t* h, const CorpusView& c, const UnitPlan& up, con
     hi = m_tile_hi < n_mtiles ? m_tile_hi : n_mtiles;
   }
   switch (kind_of_dtype(c.dtype)) {
-    case 0: return launch_tiles<0, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
-    case 1: return launch_tiles<1, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
-    case 2: return launch_tiles<2, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s);
+    case 0: return launch_tiles<0, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s, doc);
+    case 1: return launch_tiles<1, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s, doc);
+    case 2: return launch_tiles<2, false>(h, c, up, h->tmap_q, nullptr, group_ntok, n_groups_real, lo, hi, group_scores, ld, s, doc);
     default: return set_error(h, B200MS_ESTATE, "score: corpus dtype has no wgmma scorer");
   }
 }
@@ -603,16 +664,18 @@ int reserve_b1_query(b200ms_t* h, int64_t n_rows, int8_t** q_i8, int32_t** tok_c
 }
 
 int launch_b1_tiles(b200ms_t* h, const CorpusView& v, const UnitPlan& plan, const int8_t* q_i8, const int32_t* tok_const,
-                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
+                    int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s, const int32_t* group_ntok,
+                    const DocScan* doc) {
   const int n_groups_padded = int(groups_padded(n_groups_real));
   if (int e = query_tmap(h, q_i8, B200MS_I8, n_groups_padded * kGroup)) return e;
-  return launch_tiles<1, true>(h, v, plan, h->tmap_q, tok_const, nullptr, n_groups_real, 0, n_groups_padded / 4, group_scores, ld, s);
+  return launch_tiles<1, true>(h, v, plan, h->tmap_q, tok_const, group_ntok, n_groups_real, 0, n_groups_padded / 4, group_scores,
+                               ld, s, doc);
 }
 
 // 1-bit full scan: the query bits become +-1 int8 rows (b1_q_i8) and per-token constants, then the int8 kernel with the
 // expanding producer.
 int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits, const int32_t* group_ntok_dev,
-                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s) {
+                          int n_groups_real, void* group_scores, int64_t ld, cudaStream_t s, const DocScan* doc) {
   const int n_rows = int(groups_padded(n_groups_real)) * kGroup;
   int8_t* q_i8 = nullptr;
   int32_t* tok_const = nullptr;
@@ -621,7 +684,8 @@ int launch_score_b1_wgmma(b200ms_t* h, const UnitPlan& plan, const void* q_bits,
                                                                   q_i8, tok_const);
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch b1_query_expand")) return e;
-  return launch_b1_tiles(h, corpus_view(h), plan, q_i8, tok_const, n_groups_real, group_scores, ld, s);
+  return launch_b1_tiles(h, corpus_view(h), plan, q_i8, tok_const, n_groups_real, group_scores, ld, s,
+                         doc ? group_ntok_dev : nullptr, doc);
 }
 
 }  // namespace bms

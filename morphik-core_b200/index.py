@@ -1067,6 +1067,77 @@ class MaxSimIndex:
                 "b200ms_rerank_docs_batch_device")
         return ts, ti, pc, dc
 
+    # ------------------------------------------------------------------ documents as one bag of patches
+    def _doc_maxsim_args(self, q_dev, q_lens, k, per_doc, page_doc_dev, allow_mask_dev, mask_index_dev):
+        if self.tier == "host":
+            raise ValueError("document-level MaxSim reads every page of a document: it needs an HBM-tier index")
+        n_q = len(q_lens)
+        q_dtype = _check_queries(q_dev, q_lens, self.device)
+        self._check_docs_args(per_doc, page_doc_dev)
+        masks, n_masks, index = _check_device_masks(allow_mask_dev, mask_index_dev, n_q, self.n_pages, self.device)
+        if masks is not None and index is None:  # one mask for every query: a one-row matrix
+            index = torch.zeros((n_q,), dtype=torch.int32, device=self.device)
+        ds, di, dc = _topk_outputs(n_q, int(k), self.device)
+        es, ei, ec, _ = _topk_outputs(n_q, int(k), self.device, per_doc=int(per_doc))
+        return q_dtype, masks, n_masks, index, (ds, di, ei, es, ec, dc)
+
+    def search_doc_maxsim_device(self, q_dev: torch.Tensor, q_lens: Sequence[int], k: int, per_doc: int,
+                                 page_doc_dev: torch.Tensor, n_docs: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                                 mask_index_dev: Optional[torch.Tensor] = None, id_base: int = 0):
+        """The top k documents by document-level MaxSim (b200ms_search_doc_maxsim_device), asynchronous on torch's current
+        stream: a document scores sum over the query's tokens of each token's best patch on ANY of its pages, so a query
+        answered by several pages of one document ranks that document as one match.  Long documents are favoured (the
+        score only grows with pages); nothing normalises it.
+
+        page_doc_dev / masks as search_docs_device.  Returns device tensors: document scores float32 [n_q,k], document
+        ordinals int64 [n_q,k], evidence page ids + id_base int64 [n_q,k,per_doc], evidence shares float32 [n_q,k,per_doc]
+        (the token maxima each page holds; largest first), evidence pages int32 [n_q,k], documents found int32 [n_q];
+        unused entries are -inf / -1 / 0.  An HBM-tier index only (ValueError on the host tier)."""
+        q_dtype, masks, n_masks, index, out = self._doc_maxsim_args(q_dev, q_lens, k, per_doc, page_doc_dev, allow_mask_dev,
+                                                                    mask_index_dev)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_search_doc_maxsim_device(
+                    self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), len(q_lens), int(k), int(per_doc),
+                    _vp(page_doc_dev), int(n_docs), _vp(masks), n_masks, _vp(index), ctypes.c_float(self.i8_scale),
+                    ctypes.c_float(self.score_scale), int(id_base), *[_vp(t) for t in out], self._stream()),
+                "b200ms_search_doc_maxsim_device")
+        ds, di, ei, es, ec, dc = out
+        return ds, di, ei, es, ec, dc
+
+    def search_doc_maxsim(self, queries: Sequence[ArrayLike], k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                          allow_mask: Optional[np.ndarray] = None):
+        """search_doc_maxsim_device from host query matrices and an optional host allow mask (uint32 words); synchronous,
+        returns host arrays."""
+        lens = self._q_lens(queries)
+        src, _ = self._stage_rows(list(queries))
+        mask_dev = _host_mask_to_device(allow_mask, self.n_pages, self.device)
+        out = self.search_doc_maxsim_device(src, lens, k, per_doc, page_doc_dev, n_docs, allow_mask_dev=mask_dev)
+        return tuple(t.cpu().numpy() for t in out)
+
+    def rerank_doc_maxsim_batch(self, q_dev: torch.Tensor, q_lens: Sequence[int], cand_ids: torch.Tensor, k: int,
+                                per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                                allow_mask_dev: Optional[torch.Tensor] = None, mask_index_dev: Optional[torch.Tensor] = None,
+                                id_base: int = 0):
+        """search_doc_maxsim_device over the documents of each query's own first-stage pages, cand_ids int64 [n_q, n_cand]
+        (-1 = unused slot; b200ms_rerank_doc_maxsim_batch_device): every allowed page of those documents is scored, not only
+        the candidates.  Outputs as search_doc_maxsim_device."""
+        _check_candidates(cand_ids, len(q_lens), k, self.device, per_query=True)
+        q_dtype, masks, n_masks, index, out = self._doc_maxsim_args(q_dev, q_lens, k, per_doc, page_doc_dev, allow_mask_dev,
+                                                                    mask_index_dev)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(
+                nat.lib.b200ms_rerank_doc_maxsim_batch_device(
+                    self.h.ptr, _vp(q_dev), q_dtype, nat.i32_array(q_lens), len(q_lens), _vp(cand_ids),
+                    int(cand_ids.shape[1]), int(k), int(per_doc), _vp(page_doc_dev), int(n_docs), _vp(masks), n_masks,
+                    _vp(index), ctypes.c_float(self.i8_scale), ctypes.c_float(self.score_scale), int(id_base),
+                    *[_vp(t) for t in out], self._stream()),
+                "b200ms_rerank_doc_maxsim_batch_device")
+        ds, di, ei, es, ec, dc = out
+        return ds, di, ei, es, ec, dc
+
     # ------------------------------------------------------------------ explaining a match
     def explain(self, queries: Sequence[ArrayLike], page_ids, map_rows: int = 0):
         """Why pages matched: per query token, the best patch row of each named page and its similarity, computed with the

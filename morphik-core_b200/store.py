@@ -39,6 +39,8 @@ from .models import DocumentChunk
 
 logger = logging.getLogger(__name__)
 MAX_K = 4096  # B200MS_MAX_K
+# metadata key of the document score on the chunks query_similar_documents(score_by="document") returns
+DOCUMENT_SCORE_KEY = "document_score"
 
 try:  # inside a Morphik checkout the reference ABC is the real base class
     from core.vector_store.base_vector_store import BaseVectorStore  # type: ignore
@@ -410,23 +412,43 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
     async def query_similar_documents(self, query_embedding, k: int, pages_per_document: int = 1,
                                       doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None,
-                                      min_score: Optional[float] = None) -> List[List[DocumentChunk]]:
-        """The top k DOCUMENTS instead of the top k chunks (extension): one list per document, best document first, each
-        holding that document's best ``pages_per_document`` chunks in score order.  A document ranks by its best chunk and
-        scores are query_similar's, so this is query_similar's ranking grouped by document, computed on the GPU without
-        over-fetching chunks.  ``doc_ids`` / ``app_id`` filter as in query_similar; ``min_score`` drops chunks below it and
-        a document left without chunks.  Mask, GPU search and chunk construction are one critical section."""
+                                      min_score: Optional[float] = None, score_by: str = "page") -> List[List[DocumentChunk]]:
+        """The top k DOCUMENTS instead of the top k chunks (extension): one list per document, best document first.
+
+        ``score_by="page"`` (default): a document ranks by its best chunk, and each list holds that document's best
+        ``pages_per_document`` chunks in score order with query_similar's scores -- query_similar's ranking grouped by
+        document, computed on the GPU without over-fetching chunks.  ``min_score`` drops chunks below it and a document
+        left without chunks.
+
+        ``score_by="document"``: a document is scored as one bag of patches, each query token taking its best patch on ANY
+        of the document's pages (document-level MaxSim), so a document that answers different parts of the query on
+        different pages ranks as one match.  Longer documents are favoured: the score only grows with pages, and nothing
+        normalises it.  Each list holds the document's evidence chunks -- the pages holding some token's best patch, at most
+        ``pages_per_document``, largest share first -- and a chunk's ``score`` is its share (the token maxima it holds);
+        the document's score is in every chunk's ``metadata["document_score"]``.  ``min_score`` drops documents whose
+        score is below it.  Needs an HBM-tier index.
+
+        ``doc_ids`` / ``app_id`` filter as in query_similar.  Mask, GPU search and chunk construction are one critical
+        section."""
         q = as_query_matrix(query_embedding)
         per = int(pages_per_document)
         if not 1 <= per <= 64:
             raise ValueError("pages_per_document must be in [1, 64]")
+        if score_by not in ("page", "document"):
+            raise ValueError(f"score_by must be 'page' or 'document', got {score_by!r}")
         if k <= 0:
             return []
-        return await asyncio.to_thread(self._search_docs_locked, q, int(k), per, doc_ids, app_id, min_score)
+        return await asyncio.to_thread(self._search_docs_locked, q, int(k), per, doc_ids, app_id, min_score, score_by)
 
-    def _search_docs_locked(self, q, k, per, doc_ids, app_id, min_score):
+    def _page_doc_table(self):
         import torch
 
+        if self._page_doc_cache is None or self._page_doc_cache[0] != self.catalog.version:
+            table = torch.from_numpy(self.catalog.page_documents()).to(self._index.device)
+            self._page_doc_cache = (self.catalog.version, table)
+        return self._page_doc_cache[1]
+
+    def _search_docs_locked(self, q, k, per, doc_ids, app_id, min_score, score_by="page"):
         with self._lock:
             n = len(self.catalog)
             if n == 0:
@@ -436,10 +458,9 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 return []
             n_docs = self.catalog.n_documents
             kk = min(_capped_k(k), n_docs)
-            if self._page_doc_cache is None or self._page_doc_cache[0] != self.catalog.version:
-                table = torch.from_numpy(self.catalog.page_documents()).to(self._index.device)
-                self._page_doc_cache = (self.catalog.version, table)
-            page_doc = self._page_doc_cache[1]
+            page_doc = self._page_doc_table()
+            if score_by == "document":
+                return self._doc_maxsim_unlocked(q, kk, per, page_doc, n_docs, words, min_score)
             if self._two_stage is not None:
                 ts, ti, pc, dc = self._two_stage.search_docs([q], kk, per, page_doc, n_docs,
                                                              n_candidates=max(self._n_candidates, kk * per), allow_mask=words)
@@ -451,6 +472,23 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 if chunks:
                     out.append(chunks)
             return out
+
+    def _doc_maxsim_unlocked(self, q, k, per, page_doc, n_docs, words, min_score):
+        if self._two_stage is not None:
+            ds, di, ei, es, ec, dc = self._two_stage.search_doc_maxsim([q], k, per, page_doc, n_docs,
+                                                                       n_candidates=max(self._n_candidates, k), allow_mask=words)
+        else:
+            ds, di, ei, es, ec, dc = self._index.search_doc_maxsim([q], k, per, page_doc, n_docs, allow_mask=words)
+        out = []
+        for i in range(int(dc[0])):
+            score = float(ds[0, i])
+            if min_score is not None and score < min_score:
+                break  # sorted by document score descending
+            chunks = self._chunks(es[0, i], ei[0, i], int(ec[0, i]))
+            for c in chunks:
+                c.metadata[DOCUMENT_SCORE_KEY] = score
+            out.append(chunks)
+        return out
 
     async def query_similar_mmr(self, query_embedding, k: int, fetch_k: int = 20, lambda_mult: float = 0.5,
                                 doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None) -> List[DocumentChunk]:

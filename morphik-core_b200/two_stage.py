@@ -256,6 +256,18 @@ class TwoStageSearch:
         return (_host(ts, (n_q, k, per_doc), -np.inf), _host(ti, (n_q, k, per_doc), -1), _host(pc, (n_q, k), 0),
                 dc.cpu().numpy())
 
+    def search_doc_maxsim(self, queries: Sequence, k: int, per_doc: int, page_doc_dev: torch.Tensor, n_docs: int,
+                          n_candidates: int = 1000, allow_mask: Optional[np.ndarray] = None):
+        """Document-level MaxSim through the first stage: max(n_candidates, k) candidate pages per query, then
+        MaxSimIndex.rerank_doc_maxsim_batch scores every allowed page of their documents.  The host allow mask (uint32
+        words) restricts both stages.  Synchronous; returns host arrays as MaxSimIndex.search_doc_maxsim."""
+        mask_dev = _host_mask_to_device(allow_mask, self.n_pages, self.device)
+        mask = self._mask(mask_dev, len(queries))
+        src, lens, q = self._prepare(queries)
+        _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k)), mask)
+        out = self.index.rerank_doc_maxsim_batch(src, lens, ci, k, per_doc, page_doc_dev, n_docs, allow_mask_dev=mask_dev)
+        return tuple(t.cpu().numpy() for t in out)
+
     def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
         """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
         the same exact scorer that ranked them."""
