@@ -542,6 +542,42 @@ int b200ms_rerank_examples_batch_device(b200ms_t* h, const void* q_dev, int src_
 int b200ms_union_candidates_device(b200ms_t* h, const int64_t* cand_ids_dev, int n_lists, int n_cand,
                                    const int32_t* list_off_host, int n_req, int64_t* out_dev, int width, void* cuda_stream);
 
+/* ---- near-duplicate pages (new; no reference counterpart) -------------------------------------------------------------
+ * A workspace fills with copies (a PDF uploaded twice, v3 and v4 of a report, a deck's repeated template pages), and a search
+ * then spends its top-k on copies of one page.  These calls compute the duplicate relation as a page -> group table that
+ * b200ms_search_docs_device / b200ms_rerank_docs_batch_device take as page_doc with per_doc = 1.
+ *   pair_maxsim_device: for each pair i (device int64 pair_a_dev / pair_b_dev [n_pairs], page ids of the attached corpus)
+ *     sim_ab_dev[i] = sim(a -> b) and sim_ba_dev[i] = sim(b -> a), float32, where sim(j -> s) is exactly b200ms_mmr_device's
+ *     sim: the rows, dot, max rule, summation order (each 64-row block of j in row order, the blocks in order; exact int64 for
+ *     I8 / B1) and __fdiv_rn(__fmul_rn(S, score_scale), len_j) -- bit for bit.  sim(b -> a) sums b's column maxima in the
+ *     same order, in 64-row blocks of b.  Both come from ONE tensor-core product per pair (dense dtypes: a's 64-row blocks
+ *     as the A operand, b's 128-row tiles as B; the epilogue takes row maxima and, over b's true rows, column maxima; 1-bit
+ *     corpora: 128 - popc on the CUDA cores).  Maxima commute, so the values do not depend on the schedule.  A page without
+ *     rows gives 0 both ways; an id outside [0, n_pages) gives NaN both ways.  Pairs may repeat and may be (a, a).  Pages of
+ *     any length work: column maxima of a page past 2048 rows go to per-CTA scratch in the handle.  One CTA per pair in a
+ *     grid-stride loop on cuda_stream, no host synchronisation.
+ *   duplicate_groups_device: a pair is an EDGE when sim_ab >= threshold and sim_ba >= threshold (the smaller direction; a
+ *     NaN never is one), both ids lie in [0, n_pages), a != b, and allow_mask_dev (uint32 page words, NULL = every page) has
+ *     both pages.  labels_dev (device int64 [n_pages]) gets, for every allowed page, the smallest page of its connected
+ *     component, and -1 for a page the mask excludes (the grouped top-k treats it as a deleted page): a group is never
+ *     joined through a page the mask hides.  On the GPU, as a lock-free union-find rather than rounds of min-label hooking
+ *     and pointer jumping repeated until nothing changes: one pass hooks each edge's larger root onto its smaller root with
+ *     a CAS and retries while the two roots differ.  Every retry of one edge follows the hooking of a root it had found,
+ *     and each root is hooked once, so each edge retries at most n_pages - 1 times (the bound is per edge; several edges
+ *     can fail on the same hook).  Labels only decrease (atomicMin, also in the path halving of every root search), so no
+ *     racing write moves a page back down its path; a second pass points every page at its root.  The result is the unique
+ *     minimum label of each component whatever the schedule.  Three launches on cuda_stream, no host synchronisation, no
+ *     iteration count to bound.
+ *   Neither call suggests a threshold: none has been measured on real ColPali pages.
+ * B200MS_EINVAL: n_pairs < 0, NULL arrays with n_pairs > 0, score_scale not finite and > 0, a non-finite threshold, NULL
+ * labels_dev;  B200MS_ESTATE: no corpus, a host-resident corpus (both pages of a pair are read from HBM), a corpus dtype
+ * without a scorer.  Nothing is launched when a call is refused. */
+int b200ms_pair_maxsim_device(b200ms_t* h, const int64_t* pair_a_dev, const int64_t* pair_b_dev, int64_t n_pairs,
+                              float score_scale, float* sim_ab_dev, float* sim_ba_dev, void* cuda_stream);
+int b200ms_duplicate_groups_device(b200ms_t* h, const int64_t* pair_a_dev, const int64_t* pair_b_dev,
+                                   const float* sim_ab_dev, const float* sim_ba_dev, int64_t n_pairs, float threshold,
+                                   const uint32_t* allow_mask_dev, int64_t* labels_dev, void* cuda_stream);
+
 /* ---- multi-GPU: document shards, one NCCL all-gather of top-k lists (SURVEY 8e; new relative to the reference) -------------
  * One process per GPU; every rank owns a handle over its shard.  NCCL is bound at run time (dlopen libnccl.so.2, or the
  * path in B200MS_NCCL_LIB); b200ms_comm_available() says whether that worked.

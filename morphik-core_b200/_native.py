@@ -141,6 +141,8 @@ _SIGNATURES = {
                                                 c_float, c_int64, vp, vp, vp, vp, vp, vp, vp]),
     "b200ms_rerank_doc_maxsim_batch_device": (c_int, [vp, vp, c_int, i32p, c_int, vp, c_int, c_int, c_int, vp, c_int64, vp,
                                                       c_int, vp, c_float, c_float, c_int64, vp, vp, vp, vp, vp, vp, vp]),
+    "b200ms_pair_maxsim_device": (c_int, [vp, vp, vp, c_int64, c_float, vp, vp, vp]),
+    "b200ms_duplicate_groups_device": (c_int, [vp, vp, vp, vp, vp, c_int64, c_float, vp, vp, vp]),
 }
 
 

@@ -13,7 +13,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libb200ms.so")
 SOURCES = ["api.cu", "maxsim_wgmma.cu", "maxsim_b1.cu", "pack.cu", "topk.cu", "fde.cu", "comm.cu", "host_tier.cu", "maxsim_explain.cu",
            "topk_docs.cu", "scan_plan.cu", "block.cu", "compact.cu", "signs.cu", "maxsim_mmr.cu",
-           "search_pages.cu", "search_examples.cu", "doc_maxsim.cu"]
+           "search_pages.cu", "search_examples.cu", "doc_maxsim.cu", "duplicates.cu"]
 HEADERS = ["common.cuh", "ptx.cuh", "mma_tile.cuh", "topk_keys.cuh", "scan.cuh", "row_tiles.cuh", os.path.join("..", "..", "include", "b200ms.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -320,7 +320,7 @@ B200MS_API int b200ms_destroy(b200ms_t* h) {
                        &h->ht_remap, &h->ht_ps, &h->ht_chunk_page, &h->ht_scores, &h->ht_stage, &h->scan_union, &h->scan_cnt,
                        &h->scan_off, &h->scan_start, &h->scan_end, &h->scan_hdr, &h->scan_word_off, &h->scan_pages,
                        &h->compact_meta, &h->compact_bounce, &h->mmr_state, &h->mmr_partials, &h->src_pages,
-                       &h->ex_meta, &h->ex_lists, &h->ex_fused, &h->ex_union, &h->dm_table, &h->dm_scores, &h->dm_allow};
+                       &h->ex_meta, &h->ex_lists, &h->ex_fused, &h->ex_union, &h->dm_table, &h->dm_scores, &h->dm_allow, &h->dup_cols};
   for (DeviceBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   release_blocks(h);

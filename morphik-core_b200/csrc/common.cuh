@@ -329,6 +329,8 @@ struct b200ms {
   // document-level MaxSim (doc_maxsim.cu): the token table, the document scores and found mask, the candidate calls'
   // document marks and allow rows
   bms::DeviceBuf dm_table, dm_scores, dm_allow;
+  // near-duplicate pages (duplicates.cu): per-CTA column maxima of pages too long for shared memory
+  bms::DeviceBuf dup_cols;
 };
 
 namespace bms {

@@ -13,6 +13,7 @@ C-ABI of libb200ms.so (``_native``).  Nothing here falls back to the CPU.
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -26,6 +27,39 @@ ArrayLike = Union[np.ndarray, torch.Tensor]
 
 def _vp(t: Optional[torch.Tensor]):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+# sources per first-stage call of a duplicate-candidate search: bounds the query rows staged at once (a 1030-row source
+# is 1030 query tokens)
+DUP_SOURCE_BATCH = 64
+
+
+def _check_n_candidates(n_candidates) -> int:
+    n = int(n_candidates)
+    if n < 1:
+        raise ValueError(f"n_candidates must be >= 1, got {n_candidates}")
+    return n
+
+
+def candidate_pairs(parts, n_candidates: int, device) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Candidate lists -> canonical page pairs.  parts: (source ids, device int64 [n_src, width] candidate ids, -1 =
+    unused) per batch; each source keeps its first n_candidates candidates other than itself.  Returns device int64
+    (pair_a, pair_b) with pair_a < pair_b, unique, ordered by (a, b)."""
+    lo, hi = [], []
+    for src, ti in parts:
+        s = torch.as_tensor(src, dtype=torch.int64, device=ti.device).view(-1, 1).expand_as(ti)
+        ok = (ti >= 0) & (ti != s)
+        ok &= torch.cumsum(ok.to(torch.int32), dim=1) <= int(n_candidates)
+        a, b = s[ok], ti[ok]
+        lo.append(torch.minimum(a, b))
+        hi.append(torch.maximum(a, b))
+    if not lo:
+        empty = torch.zeros((0,), dtype=torch.int64, device=device)
+        return empty, empty.clone()
+    lo_t, hi_t = torch.cat(lo), torch.cat(hi)
+    base = int(hi_t.max().item()) + 1 if hi_t.numel() else 1
+    key = torch.unique(lo_t * base + hi_t, sorted=True)
+    return (key // base).contiguous(), (key % base).contiguous()
 
 
 def _aligned_bytes(nbytes: int, device: torch.device, align: int = 1024) -> torch.Tensor:
@@ -1212,6 +1246,68 @@ class MaxSimIndex:
                                           _vp(tc), _vp(sims), self._stream()),
                 "b200ms_mmr_device")
         return (ti, ts, tc, sims) if with_sims else (ti, ts, tc)
+
+    # ------------------------------------------------------------------ near-duplicate pages
+    def _check_pairs(self, pair_a: torch.Tensor, pair_b: torch.Tensor) -> int:
+        for t in (pair_a, pair_b):
+            if t.dtype != torch.int64 or t.ndim != 1 or not t.is_contiguous() or t.device != self.device:
+                raise ValueError(f"pair ids must be contiguous int64 1-D tensors on {self.device}")
+        if pair_a.shape != pair_b.shape:
+            raise ValueError(f"pair_a and pair_b differ in length: {pair_a.shape[0]} != {pair_b.shape[0]}")
+        return int(pair_a.shape[0])
+
+    def pair_maxsim(self, pair_a: torch.Tensor, pair_b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Both directions of page-to-page MaxSim for each pair (b200ms_pair_maxsim_device), asynchronous on torch's current
+        stream: sim_ab[i] = sim(pair_a[i] -> pair_b[i]), sim_ba[i] = sim(pair_b[i] -> pair_a[i]), each the sum over the
+        first page's true rows of their best dot product with a row of the second, times score_scale, over the first
+        page's row count -- mmr(..., with_sims=True)'s value for the same pair, bit for bit.  One tensor-core product per pair
+        serves both directions.  An id outside [0, n_pages) gives NaN, a page without rows 0.  HBM tier only."""
+        n = self._check_pairs(pair_a, pair_b)
+        sab = torch.empty((n,), dtype=torch.float32, device=self.device)
+        sba = torch.empty((n,), dtype=torch.float32, device=self.device)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(nat.lib.b200ms_pair_maxsim_device(self.h.ptr, _vp(pair_a), _vp(pair_b), n,
+                                                           ctypes.c_float(self.score_scale), _vp(sab), _vp(sba),
+                                                           self._stream()), "b200ms_pair_maxsim_device")
+        return sab, sba
+
+    def duplicate_groups(self, pair_a: torch.Tensor, pair_b: torch.Tensor, sim_ab: torch.Tensor, sim_ba: torch.Tensor,
+                         threshold: float, allow_mask_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Duplicate groups (b200ms_duplicate_groups_device), asynchronous on torch's current stream: a pair is an edge when
+        min(sim_ab, sim_ba) >= threshold (a NaN never is) and the allow mask (uint32 page words, None = every page) has both
+        pages; groups are the connected components of the edges.  Returns int64 [n_pages] on the device: every allowed
+        page's smallest group member, -1 for a page the mask excludes.  No threshold has been measured on real pages: the
+        caller chooses it on the scale of the sims (pair_maxsim)."""
+        n = self._check_pairs(pair_a, pair_b)
+        for t in (sim_ab, sim_ba):
+            if t.dtype != torch.float32 or t.shape != (n,) or not t.is_contiguous() or t.device != self.device:
+                raise ValueError(f"sims must be contiguous float32 [{n}] tensors on {self.device}")
+        if not math.isfinite(float(threshold)):
+            raise ValueError(f"threshold must be a finite number, got {threshold}")
+        masks = _check_device_masks(allow_mask_dev, None, 1, self.n_pages, self.device)[0]
+        labels = torch.empty((self.n_pages,), dtype=torch.int64, device=self.device)
+        self._attach()
+        with torch.cuda.device(self.device):
+            self.h.check(nat.lib.b200ms_duplicate_groups_device(self.h.ptr, _vp(pair_a), _vp(pair_b), _vp(sim_ab),
+                                                                _vp(sim_ba), n, ctypes.c_float(threshold), _vp(masks),
+                                                                _vp(labels), self._stream()),
+                         "b200ms_duplicate_groups_device")
+        return labels
+
+    def duplicate_candidates(self, src_pages, n_candidates: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                             batch: int = DUP_SOURCE_BATCH) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Candidate pairs for the source pages: each source's top n_candidates other pages by search_pages under the allow
+        mask (uint32 page words, None = every page), sources in batches of ``batch``.  Returns canonical pairs
+        (candidate_pairs): device int64 (pair_a, pair_b), pair_a < pair_b, unique, ordered by (a, b)."""
+        ids = self._src_pages(src_pages)
+        n_cand = _check_n_candidates(n_candidates)
+        parts = []
+        for i in range(0, len(ids), int(batch)):
+            src = ids[i:i + int(batch)]
+            _, ti, _ = self.search_pages(src, min(n_cand + 1, nat.MAX_K), allow_mask_dev)
+            parts.append((src, ti))
+        return candidate_pairs(parts, n_cand, self.device)
 
     # ------------------------------------------------------------------ multi-GPU (document shards, NCCL inside libb200ms)
     @staticmethod

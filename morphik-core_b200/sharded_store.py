@@ -421,6 +421,18 @@ class ShardedB200MultiVectorStore(QueryCoalescer, BaseVectorStore):
                 out.append(_document_chunk(rec, 0.0))
         return out
 
+    async def index_duplicates(self, *args, **kw):
+        """Not supported: duplicate detection runs on one HBM-tier store (B200MultiVectorStore.index_duplicates)."""
+        raise NotImplementedError("the sharded store has no duplicate detection; use B200MultiVectorStore")
+
+    async def find_duplicate_chunks(self, *args, **kw):
+        """Not supported (see index_duplicates)."""
+        raise NotImplementedError("the sharded store has no duplicate detection; use B200MultiVectorStore")
+
+    async def query_similar_distinct(self, *args, **kw):
+        """Not supported (see index_duplicates)."""
+        raise NotImplementedError("the sharded store has no duplicate detection; use B200MultiVectorStore")
+
     async def delete_chunks_by_document_id(self, document_id: str, app_id: Optional[str] = None) -> bool:
         assert self.rank == 0
         try:

@@ -41,6 +41,8 @@ logger = logging.getLogger(__name__)
 MAX_K = 4096  # B200MS_MAX_K
 # metadata key of the document score on the chunks query_similar_documents(score_by="document") returns
 DOCUMENT_SCORE_KEY = "document_score"
+# metadata key of the other visible members of a chunk's duplicate group on the chunks query_similar_distinct returns
+DUPLICATES_KEY = "duplicates"
 
 try:  # inside a Morphik checkout the reference ABC is the real base class
     from core.vector_store.base_vector_store import BaseVectorStore  # type: ignore
@@ -237,6 +239,9 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
         self._last_store_metrics: Dict[str, Any] = {}
         self.last_query_timing: Dict[str, float] = {}
         self._page_doc_cache: Optional[Tuple[int, Any]] = None  # (catalog.version, device page -> document table)
+        # index_duplicates' pair table (device pair_a, pair_b, sim_ab, sim_ba) and the pages it has taken as sources;
+        # None until the first call, not persisted
+        self._dup: Optional[Dict[str, Any]] = None
         if auto_initialize:
             self.initialize()
 
@@ -544,6 +549,166 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
             self.last_query_timing.update({k: float(v) for k, v in self._two_stage.last_timing_ms.items()})
         return out
 
+    # ------------------------------------------------------------------ near-duplicate pages
+    def _refuse_duplicates_on_host_tier(self):
+        if self.corpus_tier != "hbm":
+            raise ValueError("duplicate detection needs an HBM-tier store (corpus_tier='hbm'): the pair kernel reads both "
+                             "pages of a pair from HBM")
+
+    async def index_duplicates(self, n_candidates: int = 10, rebuild: bool = False) -> int:
+        """Build or extend the near-duplicate pair table (extension; a maintenance call, like compaction): every live page
+        added since the previous call is a source, its ``n_candidates`` most similar live pages (the store's first stage
+        in two-stage mode, else search_pages) become candidate pairs, and one tensor-core product per pair scores both
+        directions of page-to-page MaxSim (MaxSimIndex.pair_maxsim).  ``rebuild=True`` starts over with every live page as
+        a source.  The table stays on the device; deletions drop out through the masks, compaction remaps it, and it is not
+        persisted: after ``load`` / ``open`` call this again.  It holds the store lock for the whole build, as compaction
+        does, so searches and ingests wait until it returns (seconds for tens of thousands of new pages; schedule it off
+        peak).  Returns the number of pairs in the table.  HBM-tier stores only."""
+        self._refuse_duplicates_on_host_tier()
+        n_cand = int(n_candidates)
+        if n_cand < 1:
+            raise ValueError(f"n_candidates must be >= 1, got {n_candidates}")
+        return await asyncio.to_thread(self._index_duplicates_locked, n_cand, bool(rebuild))
+
+    def _index_duplicates_locked(self, n_cand, rebuild):
+        import torch
+
+        with self._lock:
+            n = len(self.catalog)
+            dev = torch.device(self._index.device)
+            empty = torch.zeros((0,), dtype=torch.int64, device=dev)
+            old = self._dup if (self._dup is not None and not rebuild) else {
+                "a": empty, "b": empty, "sab": empty.float(), "sba": empty.float(), "n_indexed": 0}
+            src = [p for p in range(old["n_indexed"], n) if self.catalog.alive[p]]
+            a, b = empty, empty
+            if src:
+                _, words = self.catalog.allow_words(None, None)
+                mask = None if words is None else torch.from_numpy(words.view(np.int32)).to(dev)
+                target = self._two_stage if self._two_stage is not None else self._index
+                a, b = target.duplicate_candidates(src, n_cand, mask)
+            if a.numel():
+                sab, sba = self._index.pair_maxsim(a, b)
+                # the new pairs all have a page the old table never saw: concatenate and keep the table ordered by (a, b)
+                a, b = torch.cat([old["a"], a]), torch.cat([old["b"], b])
+                sab, sba = torch.cat([old["sab"], sab]), torch.cat([old["sba"], sba])
+                order = torch.argsort(a * max(n, 1) + b)
+                old = {"a": a[order].contiguous(), "b": b[order].contiguous(), "sab": sab[order].contiguous(),
+                       "sba": sba[order].contiguous()}
+            self._dup = dict(old, n_indexed=n)
+            if dev.type == "cuda":
+                torch.cuda.synchronize(dev)
+            return int(self._dup["a"].numel())
+
+    @staticmethod
+    def _check_threshold(threshold) -> float:
+        t = float(threshold)
+        if not np.isfinite(t):
+            raise ValueError(f"threshold must be a finite number, got {threshold}")
+        return t
+
+    def _duplicate_labels(self, threshold, words):
+        """Duplicate labels of the visible pages (device int64 [n_pages], -1 for a page the request may not see): the
+        cached pairs with both pages visible and min(sim_ab, sim_ba) >= threshold, joined into groups on the GPU.  Nothing is
+        re-scored, and no group is joined through a page the request may not see."""
+        import torch
+
+        if self._dup is None:
+            raise RuntimeError("no duplicate table: call index_duplicates() first (it is not persisted across load / open)")
+        d = self._dup
+        mask = None if words is None else torch.from_numpy(words.view(np.int32)).to(torch.device(self._index.device))
+        return self._index.duplicate_groups(d["a"], d["b"], d["sab"], d["sba"], threshold, mask)
+
+    async def find_duplicate_chunks(self, threshold: float, doc_ids: Optional[List[str]] = None,
+                                    app_id: Optional[str] = None) -> List[List[DocumentChunk]]:
+        """Groups of near-duplicate chunks (extension): pages joined by pairs of the index_duplicates table whose smaller
+        direction of page-to-page MaxSim (per row, on the scale of query_similar_to_chunks' scores) reaches ``threshold``,
+        among the chunks the ``doc_ids`` / ``app_id`` filter lets the caller see.  Returns every group of two or more chunks,
+        groups by their first page and chunks in page order (score 0).  No threshold has been measured on real ColPali
+        pages, so there is no default.  Needs index_duplicates() first; HBM-tier stores only."""
+        self._refuse_duplicates_on_host_tier()
+        t = self._check_threshold(threshold)
+        return await asyncio.to_thread(self._find_duplicates_locked, t, doc_ids, app_id)
+
+    def _find_duplicates_locked(self, threshold, doc_ids, app_id):
+        with self._lock:
+            if self._dup is None:
+                raise RuntimeError("no duplicate table: call index_duplicates() first (it is not persisted across load / "
+                                   "open)")
+            n = len(self.catalog)
+            if n == 0:
+                return []
+            visible, words = self.catalog.allow_words(doc_ids, app_id)
+            if not visible:
+                return []
+            labels = self._duplicate_labels(threshold, words).cpu().numpy()
+            pages = np.flatnonzero(labels >= 0)
+            groups: Dict[int, List[int]] = {}
+            for p in pages.tolist():
+                groups.setdefault(int(labels[p]), []).append(p)
+            return [[_document_chunk(self.catalog.records[p], 0.0) for p in g] for _, g in sorted(groups.items())
+                    if len(g) > 1]
+
+    async def query_similar_distinct(self, query_embedding, k: int, threshold: float, doc_ids: Optional[List[str]] = None,
+                                     app_id: Optional[str] = None,
+                                     min_score: Optional[float] = None) -> List[DocumentChunk]:
+        """query_similar with near-duplicates collapsed (extension): the best chunk of each duplicate group
+        (find_duplicate_chunks' groups at ``threshold``, among the chunks the filter lets the caller see), in query_similar's
+        order and with its scores, k groups at most.  It is the store's grouped search (exhaustive or two-stage) with the
+        duplicate labels as the page-to-group table.  Each chunk's ``metadata["duplicates"]`` lists the (document_id,
+        chunk_number) of the other visible members of its group.  ``min_score`` drops chunks below it.  The labels are
+        computed per request from the cached pairs (no page is re-scored).  No threshold has been measured on real ColPali
+        pages, so there is no default.  Needs index_duplicates() first; HBM-tier stores only."""
+        self._refuse_duplicates_on_host_tier()
+        q = as_query_matrix(query_embedding)
+        t = self._check_threshold(threshold)
+        if self._dup is None:
+            raise RuntimeError("no duplicate table: call index_duplicates() first (it is not persisted across load / open)")
+        if k <= 0:
+            return []
+        return await asyncio.to_thread(self._search_distinct_locked, q, int(k), t, doc_ids, app_id, min_score)
+
+    def _search_distinct_locked(self, q, k, threshold, doc_ids, app_id, min_score):
+        import torch
+
+        t0 = time.perf_counter()
+        with self._lock:
+            n = len(self.catalog)
+            if n == 0:
+                return []
+            visible, words = self.catalog.allow_words(doc_ids, app_id)
+            if not visible:
+                return []
+            kk = min(_capped_k(k), n)
+            labels = self._duplicate_labels(threshold, words)
+            t1 = time.perf_counter()
+            group = labels.to(torch.int32).contiguous()  # -1: not visible, as a deleted page in the grouped search
+            if self._two_stage is not None:
+                ts, ti, pc, dc = self._two_stage.search_docs([q], kk, 1, group, n, n_candidates=max(self._n_candidates, kk),
+                                                             allow_mask=words)
+            else:
+                ts, ti, pc, dc = self._index.search_docs([q], kk, 1, group, n, allow_mask=words)
+            t2 = time.perf_counter()
+            lab = labels.cpu().numpy()
+            # the pages of each group as one slice of the pages sorted by label (one sort per request, not a scan per hit)
+            by_label = np.argsort(lab, kind="stable")
+            sorted_lab = lab[by_label]
+            out = []
+            for i in range(int(dc[0])):
+                if int(pc[0, i]) < 1:
+                    continue
+                if min_score is not None and float(ts[0, i, 0]) < min_score:
+                    break  # sorted by score descending
+                p = int(ti[0, i, 0])
+                chunk = _document_chunk(self.catalog.records[p], ts[0, i, 0])
+                lo, hi = np.searchsorted(sorted_lab, lab[p], "left"), np.searchsorted(sorted_lab, lab[p], "right")
+                chunk.metadata[DUPLICATES_KEY] = [(self.catalog.records[o].document_id, self.catalog.records[o].chunk_number)
+                                                  for o in by_label[lo:hi].tolist() if o != p]
+                out.append(chunk)
+            t3 = time.perf_counter()
+        self.last_query_timing = {"labels_ms": (t1 - t0) * 1e3, "gpu_search_ms": (t2 - t1) * 1e3,
+                                  "build_chunks_ms": (t3 - t2) * 1e3, "total_ms": (t3 - t0) * 1e3}
+        return out
+
     async def query_similar_to_chunks(self, chunk_identifiers: List[Tuple[str, int]], k: int,
                                       doc_ids: Optional[List[str]] = None, app_id: Optional[str] = None,
                                       include_same_document: bool = False,
@@ -737,11 +902,20 @@ class B200MultiVectorStore(QueryCoalescer, BaseVectorStore):
 
     def _compact_locked(self):
         """Drop tombstoned pages: rebuild the device corpus from the surviving packed rows (device-to-device)."""
-        keep, _ = self.catalog.compaction_plan()
+        keep, remap = self.catalog.compaction_plan()
         target = self._two_stage or self._index
         if hasattr(target, "compact"):
             target.compact(keep)
         self.catalog.apply_compaction(keep)
+        if self._dup is not None:  # the pair table follows the pages: pairs with a dropped page go
+            import torch
+
+            d = self._dup
+            m = torch.from_numpy(remap).to(d["a"].device)
+            a, b = m[d["a"]], m[d["b"]]
+            ok = (a >= 0) & (b >= 0)
+            self._dup = {"a": a[ok].contiguous(), "b": b[ok].contiguous(), "sab": d["sab"][ok].contiguous(),
+                         "sba": d["sba"][ok].contiguous(), "n_indexed": int((keep < d["n_indexed"]).sum())}
 
     # ------------------------------------------------------------------ persistence (SURVEY 8f-2)
     def save(self, directory: str) -> None:

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .index import MaxSimIndex, _check_device_masks, _host_mask_to_device
+from .index import DUP_SOURCE_BATCH, MaxSimIndex, _check_device_masks, _check_n_candidates, _host_mask_to_device, candidate_pairs
 
 
 def _host(t: torch.Tensor, shape: Tuple[int, ...], fill) -> np.ndarray:
@@ -267,6 +267,23 @@ class TwoStageSearch:
         _, ci, _ = self._scan(q, lens, self._n_cand(max(n_candidates, k)), mask)
         out = self.index.rerank_doc_maxsim_batch(src, lens, ci, k, per_doc, page_doc_dev, n_docs, allow_mask_dev=mask_dev)
         return tuple(t.cpu().numpy() for t in out)
+
+    def duplicate_candidates(self, src_pages, n_candidates: int, allow_mask_dev: Optional[torch.Tensor] = None,
+                             batch: int = DUP_SOURCE_BATCH) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Candidate pairs for the source pages from the first stage alone: each source's dequantised rows
+        (MaxSimIndex.page_rows) go through the first-stage scan under the allow mask (uint32 page words, None = every page),
+        and its first n_candidates other pages become pairs.  No rerank: MaxSimIndex.pair_maxsim scores the pairs.  Returns
+        canonical pairs as MaxSimIndex.duplicate_candidates."""
+        ids = self.index._src_pages(src_pages)
+        n_cand = _check_n_candidates(n_candidates)
+        parts = []
+        for i in range(0, len(ids), int(batch)):
+            src = ids[i:i + int(batch)]
+            rows, lens = self.index.page_rows(src)
+            q = self._encode(None, (rows, nat.F32, lens))
+            _, ci, _ = self._scan(q, lens, self._n_cand(n_cand + 1), self._mask(allow_mask_dev, len(src)))
+            parts.append((src, ci))
+        return candidate_pairs(parts, n_cand, self.device)
 
     def explain(self, queries: Sequence, page_ids, map_rows: int = 0):
         """Per-token breakdown of the named pages' MaxSim (MaxSimIndex.explain): the pages a search returned are explained by
