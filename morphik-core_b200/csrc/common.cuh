@@ -412,6 +412,13 @@ inline CorpusView corpus_view(const b200ms_t* h) {
   return v;
 }
 
+// CTAs of a grid-stride launch over n items, per_block items per CTA: enough to cover them, at least 1 and at most per_sm
+// per SM
+inline int grid_stride_blocks(const b200ms_t* h, int64_t n, int per_block, int per_sm) {
+  const int64_t want = (n + per_block - 1) / per_block, cap = int64_t(h->num_sms) * per_sm;
+  return int(want < 1 ? 1 : want < cap ? want : cap);
+}
+
 // Pages of a host-resident corpus named by ids[0..n_slots) (host_tier.cu): dedup them, gather them into the staging block in
 // rounds of at most host_stage_bytes and call round_fn after each round's gather with the block as a corpus view and remap
 // (slot -> page of the view; -1 = invalid id or a page of another round).  Sets the gather stats; h->ht_rounds stays 0 when

@@ -200,11 +200,6 @@ __global__ void doc_empty_kernel(int n, int k, int per_doc, float* doc_scores, i
   }
 }
 
-static int blocks_for(const b200ms_t* h, int64_t n) {
-  const int64_t b = (n + 255) / 256;
-  return int(std::max<int64_t>(1, std::min<int64_t>(b, int64_t(h->num_sms) * 8)));
-}
-
 int64_t doc_table_bytes(int64_t groups, int64_t n_docs) { return groups * kGroup * n_docs * 8; }
 
 // One pass: queries [q0, q0 + n) of the call.  allow / mask_index as DocScan (mask_index already offset to the pass);
@@ -241,8 +236,8 @@ static int doc_pass(b200ms_t* h, const DocMaxSimCall& x, int q0, int n, const ui
   int64_t* ev_ids = x.ev_ids + int64_t(q0) * x.k * x.per_doc;
   int32_t* ev_counts = x.ev_counts + int64_t(q0) * x.k;
   if (ng == 0 || x.n_docs == 0 || c.n_pages == 0) {
-    doc_empty_kernel<<<blocks_for(h, int64_t(n) * x.k * x.per_doc), 256, 0, s>>>(n, x.k, x.per_doc, doc_scores, doc_ids,
-                                                                                 ev_scores, ev_ids, ev_counts, doc_counts);
+    doc_empty_kernel<<<grid_stride_blocks(h, int64_t(n) * x.k * x.per_doc, 256, 8), 256, 0, s>>>(
+        n, x.k, x.per_doc, doc_scores, doc_ids, ev_scores, ev_ids, ev_counts, doc_counts);
     h->launches++;
     return check_cuda(h, cudaGetLastError(), "launch doc_empty");
   }
@@ -344,13 +339,12 @@ int doc_maxsim(b200ms_t* h, const DocMaxSimCall& x, cudaStream_t s) {
     uint32_t* rows = docs + int64_t(x.n_q) * doc_words;
     if (int e = check_cuda(h, cudaMemsetAsync(docs, 0, size_t(x.n_q) * size_t(doc_words) * 4, s), "doc_maxsim: memset"))
       return e;
-    doc_mark_kernel<<<blocks_for(h, int64_t(x.n_q) * x.n_cand), 256, 0, s>>>(x.cand, x.n_cand, x.n_q, c.n_pages, x.page_doc,
-                                                                             x.n_docs, docs, doc_words);
+    doc_mark_kernel<<<grid_stride_blocks(h, int64_t(x.n_q) * x.n_cand, 256, 8), 256, 0, s>>>(
+        x.cand, x.n_cand, x.n_q, c.n_pages, x.page_doc, x.n_docs, docs, doc_words);
     h->launches++;
     if (int e = check_cuda(h, cudaGetLastError(), "launch doc_mark")) return e;
-    doc_allow_kernel<<<blocks_for(h, int64_t(x.n_q) * words), 256, 0, s>>>(docs, doc_words, x.n_q, c.n_pages, x.page_doc,
-                                                                           x.n_docs, allow, x.n_masks > 0 ? x.mask_index : nullptr,
-                                                                           rows);
+    doc_allow_kernel<<<grid_stride_blocks(h, int64_t(x.n_q) * words, 256, 8), 256, 0, s>>>(
+        docs, doc_words, x.n_q, c.n_pages, x.page_doc, x.n_docs, allow, x.n_masks > 0 ? x.mask_index : nullptr, rows);
     h->launches++;
     if (int e = check_cuda(h, cudaGetLastError(), "launch doc_allow")) return e;
     allow = rows;

@@ -4,12 +4,12 @@
 //
 // Pair kernel.  sim(a -> b) needs, per true row of a, the max over b's true rows; sim(b -> a) needs, per true row of b, the
 // max over a's true rows.  Both are reductions of the same row x row product, so one CTA (one warpgroup) runs a against b
-// once through row_tiles.cuh (A = 64-row blocks of a, B = 128-row tiles of b) and takes both from each accumulator tile:
-// row maxima exactly as mmr_round_wgmma takes them, and column maxima, folded over a's blocks into one value per row of b
-// (shared memory for pages up to kPairSmemCols rows, else a slice of global scratch owned by the CTA).  Maxima commute, so
-// neither depends on the schedule.  The sums then follow b200ms_mmr_device's order: true rows in row order inside a
-// 64-row block, the blocks in order, __fdiv_rn(__fmul_rn(S, scale), len).  1-bit corpora run 128 - popc on the CUDA cores,
-// as mmr_round_b1 does.
+// once through row_tiles.cuh's row_block_maxsim (A = 64-row blocks of a, B = 128-row tiles of b), the routine
+// mmr_round_wgmma runs: it gives the row maxima, and its per-tile hook takes the column maxima, folded over a's blocks into
+// one value per row of b (shared memory for pages up to kPairSmemCols rows, else a slice of global scratch owned by the
+// CTA).  Maxima commute, so neither depends on the schedule.  Both sums take b200ms_mmr_device's order from the same
+// helpers (ordered_sum, page_sim).  1-bit corpora run row_block_maxsim_b1 (128 - popc on the CUDA cores), as mmr_round_b1
+// does, its per-row hook taking the column maxima.
 //
 // Groups.  Lock-free union-find on the labels: every edge hooks the larger of its two roots onto the smaller with a CAS
 // and retries while its endpoints have different roots, so after one pass every component is one tree whose root is its
@@ -25,7 +25,6 @@
 namespace bms {
 
 constexpr int kPairSmemCols = 2048;  // column maxima of a page up to this many rows stay in shared memory
-constexpr int kPairB1Threads = 256;  // 1-bit pair kernel: 8 warps, 8 rows of a's 64-row block each
 constexpr int kLabelThreads = 256;
 
 struct PairArgs {
@@ -61,47 +60,21 @@ __device__ __forceinline__ bool pair_item(const PairArgs& a, int64_t i, int64_t&
   return true;
 }
 
-template <typename P>
-__device__ __forceinline__ float finish_pair(P s, float scale, int len) {
-  float sf;
-  if constexpr (std::is_same<P, float>::value) {
-    sf = s;
-  } else {
-    sf = __ll2float_rn(s);
-  }
-  return __fdiv_rn(__fmul_rn(sf, scale), float(len));
-}
-
-// thread 0: the sum of col[0 .. len) in 64-row blocks, each in row order from 0, the blocks added in order
-template <typename Acc, typename P>
-__device__ __forceinline__ P block_ordered_sum(const Acc* col, int len) {
-  P total = P(0);
-  for (int r0 = 0; r0 < len; r0 += kABlockRows) {
-    P s = P(0);
-    const int r1 = r0 + kABlockRows < len ? r0 + kABlockRows : len;
-    for (int r = r0; r < r1; ++r) s += P(col[r]);
-    total += s;
-  }
-  return total;
-}
-
 // ------------------------------------------------------------------ dense dtypes on wgmma (row_tiles.cuh)
 template <int KIND>
 __global__ void __launch_bounds__(kRowTileThreads) pair_maxsim_wgmma(const __grid_constant__ PairArgs a) {
-  using K = Kind<KIND>;
-  using Acc = typename K::Acc;
-  using P = typename std::conditional<KIND == 1, long long, float>::type;
+  using Acc = typename Kind<KIND>::Acc;
+  using P = RowSum<KIND>;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ Acc rowmax[kABlockRows];
   __shared__ Acc tile_cols[4][kTileN];  // per warp: max over its 16 rows of a, per column of the current tile
   __shared__ Acc col_smem[kPairSmemCols];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t b_addr = smem_u32(smem);
-  const uint32_t a_addr = b_addr + K::kPanels * kSubtileBytes;
+  const uint32_t a_addr = b_addr + Kind<KIND>::kPanels * kSubtileBytes;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = 16 * warp + (lane >> 2);
   const uint4* prows = static_cast<const uint4*>(a.rows);
-  const Acc none = KIND == 1 ? Acc(INT32_MIN) : Acc(__int_as_float(0x7fffffff));
+  const Acc none = max_none<Acc>();
   Acc* const col_global = static_cast<Acc*>(a.col_scratch) + int64_t(blockIdx.x) * a.col_stride;
   for (int64_t i = blockIdx.x; i < a.n_pairs; i += gridDim.x) {
     int64_t pa, pb;
@@ -111,24 +84,15 @@ __global__ void __launch_bounds__(kRowTileThreads) pair_maxsim_wgmma(const __gri
     // column c is only ever touched by thread c % 128 until the sums below
     for (int c = threadIdx.x; c < lb; c += kRowTileThreads) col[c] = none;
     const int64_t a0 = __ldg(a.page_start + pa), b0 = __ldg(a.page_start + pb);
-    P s_ab = P(0);
-    for (int tt = 0; tt * kABlockRows < la; ++tt) {
+    const P s_ab = ordered_sum<P>((la + kABlockRows - 1) / kABlockRows, [&](int tt) {
       const int rows = la - tt * kABlockRows < kABlockRows ? la - tt * kABlockRows : kABlockRows;
       const bool ok0 = m0 < rows, ok1 = m0 + 8 < rows;
-      Acc mx0 = none, mx1 = none;
-      rows_vs_page_tiles<KIND>(
-          a_addr, b_addr, prows, b0, (lb + kGroup - 1) & ~(kGroup - 1),
-          [&] { load_a_block<KIND>(a_addr, prows, a0 + int64_t(tt) * kABlockRows, a.n_rows); },
-          [&](const Acc(&d)[64], int n) {
-            const int rbase = n * kTileN + 2 * (lane & 3);
+      return row_block_maxsim<KIND>(
+          a_addr, b_addr, prows, a0 + int64_t(tt) * kABlockRows, rows, a.n_rows, b0, lb, [&](const Acc(&d)[64], int n) {
 #pragma unroll
             for (int jb = 0; jb < 16; ++jb) {
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                if (rbase + 8 * jb + e < lb) {
-                  mx0 = acc_max(mx0, d[4 * jb + e]);
-                  mx1 = acc_max(mx1, d[4 * jb + 2 + e]);
-                }
                 // column 8 jb + 2 (lane & 3) + e of the tile over this warp's true rows of a
                 Acc v = ok0 ? d[4 * jb + e] : none;
                 if (ok1) v = acc_max(v, d[4 * jb + 2 + e]);
@@ -147,35 +111,20 @@ __global__ void __launch_bounds__(kRowTileThreads) pair_maxsim_wgmma(const __gri
             }
             // tile_cols is rewritten only after the tile loop's next barrier
           });
-      mx0 = quad_max(mx0);
-      mx1 = quad_max(mx1);
-      if ((lane & 3) == 0) {
-        rowmax[m0] = mx0;
-        rowmax[m0 + 8] = mx1;
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        P s = P(0);
-        for (int r = 0; r < rows; ++r) s += P(rowmax[r]);
-        s_ab += s;
-      }
-      // rowmax is rewritten only after the next block's first barrier
-    }
+    });
     __syncthreads();  // every column maximum is final
     if (threadIdx.x == 0) {
-      a.sim_ab[i] = finish_pair<P>(s_ab, a.scale, la);
-      a.sim_ba[i] = finish_pair<P>(block_ordered_sum<Acc, P>(col, lb), a.scale, lb);
+      a.sim_ab[i] = page_sim<P>(s_ab, a.scale, la);
+      a.sim_ba[i] = page_sim<P>(block_ordered_sum<P>(col, lb), a.scale, lb);
     }
     __syncthreads();  // col is read before the next pair initialises it
   }
 }
 
 // ------------------------------------------------------------------ 1-bit corpora: 128 - popc(a ^ b), exact
-__global__ void __launch_bounds__(kPairB1Threads) pair_maxsim_b1(const __grid_constant__ PairArgs a) {
-  constexpr int kRowsPerWarp = kABlockRows / (kPairB1Threads / 32);
-  __shared__ int rowmax[kABlockRows];
+__global__ void __launch_bounds__(kRowBlockB1Threads) pair_maxsim_b1(const __grid_constant__ PairArgs a) {
   __shared__ int col_smem[kPairSmemCols];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const uint4* prows = static_cast<const uint4*>(a.rows);
   int* const col_global = static_cast<int*>(a.col_scratch) + int64_t(blockIdx.x) * a.col_stride;
   for (int64_t i = blockIdx.x; i < a.n_pairs; i += gridDim.x) {
@@ -183,50 +132,25 @@ __global__ void __launch_bounds__(kPairB1Threads) pair_maxsim_b1(const __grid_co
     int la, lb;
     if (!pair_item(a, i, pa, pb, la, lb)) continue;
     int* col = lb <= kPairSmemCols ? col_smem : col_global;
-    for (int c = threadIdx.x; c < lb; c += kPairB1Threads) col[c] = INT32_MIN;
+    for (int c = threadIdx.x; c < lb; c += kRowBlockB1Threads) col[c] = INT32_MIN;
     __syncthreads();  // the column maxima are updated by every warp
     const int64_t a0 = __ldg(a.page_start + pa), b0 = __ldg(a.page_start + pb);
-    long long s_ab = 0;
-    for (int tt = 0; tt * kABlockRows < la; ++tt) {
+    const long long s_ab = ordered_sum<long long>((la + kABlockRows - 1) / kABlockRows, [&](int tt) {
       const int rows = la - tt * kABlockRows < kABlockRows ? la - tt * kABlockRows : kABlockRows;
-      const int warp_rows = rows - warp * kRowsPerWarp;  // this warp's true rows of the block (may be <= 0)
-      uint4 av[kRowsPerWarp];
-      int mx[kRowsPerWarp];
+      const int warp_rows = rows - warp * kB1RowsPerWarp;  // this warp's true rows of the block (may be <= 0)
+      return row_block_maxsim_b1(prows, a0 + int64_t(tt) * kABlockRows, rows, b0, lb,
+                                 [&](int row, const int (&v)[kB1RowsPerWarp]) {
+                                   int cm = INT32_MIN;
 #pragma unroll
-      for (int k = 0; k < kRowsPerWarp; ++k) {
-        av[k] = k < warp_rows ? __ldg(prows + a0 + int64_t(tt) * kABlockRows + warp * kRowsPerWarp + k)
-                              : make_uint4(0, 0, 0, 0);
-        mx[k] = INT32_MIN;
-      }
-      for (int row = lane; row < lb; row += 32) {
-        const uint4 dv = __ldg(prows + b0 + row);
-        int cm = INT32_MIN;
-#pragma unroll
-        for (int k = 0; k < kRowsPerWarp; ++k) {
-          const int v = 128 - (__popc(av[k].x ^ dv.x) + __popc(av[k].y ^ dv.y) + __popc(av[k].z ^ dv.z) +
-                               __popc(av[k].w ^ dv.w));
-          mx[k] = max(mx[k], v);
-          if (k < warp_rows) cm = max(cm, v);
-        }
-        if (warp_rows > 0) atomicMax(col + row, cm);
-      }
-#pragma unroll
-      for (int k = 0; k < kRowsPerWarp; ++k) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx[k] = max(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
-        if (lane == 0) rowmax[warp * kRowsPerWarp + k] = mx[k];
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        long long s = 0;
-        for (int r = 0; r < rows; ++r) s += rowmax[r];
-        s_ab += s;
-      }
-      __syncthreads();  // rowmax is read before the next block writes it
-    }
+                                   for (int k = 0; k < kB1RowsPerWarp; ++k)
+                                     if (k < warp_rows) cm = max(cm, v[k]);
+                                   if (warp_rows > 0) atomicMax(col + row, cm);
+                                 });
+    });
+    // row_block_maxsim_b1 ends with a barrier (la > 0): every column maximum is final
     if (threadIdx.x == 0) {
-      a.sim_ab[i] = finish_pair<long long>(s_ab, a.scale, la);
-      a.sim_ba[i] = finish_pair<long long>(block_ordered_sum<int, long long>(col, lb), a.scale, lb);
+      a.sim_ab[i] = page_sim<long long>(s_ab, a.scale, la);
+      a.sim_ba[i] = page_sim<long long>(block_ordered_sum<long long>(col, lb), a.scale, lb);
     }
     __syncthreads();  // col is read before the next pair initialises it
   }
@@ -290,11 +214,6 @@ __global__ void __launch_bounds__(kLabelThreads) labels_finish_kernel(int64_t* l
     if (L[p] >= 0) atomicMin(reinterpret_cast<long long*>(labels + p), static_cast<long long>(find_root(L, p)));
 }
 
-static int grid_for(const b200ms_t* h, int64_t n, int threads) {
-  const int64_t want = (n + threads - 1) / threads, cap = int64_t(h->num_sms) * 8;
-  return int(want < 1 ? 1 : want < cap ? want : cap);
-}
-
 }  // namespace bms
 
 using namespace bms;
@@ -318,21 +237,14 @@ B200MS_API int b200ms_pair_maxsim_device(b200ms_t* h, const int64_t* pair_a_dev,
   cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
   StreamOrder order(h, s);
   if (int e = order.error()) return e;
-  const bool b1 = c.dtype == B200MS_B1;
-  const void* kern = b1 ? reinterpret_cast<const void*>(pair_maxsim_b1) : nullptr;
-  int smem = 0;
-  switch (kind_of_dtype(c.dtype)) {
-    case 0: kern = reinterpret_cast<const void*>(pair_maxsim_wgmma<0>); smem = row_tiles_smem<0>(); break;
-    case 1: kern = reinterpret_cast<const void*>(pair_maxsim_wgmma<1>); smem = row_tiles_smem<1>(); break;
-    case 2: kern = reinterpret_cast<const void*>(pair_maxsim_wgmma<2>); smem = row_tiles_smem<2>(); break;
-    default: break;
-  }
-  if (!b1)
-    if (int e = ensure_smem(h, kern, smem, "cudaFuncSetAttribute(pair_maxsim_wgmma)")) return e;
+  RowTileKernel<PairArgs> k;
+  if (int e = row_tile_kernel(h, c.dtype, pair_maxsim_wgmma<0>, pair_maxsim_wgmma<1>, pair_maxsim_wgmma<2>, pair_maxsim_b1,
+                              kRowBlockB1Threads, "pair_maxsim", &k))
+    return e;
   // one CTA per pair in a grid-stride loop: as many CTAs as fit on the card at once
   int per_sm = 0;
-  if (int e = check_cuda(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, b1 ? kPairB1Threads : kRowTileThreads,
-                                                                          size_t(smem)),
+  if (int e = check_cuda(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reinterpret_cast<const void*>(k.fn),
+                                                                          k.threads, size_t(k.smem)),
                          "pair_maxsim: occupancy"))
     return e;
   const int64_t cap = int64_t(h->num_sms) * (per_sm > 0 ? per_sm : 1);
@@ -355,13 +267,7 @@ B200MS_API int b200ms_pair_maxsim_device(b200ms_t* h, const int64_t* pair_a_dev,
     a.col_scratch = h->dup_cols.p;
     a.col_stride = c.max_page_rows;
   }
-  void* args[] = {&a};
-  if (int e = check_cuda(h, cudaLaunchKernel(kern, dim3(grid), dim3(b1 ? kPairB1Threads : kRowTileThreads), args,
-                                             size_t(smem), s),
-                         "launch pair_maxsim"))
-    return e;
-  h->launches++;
-  return check_cuda(h, cudaGetLastError(), "launch pair_maxsim");
+  return launch_row_tiles(h, k, dim3(grid), a, s, "launch pair_maxsim");
 }
 
 B200MS_API int b200ms_duplicate_groups_device(b200ms_t* h, const int64_t* pair_a_dev, const int64_t* pair_b_dev,
@@ -380,16 +286,17 @@ B200MS_API int b200ms_duplicate_groups_device(b200ms_t* h, const int64_t* pair_a
   cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
   StreamOrder order(h, s);
   if (int e = order.error()) return e;
-  labels_init_kernel<<<grid_for(h, c.n_pages, kLabelThreads), kLabelThreads, 0, s>>>(labels_dev, c.n_pages, allow_mask_dev);
+  labels_init_kernel<<<grid_stride_blocks(h, c.n_pages, kLabelThreads, 8), kLabelThreads, 0, s>>>(
+      labels_dev, c.n_pages, allow_mask_dev);
   h->launches++;
   if (int e = check_cuda(h, cudaGetLastError(), "launch labels_init")) return e;
   if (n_pairs > 0) {
-    hook_edges_kernel<<<grid_for(h, n_pairs, kLabelThreads), kLabelThreads, 0, s>>>(
+    hook_edges_kernel<<<grid_stride_blocks(h, n_pairs, kLabelThreads, 8), kLabelThreads, 0, s>>>(
         pair_a_dev, pair_b_dev, sim_ab_dev, sim_ba_dev, n_pairs, threshold, c.n_pages, allow_mask_dev, labels_dev);
     h->launches++;
     if (int e = check_cuda(h, cudaGetLastError(), "launch hook_edges")) return e;
   }
-  labels_finish_kernel<<<grid_for(h, c.n_pages, kLabelThreads), kLabelThreads, 0, s>>>(labels_dev, c.n_pages);
+  labels_finish_kernel<<<grid_stride_blocks(h, c.n_pages, kLabelThreads, 8), kLabelThreads, 0, s>>>(labels_dev, c.n_pages);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch labels_finish");
 }

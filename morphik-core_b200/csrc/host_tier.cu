@@ -147,13 +147,6 @@ __global__ void ht_merge_round_kernel(int32_t* __restrict__ dst, const int32_t* 
   }
 }
 
-static int grid_of(const b200ms_t* h, int64_t n) {
-  int64_t b = (n + 255) / 256;
-  const int64_t cap = int64_t(h->num_sms) * 8;
-  if (b > cap) b = cap;
-  return b < 1 ? 1 : int(b);
-}
-
 // round geometry: capacity cap rows (the budget, at least the largest page), pages starting in each W-row window
 static void round_geometry(const b200ms_t* h, int64_t* cap, int64_t* W) {
   const Corpus& c = h->corpus;
@@ -191,9 +184,9 @@ int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStrea
   const int64_t* ps = static_cast<const int64_t*>(h->page_start.p);
   // 1-2: dedup + plan
   if (int e = check_cuda(h, cudaMemsetAsync(bitmap, 0, size_t(n_words > 0 ? n_words : 1) * 4, s), "host tier: memset")) return e;
-  ht_mark_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(ids, n_slots, c.n_pages, bitmap);
+  ht_mark_kernel<<<grid_stride_blocks(h, n_slots, 256, 8), 256, 0, s>>>(ids, n_slots, c.n_pages, bitmap);
   ht_scan_words_kernel<<<1, kScanThreads, 0, s>>>(bitmap, n_words, wpre);
-  ht_compact_kernel<<<grid_of(h, n_words), 256, 0, s>>>(bitmap, n_words, wpre, uniq);
+  ht_compact_kernel<<<grid_stride_blocks(h, n_words, 256, 8), 256, 0, s>>>(bitmap, n_words, wpre, uniq);
   ht_scan_rows_kernel<<<1, kScanThreads, 0, s>>>(uniq, wpre + n_words, ps, stage_off, static_cast<int64_t*>(h->ht_hdr.p));
   h->launches += 4;
   if (int e = check_cuda(h, cudaGetLastError(), "launch host-tier dedup")) return e;
@@ -236,9 +229,10 @@ int gather_host_tier(b200ms_t* h, const int64_t* ids, int64_t n_slots, cudaStrea
   v.page_start = static_cast<const int64_t*>(h->ht_ps.p);
   const int piece_shift = rb == 256 ? 4 : rb == 128 ? 3 : 0;
   for (int r = 0; r < rounds; ++r) {
-    ht_round_plan_kernel<<<grid_of(h, n_uniq), 256, 0, s>>>(stage_off, n_uniq, W, r, static_cast<int64_t*>(h->ht_ps.p),
-                                                          static_cast<int32_t*>(h->ht_chunk_page.p));
-    ht_remap_kernel<<<grid_of(h, n_slots), 256, 0, s>>>(ids, n_slots, c.n_pages, bitmap, wpre, stage_off, n_uniq, W, r, remap);
+    ht_round_plan_kernel<<<grid_stride_blocks(h, n_uniq, 256, 8), 256, 0, s>>>(
+        stage_off, n_uniq, W, r, static_cast<int64_t*>(h->ht_ps.p), static_cast<int32_t*>(h->ht_chunk_page.p));
+    ht_remap_kernel<<<grid_stride_blocks(h, n_slots, 256, 8), 256, 0, s>>>(
+        ids, n_slots, c.n_pages, bitmap, wpre, stage_off, n_uniq, W, r, remap);
     if (int e = check_cuda(h, cudaEventRecord(h->ht_ev[2 * r], s), "host tier: event record")) return e;
     ht_gather_kernel<<<h->num_sms * 8, 256, 0, s>>>(static_cast<const uint4*>(c.rows), piece_shift, ps, uniq, stage_off, n_uniq,
                                                    W, r, v.page_start, v.chunk_page, static_cast<uint4*>(stage));
@@ -274,9 +268,8 @@ int score_host_tier(b200ms_t* h, const CandSpec& cs, int n_q, int64_t gp, int64_
         return e;
     }
     if (int e = x.score_round(hh, v, remap, hh->ht_scores.p, true, x.ctx)) return e;
-    ht_merge_round_kernel<<<grid_of(hh, x.gp * x.n_slots), 256, 0, x.s>>>(static_cast<int32_t*>(x.group_scores),
-                                                                        static_cast<const int32_t*>(hh->ht_scores.p), remap,
-                                                                        x.n_slots, x.gp, x.ld);
+    ht_merge_round_kernel<<<grid_stride_blocks(hh, x.gp * x.n_slots, 256, 8), 256, 0, x.s>>>(
+        static_cast<int32_t*>(x.group_scores), static_cast<const int32_t*>(hh->ht_scores.p), remap, x.n_slots, x.gp, x.ld);
     hh->launches++;
     return check_cuda(hh, cudaGetLastError(), "launch host-tier merge");
   };

@@ -264,25 +264,11 @@ static int launch_explain(b200ms_t* h, const ExplainArgs& a, int dtype, cudaStre
   int gx = (h->num_sms * 8 + gy - 1) / gy;
   if (gx > n_slots) gx = n_slots;
   const dim3 grid{unsigned(gx), unsigned(gy)};
-  if (dtype == B200MS_B1) {
-    maxsim_explain_b1<<<grid, kExplainB1Threads, 0, s>>>(a);
-  } else {
-    const void* kern = nullptr;
-    int smem = 0;
-    switch (kind_of_dtype(dtype)) {
-      case 0: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<0>); smem = row_tiles_smem<0>(); break;
-      case 1: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<1>); smem = row_tiles_smem<1>(); break;
-      case 2: kern = reinterpret_cast<const void*>(maxsim_explain_wgmma<2>); smem = row_tiles_smem<2>(); break;
-      default: return set_error(h, B200MS_ESTATE, "explain: corpus dtype has no scorer");
-    }
-    if (int e = ensure_smem(h, kern, smem, "cudaFuncSetAttribute(maxsim_explain_wgmma)")) return e;
-    void* args[] = {const_cast<ExplainArgs*>(&a)};
-    if (int e = check_cuda(h, cudaLaunchKernel(kern, grid, dim3(kExplainThreads), args, size_t(smem), s),
-                           "launch maxsim_explain_wgmma"))
-      return e;
-  }
-  h->launches++;
-  return check_cuda(h, cudaGetLastError(), "launch maxsim_explain");
+  RowTileKernel<ExplainArgs> k;
+  if (int e = row_tile_kernel(h, dtype, maxsim_explain_wgmma<0>, maxsim_explain_wgmma<1>, maxsim_explain_wgmma<2>,
+                              maxsim_explain_b1, kExplainB1Threads, "maxsim_explain", &k))
+    return e;
+  return launch_row_tiles(h, k, grid, a, s, "launch maxsim_explain");
 }
 
 }  // namespace bms

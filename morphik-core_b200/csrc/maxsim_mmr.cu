@@ -3,8 +3,9 @@
 //
 // Coverage is page-to-page MaxSim, sim(j -> s) = sum over the true rows of j of the max over the true rows of s of the row
 // dot product, per row of j.  Rows against rows of two pages is the scan's work, so it runs on the scan's instructions:
-// the dense dtypes through row_tiles.cuh (the tile loop b200ms_explain_device uses; A = a 64-row tile of candidate j, B =
-// the page picked last, in 128-row tiles), 1-bit corpora as 128 - popc on the CUDA cores.
+// the dense dtypes through row_tiles.cuh's row_block_maxsim (the tile loop b200ms_explain_device uses; A = a 64-row tile of
+// candidate j, B = the page picked last, in 128-row tiles), 1-bit corpora through row_block_maxsim_b1 (128 - popc on the
+// CUDA cores).  b200ms_pair_maxsim_device (duplicates.cu) runs the same routines, so its sims are these bit for bit.
 //
 // One call = a setup kernel (outputs, the live-slot table with the duplicate rule, pick 1 by relevance) and per further pick
 // two kernels on the caller's stream, without a host synchronisation:
@@ -25,7 +26,6 @@
 namespace bms {
 
 constexpr int kMmrPickThreads = 256;  // setup / pick kernels: one CTA per query
-constexpr int kMmrB1Threads = 256;    // 1-bit round kernel: 8 warps, 8 rows of the tile each
 
 struct MmrArgs {
   const int64_t* ids = nullptr;       // [n_q, n_cand] corpus page ids (-1 / out of range = unused slot)
@@ -135,21 +135,12 @@ __global__ void __launch_bounds__(kMmrPickThreads) mmr_setup_kernel(const __grid
   }
 }
 
-// sim(j -> s) from slot j's partials: score_scale * S / len_j in fp32, 0 when either page has no rows
+// sim(j -> s) from slot j's partials, added in tile order; 0 when either page has no rows
 template <typename P>
 __device__ __forceinline__ float finish_sim(const MmrArgs& a, int64_t slot, int len_j, int len_s) {
   if (len_j == 0 || len_s == 0) return 0.f;
   const P* p = static_cast<const P*>(a.partials) + slot * a.n_tiles;
-  P acc = P(0);
-  const int nt = (len_j + kABlockRows - 1) / kABlockRows;
-  for (int t = 0; t < nt; ++t) acc += p[t];
-  float sf;
-  if constexpr (std::is_same<P, float>::value) {
-    sf = acc;
-  } else {
-    sf = __ll2float_rn(acc);
-  }
-  return __fdiv_rn(__fmul_rn(sf, a.scale), float(len_j));
+  return page_sim<P>(ordered_sum<P>((len_j + kABlockRows - 1) / kABlockRows, [&](int t) { return p[t]; }), a.scale, len_j);
 }
 
 // sims against pick i - 1 into red (and row i - 1 of sims), then pick i; choose_next == 0: the sims row only
@@ -197,98 +188,34 @@ __device__ __forceinline__ MmrItem mmr_item(const MmrArgs& a, int64_t slot, int 
   return x;
 }
 
-// thread 0: the tile's partial, the sum of its true rows' maxima in row order
-template <typename Acc, typename P>
-__device__ __forceinline__ void write_partial(const MmrArgs& a, int64_t slot, int tt, const Acc* rowmax, int rows) {
-  P acc = P(0);
-  for (int r = 0; r < rows; ++r) acc += P(rowmax[r]);
-  static_cast<P*>(a.partials)[slot * a.n_tiles + tt] = acc;
-}
-
 // ------------------------------------------------------------------ dense dtypes on wgmma (row_tiles.cuh)
 template <int KIND>
 __global__ void __launch_bounds__(kRowTileThreads) mmr_round_wgmma(const __grid_constant__ MmrArgs a) {
-  using K = Kind<KIND>;
-  using Acc = typename K::Acc;
-  using P = typename std::conditional<KIND == 1, long long, float>::type;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ Acc rowmax[kABlockRows];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t b_addr = smem_u32(smem);                       // [kPanels][128 rows x 128 B]
-  const uint32_t a_addr = b_addr + K::kPanels * kSubtileBytes;  // [kPanels][64 rows x 128 B]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = 16 * warp + (lane >> 2);
+  const uint32_t b_addr = smem_u32(smem);                                  // [kPanels][128 rows x 128 B]
+  const uint32_t a_addr = b_addr + Kind<KIND>::kPanels * kSubtileBytes;  // [kPanels][64 rows x 128 B]
   const uint4* prows = static_cast<const uint4*>(a.rows);
-  // the max over no row yet: fmaxf's identity (a NaN row max stays NaN only when every row is NaN) / the least int
-  const Acc none = KIND == 1 ? Acc(INT32_MIN) : Acc(__int_as_float(0x7fffffff));
   const int64_t n_slots = int64_t(a.n_q) * a.n_cand;
   for (int tt = blockIdx.y; tt < a.n_tiles; tt += gridDim.y)
   for (int64_t slot = blockIdx.x; slot < n_slots; slot += gridDim.x) {
     const MmrItem x = mmr_item(a, slot, tt);
     if (!x.compute) continue;
-    Acc mx0 = none, mx1 = none;  // A rows m0 and m0 + 8: this lane's max over its columns
-    rows_vs_page_tiles<KIND>(
-        a_addr, b_addr, prows, x.b_row0, (x.len_s + kGroup - 1) & ~(kGroup - 1),
-        [&] { load_a_block<KIND>(a_addr, prows, x.a_row0, a.n_rows); },
-        [&](const Acc(&d)[64], int n) {
-          const int rbase = n * kTileN + 2 * (lane & 3);
-#pragma unroll
-          for (int jb = 0; jb < 16; ++jb) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              if (rbase + 8 * jb + e < x.len_s) {
-                mx0 = acc_max(mx0, d[4 * jb + e]);
-                mx1 = acc_max(mx1, d[4 * jb + 2 + e]);
-              }
-            }
-          }
-        });
-    mx0 = quad_max(mx0);
-    mx1 = quad_max(mx1);
-    if ((lane & 3) == 0) {
-      rowmax[m0] = mx0;
-      rowmax[m0 + 8] = mx1;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) write_partial<Acc, P>(a, slot, tt, rowmax, x.rows);
+    const RowSum<KIND> s = row_block_maxsim<KIND>(a_addr, b_addr, prows, x.a_row0, x.rows, a.n_rows, x.b_row0, x.len_s);
+    if (threadIdx.x == 0) static_cast<RowSum<KIND>*>(a.partials)[slot * a.n_tiles + tt] = s;
   }
 }
 
 // ------------------------------------------------------------------ 1-bit corpora: 128 - popc(a ^ b), exact
-__global__ void __launch_bounds__(kMmrB1Threads) mmr_round_b1(const __grid_constant__ MmrArgs a) {
-  constexpr int kRowsPerWarp = kABlockRows / (kMmrB1Threads / 32);
-  __shared__ int rowmax[kABlockRows];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+__global__ void __launch_bounds__(kRowBlockB1Threads) mmr_round_b1(const __grid_constant__ MmrArgs a) {
   const uint4* prows = static_cast<const uint4*>(a.rows);
   const int64_t n_slots = int64_t(a.n_q) * a.n_cand;
   for (int tt = blockIdx.y; tt < a.n_tiles; tt += gridDim.y)
   for (int64_t slot = blockIdx.x; slot < n_slots; slot += gridDim.x) {
     const MmrItem x = mmr_item(a, slot, tt);
     if (!x.compute) continue;
-    uint4 av[kRowsPerWarp];
-    int mx[kRowsPerWarp];
-#pragma unroll
-    for (int i = 0; i < kRowsPerWarp; ++i) {
-      const int r = warp * kRowsPerWarp + i;
-      av[i] = r < x.rows ? __ldg(prows + x.a_row0 + r) : make_uint4(0, 0, 0, 0);
-      mx[i] = INT32_MIN;
-    }
-    for (int row = lane; row < x.len_s; row += 32) {
-      const uint4 dv = __ldg(prows + x.b_row0 + row);
-#pragma unroll
-      for (int i = 0; i < kRowsPerWarp; ++i)
-        mx[i] = max(mx[i], 128 - (__popc(av[i].x ^ dv.x) + __popc(av[i].y ^ dv.y) + __popc(av[i].z ^ dv.z) +
-                                  __popc(av[i].w ^ dv.w)));
-    }
-#pragma unroll
-    for (int i = 0; i < kRowsPerWarp; ++i) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx[i] = max(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], o));
-      if (lane == 0) rowmax[warp * kRowsPerWarp + i] = mx[i];
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) write_partial<int, long long>(a, slot, tt, rowmax, x.rows);
-    __syncthreads();  // rowmax is read before the next item writes it
+    const long long s = row_block_maxsim_b1(prows, x.a_row0, x.rows, x.b_row0, x.len_s);
+    if (threadIdx.x == 0) static_cast<long long*>(a.partials)[slot * a.n_tiles + tt] = s;
   }
 }
 
@@ -300,24 +227,11 @@ static int launch_round(b200ms_t* h, const MmrArgs& a, int dtype, cudaStream_t s
   int64_t gx = (int64_t(h->num_sms) * 8 + gy - 1) / gy;
   if (gx > n_slots) gx = n_slots;
   const dim3 grid{unsigned(gx), unsigned(gy)};
-  if (dtype == B200MS_B1) {
-    mmr_round_b1<<<grid, kMmrB1Threads, 0, s>>>(a);
-  } else {
-    const void* kern = nullptr;
-    int smem = 0;
-    switch (kind_of_dtype(dtype)) {
-      case 0: kern = reinterpret_cast<const void*>(mmr_round_wgmma<0>); smem = row_tiles_smem<0>(); break;
-      case 1: kern = reinterpret_cast<const void*>(mmr_round_wgmma<1>); smem = row_tiles_smem<1>(); break;
-      case 2: kern = reinterpret_cast<const void*>(mmr_round_wgmma<2>); smem = row_tiles_smem<2>(); break;
-      default: return set_error(h, B200MS_ESTATE, "mmr: corpus dtype has no scorer");
-    }
-    if (int e = ensure_smem(h, kern, smem, "cudaFuncSetAttribute(mmr_round_wgmma)")) return e;
-    void* args[] = {const_cast<MmrArgs*>(&a)};
-    if (int e = check_cuda(h, cudaLaunchKernel(kern, grid, dim3(kRowTileThreads), args, size_t(smem), s), "launch mmr_round"))
-      return e;
-  }
-  h->launches++;
-  return check_cuda(h, cudaGetLastError(), "launch mmr_round");
+  RowTileKernel<MmrArgs> k;
+  if (int e = row_tile_kernel(h, dtype, mmr_round_wgmma<0>, mmr_round_wgmma<1>, mmr_round_wgmma<2>, mmr_round_b1,
+                              kRowBlockB1Threads, "mmr_round", &k))
+    return e;
+  return launch_row_tiles(h, k, grid, a, s, "launch mmr_round");
 }
 
 static int launch_pick(b200ms_t* h, const MmrArgs& a, int dtype, int i, int choose_next, cudaStream_t s) {

@@ -202,26 +202,19 @@ int launch_hamming_batch(b200ms_t* h, const void* q, const void* cand, int64_t n
   return check_cuda(h, cudaGetLastError(), "launch hamming_batch");
 }
 
-static int grid_for(b200ms_t* h, int64_t warps) {
-  int64_t blocks = (warps + 7) / 8;
-  const int64_t cap = int64_t(h->num_sms) * 16;
-  if (blocks > cap) blocks = cap;
-  return blocks < 1 ? 1 : int(blocks);
-}
-
 int launch_pack_rows(b200ms_t* h, const void* src, int src_dtype, const int64_t* src_start_dev,
                      const int64_t* dst_start_dev, int64_t n_items, int64_t dst_rows, int pad_mode, void* dst,
                      int dst_dtype, float i8_scale, cudaStream_t s) {
   if (dst_rows <= 0) return B200MS_OK;
-  pack_rows_kernel<<<grid_for(h, dst_rows), 256, 0, s>>>(src, src_dtype, src_start_dev, dst_start_dev, n_items, dst_rows,
-                                                        pad_mode, dst, dst_dtype, i8_scale);
+  pack_rows_kernel<<<grid_stride_blocks(h, dst_rows, 8, 16), 256, 0, s>>>(
+      src, src_dtype, src_start_dev, dst_start_dev, n_items, dst_rows, pad_mode, dst, dst_dtype, i8_scale);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch pack_rows");
 }
 
 int launch_chunk_page(b200ms_t* h, const int64_t* page_start_dev, int64_t n_pages, int32_t* chunk_page, cudaStream_t s) {
   if (n_pages <= 0) return B200MS_OK;
-  chunk_page_kernel<<<grid_for(h, n_pages), 256, 0, s>>>(page_start_dev, n_pages, chunk_page);
+  chunk_page_kernel<<<grid_stride_blocks(h, n_pages, 8, 16), 256, 0, s>>>(page_start_dev, n_pages, chunk_page);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch chunk_page");
 }

@@ -105,17 +105,11 @@ union_candidates_kernel(const int64_t* __restrict__ cand, int n_cand, const int3
   for (int64_t j = (count < width ? count : width) + tid; j < width; j += kUnionThreads) out[int64_t(r) * width + j] = -1;
 }
 
-static int grid_of(b200ms_t* h, int64_t threads) {
-  int64_t b = (threads + 255) / 256;
-  const int64_t cap = int64_t(h->num_sms) * 16;
-  return int(b < 1 ? 1 : b > cap ? cap : b);
-}
-
 template <typename T>
 int launch_gather_rows(b200ms_t* h, const T* src, int64_t row_len, const int32_t* idx, int n_rows, T* dst, cudaStream_t s) {
   const int64_t total = row_len * n_rows;
   if (total <= 0) return B200MS_OK;
-  gather_rows_kernel<T><<<grid_of(h, total), 256, 0, s>>>(src, row_len, idx, total, dst);
+  gather_rows_kernel<T><<<grid_stride_blocks(h, total, 256, 16), 256, 0, s>>>(src, row_len, idx, total, dst);
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch gather_rows");
 }

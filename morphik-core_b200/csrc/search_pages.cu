@@ -113,18 +113,12 @@ __global__ void normalise_pages_kernel(const int64_t* __restrict__ src, const in
   if (threadIdx.x == 0 && len <= 0) counts[q] = 0;
 }
 
-static int blocks_for(b200ms_t* h, int64_t threads) {
-  int64_t b = (threads + 255) / 256;
-  const int64_t cap = int64_t(h->num_sms) * 16;
-  return int(b < 1 ? 1 : b > cap ? cap : b);
-}
-
 int launch_pack_src_pages(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev, const int64_t* ds_dev, int64_t n_src,
                           int64_t row0, int64_t dst_rows, void* dst, cudaStream_t s) {
   if (dst_rows <= row0) return B200MS_OK;
   const Corpus& c = h->corpus;
   const int64_t ppr = b200ms_row_bytes(c.dtype) / 16;
-  pack_src_pages_kernel<<<blocks_for(h, (dst_rows - row0) * ppr), 256, 0, s>>>(
+  pack_src_pages_kernel<<<grid_stride_blocks(h, (dst_rows - row0) * ppr, 256, 16), 256, 0, s>>>(
       static_cast<const uint4*>(c.rows), ppr, static_cast<const int64_t*>(h->page_start.p), src_dev, ss_dev, ds_dev, n_src,
       dst_rows, static_cast<uint4*>(dst));
   h->launches++;
@@ -135,8 +129,9 @@ int launch_page_rows(b200ms_t* h, const int64_t* src_dev, const int64_t* ss_dev,
                      float* out, cudaStream_t s) {
   if (n_rows <= 0) return B200MS_OK;
   const Corpus& c = h->corpus;
-  page_rows_kernel<<<blocks_for(h, n_rows * 32), 256, 0, s>>>(c.rows, c.dtype, static_cast<const int64_t*>(h->page_start.p),
-                                                             src_dev, ss_dev, n_src, scale, reinterpret_cast<float4*>(out));
+  page_rows_kernel<<<grid_stride_blocks(h, n_rows * 32, 256, 16), 256, 0, s>>>(
+      c.rows, c.dtype, static_cast<const int64_t*>(h->page_start.p), src_dev, ss_dev, n_src, scale,
+      reinterpret_cast<float4*>(out));
   h->launches++;
   return check_cuda(h, cudaGetLastError(), "launch page_rows");
 }
